@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- images/s of the Salience-DETR encoder forward (salience filter + 6 encoder layers) on B200.
+"""bench.py -- images/s of the Salience-DETR encoder forward (salience filter + 6 encoder layers) on H100.
 
 Workload (BASELINE.json configs[1]): salience_detr_resnet50_800_1333, bs=2 per GPU, synthetic COCO-shape inputs
 (800x1333 padded to 800x1344 -> levels 100x168, 50x84, 25x42, 13x21; Nv=22323, K=11363), fp32, eval, random-init
 weights.  A "step" is one encoder-half forward (salience_transformer.py:106-183 of the reference) over one batch.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's sm_100a path
+  python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's sm_90a path
+  python bench.py ... --dump-outputs DIR                          # also write the last timed step's memory as DIR/memory.npy
   python bench.py --impl reference ...                           # the reference's CPU path (oracle port), rank 0 only
   torchrun --nproc-per-node N bench.py --gpus N ...              # one process per GPU, weak scaling (replicas)
 
@@ -61,11 +62,11 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -255,9 +256,8 @@ def time_gemm_kernels(pkg, runner, reps=10):
 
 def use_host_cores():
     """The CPU arm uses every PHYSICAL core this process may run on (torchrun pins OMP_NUM_THREADS=1 by default).  One
-    thread per logical CPU was measured on the pool's 64-core / 128-thread hosts: 0.045 images/s at 128 threads against
-    0.56 at 64 (gpurun_out/r2_bench_a.json vs BENCH_r01.json) -- SMT siblings fight over the FMA units -- so the faster,
-    fairer setting is used and its thread count reported as `cores`."""
+    thread per logical CPU is slower on SMT hosts -- siblings fight over the FMA units -- so the faster, fairer setting is
+    used and its thread count reported as `cores`."""
     n = os.cpu_count() or 1
     try:
         n = len(os.sched_getaffinity(0))
@@ -322,7 +322,7 @@ def model_cfg(model):
 def reference_step_fn(model, device="cpu"):
     """One encoder-half forward (salience_transformer.py:106-183) of the REFERENCE on `device`, same weights as `model`.
     -> (step(feats, masks, pos) -> memory, kind, description).  kind "reference": the unmodified reference modules
-    installed under baseline/_ref (oracle/ref_import.py; on a GPU its pure-PyTorch grid_sample MSDA runs, because its
+    from the checkout named by SDETR_REFERENCE_ROOT (oracle/ref_import.py; on a GPU its pure-PyTorch grid_sample MSDA runs, because its
     CUDA extension does not build against this torch); kind "port": the oracle's torch restatement (fallback when the
     install is absent)."""
     from oracle import ref_import  # reference arm / cpu_baseline / gpu_comparator legs only
@@ -339,7 +339,7 @@ def reference_step_fn(model, device="cpu"):
         assert not res.unexpected_keys, res.unexpected_keys  # our parameter names ARE the reference's
         tr = tr.to(device).eval()
         return (lambda f, mk, p: ref_import.run_encoder_half(tr, f, mk, p)[0], "reference",
-                "unmodified reference modules (baseline/_ref: models/bricks/salience_transformer.py:106-183 with the "
+                "unmodified reference modules (SDETR_REFERENCE_ROOT: models/bricks/salience_transformer.py:106-183 with the "
                 "pure-PyTorch grid_sample MSDA, ms_deform_attn.py:159-212), same weights and inputs")
     from oracle import oracle as orc
     sd = {k: v.detach().cpu() for k, v in model.state_dict().items()}
@@ -348,7 +348,7 @@ def reference_step_fn(model, device="cpu"):
         with torch.no_grad():
             return orc.encoder_half_forward(sd, f, mk, p, cfg, core="torch")[0]
 
-    return port, "port", "oracle port of the reference PyTorch CPU path (baseline/_ref not installed)"
+    return port, "port", "oracle port of the reference PyTorch CPU path (SDETR_REFERENCE_ROOT not set)"
 
 
 def cpu_baseline(pkg, model, budget_s=20.0):
@@ -370,11 +370,11 @@ def cpu_baseline(pkg, model, budget_s=20.0):
 
 
 def gpu_comparator(model, feats, masks, pos, steps=10, warmup=3):
-    """What the reference really executes on this image ON THE B200: its own modules (pure-PyTorch MSDA, ~40 host syncs
+    """What the reference really executes on this image ON THE GPU: its own modules (pure-PyTorch MSDA, ~40 host syncs
     and ~1000 launches per forward), same weights / inputs, CUDA-event timed like tools/benchmark_model.py:44-61."""
     step, kind, desc = reference_step_fn(model, feats[0].device)
     if kind != "reference":
-        return {"unavailable": "baseline/_ref not installed"}
+        return {"unavailable": "SDETR_REFERENCE_ROOT not set"}
     prev = torch.backends.cuda.matmul.allow_tf32
     torch.backends.cuda.matmul.allow_tf32 = False  # fp32 like the reference's default
     try:
@@ -560,6 +560,8 @@ def main():
     ap.add_argument("--e2e-persistent-ctas", type=int, default=0,
                     help="cap of the persistent GEMM / FFN kernels during the e2e (multi-lane) measurement; 0 = one CTA per SM")
     ap.add_argument("--pipeline-depth", type=int, default=4, help="lanes of the host-buffer pipeline (e2e)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (the encoder memory, float32) as DIR/memory.npy")
     args = ap.parse_args()
     _claim_stdout()
     rank = int(os.environ.get("RANK", "0"))
@@ -577,7 +579,7 @@ def main():
     args.warmup = max(3, args.warmup if args.warmup is not None else 10)
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a GPU: the sm_100a path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs a GPU: the sm_90a path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     import torch.distributed as dist
@@ -635,6 +637,7 @@ def main():
         clk.wait_first()
         total_ms = timed(runner.step, args.steps, args.warmup, on_start=clk.mark)
         clk.mark_end()
+        last_memory = runner.memory.detach().float().cpu() if args.dump_outputs else None
         t_probe = time.time()
         while clk.proc is not None and clk.since_mark() < 3 and time.time() - t_probe < 3.0:  # same step, same flush, untimed
             with torch.cuda.stream(stream):
@@ -648,10 +651,10 @@ def main():
     # end to end through the public host-buffer API (the detector-side boundary, salience_detr.py:172-203: feature maps and
     # padding masks in, memory out; the sine position embedding is a function of the masks and is derived on the device).
     # Every step copies its feature maps from pinned host memory and its result back.  serial = one stream; pipelined =
-    # HostPipeline, double-buffered, copies overlap compute.  e2e is timed over >= 200 steps (round 1: 20 steps = 60 ms
-    # was too short to be stable across boxes).
+    # HostPipeline, double-buffered, copies overlap compute.  Every timed leg runs --steps steps: pass enough of them for a
+    # stable e2e figure (a window of a few tens of milliseconds is not).
     from salience_detr_b200.runner import HostPipeline
-    e2e_steps = max(args.steps, 200)
+    e2e_steps = args.steps
     host_runner = EncoderRunner(model, feats, masks, None, use_graph=not args.no_graph, use_order=not args.no_order)
     host_runner.bind_host(feats_h)
     stream_keep, stream = stream, host_runner.stream
@@ -688,8 +691,8 @@ def main():
         out_pin.copy_(mem, non_blocking=True)
 
     stream_keep, stream = stream, torch.cuda.current_stream(dev)
-    fresh_ms = timed(fresh_step, max(10, args.steps // 2), 3)
-    fresh_serial_val = sdist.aggregate_throughput(bsz, max(10, args.steps // 2), world, fresh_ms)
+    fresh_ms = timed(fresh_step, args.steps, 3)
+    fresh_serial_val = sdist.aggregate_throughput(bsz, args.steps, world, fresh_ms)
     stream = stream_keep
     # the same, pipelined: copies, plan (own stream) and eager forwards of consecutive batches overlap; every batch still pays
     # its own plan and an eager forward
@@ -698,7 +701,7 @@ def main():
     fresh_batch = (feats_pin, masks_pin)
     fpipe.run([fresh_batch] * 6)
     barrier()
-    fresh_steps = max(args.steps, 100)
+    fresh_steps = args.steps
     t0 = torch.cuda.Event(enable_timing=True)
     t1 = torch.cuda.Event(enable_timing=True)
     t0.record()
@@ -732,8 +735,8 @@ def main():
             tf32_peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"] / (1.0 if f16 else 2.0)
             gemm_peak_src = "MEASURED_PEAKS.json bf16_tflops" + ("" if f16 else " / 2 (TF32 dense = half the bf16 rate)")
         except Exception:
-            tf32_peak = 1590.0 / (1.0 if f16 else 2.0)  # B200_PROFILING.md fallback
-            gemm_peak_src = "fallback (B200_PROFILING.md)"
+            tf32_peak = 989.0 / (1.0 if f16 else 2.0)  # dense FP16 / TF32 of the H100 SXM data sheet (700 W)
+            gemm_peak_src = "H100 SXM data sheet, dense " + ("FP16" if f16 else "TF32")
         passes = 1 if pkg.gemm.MODE in ("fp32", "tf32") else 3
         gemm_exec = passes * gemm_flops / (gemm_ms / 1000.0) / 1e12
         line = {
@@ -744,13 +747,13 @@ def main():
                        "parallelism": f"dp{world} (independent replicas, no forward collective)",
                        "weights": "random init (seed 0) + N(0,0.02) sampling-offset weights",
                        "gemm": {"auto": ("3xFP16 (fp32-class accuracy, 22-bit operands: hi/lo fp16 split with exact power-of-two range scaling): "
-                                         "hand-written persistent tcgen05.mma.kind::f16 GEMM" if pkg.gemm.OWN_KERNEL == "f16x3" else
-                                         "3xTF32 (fp32-class accuracy): hand-written persistent tcgen05.mma.kind::tf32 GEMM") +
-                                        " (TMA, pre-split weight, activation split in the kernel into tensor memory, double-buffered TMEM "
-                                        "accumulator, TMA-store epilogue) for every projection; linear1 -> ReLU -> linear2 -> +residual -> LayerNorm of the encoder "
-                                        "layers as ONE tensor-core kernel with the hidden activations in tensor memory; GEMMs of <= 2304 rows "
+                                         "hand-written persistent wgmma .f16 GEMM" if pkg.gemm.OWN_KERNEL == "f16x3" else
+                                         "3xTF32 (fp32-class accuracy): hand-written persistent wgmma .tf32 GEMM") +
+                                        " (TMA producer warpgroup, pre-split weight, activation split in registers as the wgmma A operand, "
+                                        "register accumulators) for every projection; linear1 -> ReLU -> linear2 -> +residual -> LayerNorm of the encoder "
+                                        "layers as two such GEMMs and a row kernel; GEMMs of <= 2304 rows "
                                         "(latency-bound) on cuBLAS fp32 or the two-launch small-level predictor kernels",
-                                "tcgen05": "hand-written tcgen05.mma.kind::tf32 GEMM (TMA, in-kernel 3xTF32 split, TMEM accumulator; fp32-class accuracy)",
+                                "tcgen05": "hand-written wgmma .tf32 GEMM (TMA, in-kernel 3xTF32 split, register accumulator; fp32-class accuracy)",
                                 "3xtf32": "cuBLAS TF32 tensor cores on 3-way split operands (3xTF32, fp32-class accuracy)",
                                 "fp32": "cuBLAS fp32 SIMT", "tf32": "cuBLAS TF32 (reduced precision)"}[pkg.gemm.MODE], "cuda_graph": runner.graph is not None,
                        "msda_order": "spatial tiles" if runner.use_order else "score order",
@@ -771,8 +774,7 @@ def main():
                     "numa": numa},
             "gpu_launches": runner.launches_per_step * args.steps,
             "gpu_launches_per_step": runner.launches_per_step,
-            "roofline": {"bound": "hbm (SURVEY.md 8(d) denominator; measured: the gather is bound by the L1 tag stage, ~2 clk per "
-                                  "128-byte line, DESIGN.md 3.1)",
+            "roofline": {"bound": "hbm (SURVEY.md 8(d) denominator)",
                          "kernel": "sdetr::msda_fwd_kernel<32,4,4,fused> (6 launches/step)",
                          "achieved": round(achieved, 1), "peak": peak, "peak_source": peak_src, "unit": "GB/s",
                          "frac": round(achieved / peak, 4), "traffic": traffic,
@@ -783,9 +785,9 @@ def main():
                                            "per_layer_us": [round(1000 * x, 1) for x in cold],
                                            "how": "the same six launches replayed alone after an L2 flush (round-1 definition)"}},
             # secondary leg: the dense projections (tensor-bound; 3xTF32 issues 3 TF32 MMA passes per logical product)
-            "roofline_gemm": {"bound": "tensor (measured: the kernel is bound by L2<->SM operand/result traffic, DESIGN.md 3.4)",
-                              "kernels": ("sdetr::gemm_f16x3_kernel + sdetr::ffn_fused_kernel (3xFP16, tcgen05.mma.kind::f16; the FFN keeps its hidden activations in tensor memory)" if f16 else
-                                          "sdetr::gemm_3xtf32_p_kernel<presplit>") + " (+ cuBLAS fp32 for <= 2304-row GEMMs)",
+            "roofline_gemm": {"bound": "tensor",
+                              "kernels": ("sdetr::gemm3x_kernel<true, false> (3xFP16, wgmma .f16)" if f16 else
+                                          "sdetr::gemm3x_kernel<false, false> (3xTF32, wgmma .tf32)") + " (+ cuBLAS fp32 for <= 2304-row GEMMs)",
                               "achieved": round(gemm_exec, 1), "peak": round(tf32_peak, 1), "peak_source": gemm_peak_src,
                               "unit": "TFLOP/s", "frac": round(gemm_exec / tf32_peak, 4),
                               "logical_tflops": round(gemm_flops / (gemm_ms / 1000.0) / 1e12, 1),
@@ -796,6 +798,10 @@ def main():
             line["gpu_comparator"] = gpu_comparator(model, feats, masks, pos)
             line["cpu_baseline"] = cpu_baseline(pkg, model)
         emit(json.dumps(line))
+        if args.dump_outputs:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "memory.npy"), last_memory.numpy())
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()

@@ -1,12 +1,12 @@
 /*
- * sdetr_b200.h -- C-ABI of the B200-native (sm_100a) Salience-DETR encoder hot path.
+ * sdetr_b200.h -- C-ABI of the H100-native (sm_90a) Salience-DETR encoder hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  All pointers are DEVICE
  * pointers unless the parameter name ends in `_host`.  Every call is asynchronous on `stream`
  * (a cudaStream_t passed as void*) of the CURRENT device, allocates nothing, never synchronises, and is
  * re-entrant across streams, threads and devices (per-device kernel attributes are set on first use per device).
- * The only process-global state are the benchmarking knobs sdetr_set_option / sdetr_gemm_set_variant /
- * sdetr_gemm_set_trace (atomics: a call reads them once at launch).  Return value: 0 on success, negative sdetr_status on error (message: sdetr_last_error(),
+ * The only process-global state are the knobs sdetr_set_option / sdetr_set_persistent_ctas (atomics: a call reads them once
+ * at launch).  Return value: 0 on success, negative sdetr_status on error (message: sdetr_last_error(),
  * thread-local).  Launch errors are RETURNED (the reference only printf's them:
  * models/bricks/ops/cuda/ms_deform_im2col_cuda.cuh:937-941, 1310-1314).
  *
@@ -38,7 +38,7 @@ int sdetr_version(void);
 const char *sdetr_last_error(void);
 /* number of kernels this library has launched in the calling process (bench.py "gpu_launches") */
 unsigned long long sdetr_launch_count(void);
-/* The persistent tensor-core kernels (sdetr_gemm_f16x3_pre, sdetr_ffn_fused_layernorm) launch one CTA per SM and leave no room
+/* The persistent tensor-core kernels (the sdetr_gemm_* entry points, sdetr_ffn_fused_layernorm) launch one CTA per SM and leave no room
  * for anything else on it; n > 0 caps them at n CTAs so that concurrently running streams (other lanes of a pipeline) find free
  * SMs for their small kernels.  0 (default) = every SM.  Process-wide. */
 int sdetr_set_persistent_ctas(int n);
@@ -325,37 +325,30 @@ int sdetr_rows_scatter(float *dst, const int64_t *index, int batch, int num_rows
 int sdetr_split_tf32(const float *x, int64_t x_row_stride, int64_t rows, int K, int chunk, int layout_b, int relu,
                      float *out, sdetr_stream_t stream);
 
-/* Dense projection on the tcgen05 tensor cores with fp32-class accuracy (hand-written sm_100a GEMM):
+/* Dense projection on the tensor cores with fp32-class accuracy (hand-written sm_90a wgmma GEMM):
  *   C[M,N] = act(A)[M,K] . W[N,K]^T + bias,  act = ReLU (relu_a = 1, salience_transformer.py:348), exact GELU (relu_a = 2, :23-29) or identity (0).
  * A (M,K) row pitch lda floats; W_hi/W_lo (N,K) contiguous = sdetr_split_tf32_pair(W); bias (N) nullable;
  * C (M,N) row pitch ldc.  K % 32 == 0; A/W 16-byte aligned, lda % 4 == 0.  The activation is split into TF32 pieces
- * inside the kernel (no extra HBM pass); products A_hi.W_hi + A_hi.W_lo + A_lo.W_hi accumulate in TMEM (fp32).
+ * inside the kernel (no extra HBM pass); products A_hi.W_hi + A_hi.W_lo + A_lo.W_hi accumulate in fp32 registers.
  * Replaces the cuBLAS path for: value_proj / sampling_offsets|attention_weights / output_proj
  * (models/bricks/ms_deform_attn.py:316,322-328,375), FFN (salience_transformer.py:347-351), class head (:462),
  * MaskPredictor (:16-47), enc_output (base_transformer.py:111). */
 /* Same contract with the RAW weight W (N,K): the kernel splits both operands itself (32 KB instead of 48 KB of TMA
- * traffic per k-block), keeps the split activation in tensor memory, and runs two CTAs per SM. */
+ * traffic per k-block), with the arithmetic of sdetr_split_tf32_pair: results are bit-identical to the pre-split form. */
 int sdetr_gemm_3xtf32_raw(const float *A, int64_t lda, const float *W, const float *bias, float *C, int64_t ldc, int M,
                           int N, int K, int act, sdetr_stream_t stream);
-/* kernel variants: sdetr_gemm_3xtf32: 0 = "SS" (both operands from shared memory), 1 = "TS" (the split activation is
- * written to tensor memory by the converter warps and the MMAs read A from TMEM); sdetr_gemm_3xtf32_raw: 2 = "TS2"
- * (one tile per CTA, two CTAs per SM), 3 = "P" (default: persistent tile loop, double-buffered TMEM accumulator,
- * dedicated epilogue warps) */
-int sdetr_gemm_set_variant(int variant);
-/* debugging aid: when set, CTA (0,0) of every sdetr_gemm_3xtf32 launch records clock64() per pipeline event */
-int sdetr_gemm_set_trace(long long *device_buffer);
 int sdetr_split_tf32_pair(const float *w, int64_t count, float *w_hi, float *w_lo, sdetr_stream_t stream);
 int sdetr_gemm_3xtf32(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, float *C,
                       int64_t ldc, int M, int N, int K, int relu_a, sdetr_stream_t stream);
-/* Same contract as sdetr_gemm_3xtf32 (pre-split weight), on the persistent kernel: one CTA per SM walks the output
- * tiles, the weight halves arrive as two TMA tiles per stage and only the activation is converted in the kernel. */
+/* Same contract and kernel as sdetr_gemm_3xtf32 (pre-split weight): one CTA per SM walks the output tiles, the weight
+ * halves arrive as two TMA tiles per stage and only the activation is converted in the kernel. */
 int sdetr_gemm_3xtf32_pre(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, float *C,
                           int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream);
 
-/* ---- "3xFP16": the same error-compensated product on tcgen05.mma.kind::f16 -----------------------------------------
+/* ---- "3xFP16": the same error-compensated product on wgmma .f16 ---------------------------------------------------------
  * An fp16 significand is as wide as a TF32 one (11 bits), so  A_hi.W_hi + A_hi.W_lo + A_lo.W_hi  with
  * hi = fp16(x), lo = fp16(x - hi) keeps the 22 significand bits per operand of 3xTF32 at twice the MMA rate and half the
- * operand bytes.  Exponent range is restored by exact power-of-two scalings: the kernel multiplies the activation by 16
+ * weight bytes.  Exponent range is restored by exact power-of-two scalings: the kernel multiplies the activation by 16
  * before the split (full accuracy for 2^-7 <= |x| < 4094, absolute error floor 2^-29 below, inf/NaN above), the caller
  * scales the weight by `scale` = 2^s with max|scale * W| in [2^13, 2^14) when splitting, and the epilogue multiplies the
  * fp32 accumulator by 2^-(4+s) before the bias.  Replaces the same reference projections as sdetr_gemm_3xtf32
@@ -378,21 +371,6 @@ int sdetr_split_f16_pair_dev(const float *W, int64_t count, const float *scale_d
 /* *scale = 2^s with max|x| * 2^s in [2^(target_log2 - 1), 2^target_log2) (1 for an all-zero x); one launch, deterministic.
  * state: 8 bytes of device memory, zero before the first call (the kernel leaves them zero). */
 int sdetr_pow2_scale(const float *x, int64_t count, int target_log2, void *state, float *scale, sdetr_stream_t stream);
-/* benchmarking knob: 0 (default) = always the streaming kernel, 1 = K <= 256 and >= 2 output tiles per work unit use the
- * activation-stationary kernel (the split activation panel stays in tensor memory across the unit's output tiles) */
-int sdetr_gemm_f16x3_set_as(int enable);
-/* benchmarking knob, streaming kernel epilogue: 0 (default) = two shared 16 KB boxes + TMA bulk stores, 1 = warp-private
- * transpose boxes + coalesced 128-bit global stores (no CTA-level barrier in the epilogue) */
-int sdetr_gemm_f16x3_set_epilogue(int variant);
-/* benchmarking knob, streaming kernel: 4 (default) or 8 epilogue warps (8: two groups of four, each draining half of a tile's
- * columns through its own store box) */
-int sdetr_gemm_f16x3_set_epilogue_warps(int warps);
-/* debugging aid: when set, CTA 0 of every streaming sdetr_gemm_f16x3_pre launch records clock64() per pipeline event
- * (device_buffer: 10 x 256 int64) */
-int sdetr_gemm_f16x3_set_trace(long long *device_buffer);
-/* benchmarking knob: 1 = clusters of two CTAs (adjacent 128-row panels, same output columns) share the weight k-blocks by
- * TMA multicast (measured slower, off by default); 0 (default) = independent CTAs */
-int sdetr_gemm_f16x3_set_cluster(int enable);
 
 /* ---- MaskPredictor of one small feature level in two launches ---------------------------------------------------------------
  * Replaces, for a level of few token rows, score modulation + MaskPredictor (models/bricks/salience_transformer.py:16-47, :134-143):
@@ -411,32 +389,21 @@ int sdetr_mask_predictor_level(const float *mem, int64_t mem_batch_stride, int b
                                const float *w2c, const float *b2c, float *workspace, int64_t workspace_floats, float *out,
                                int64_t out_batch_stride, sdetr_stream_t stream);
 
-/* ---- fused encoder FFN: y = LayerNorm(x + linear2(ReLU(linear1(x)))) ------------------------------------------------------
+/* ---- encoder FFN: y = LayerNorm(x + linear2(ReLU(linear1(x)))) ------------------------------------------------------------
  * Replaces `forward_ffn` + `norm2` of the encoder layer (models/bricks/salience_transformer.py:347-351, :391) for embed_dim 256:
- * one persistent tcgen05 kernel keeps a 128-row panel on chip from x to the output accumulator (the hidden activations never
- * reach HBM; only the weights stream), then a row kernel adds the partial sums, b2 and the residual and normalises.
+ * linear1 and linear2 (the ReLU fused into its operand load) on the 3xFP16 kernel, then a row kernel adds the residual and
+ * normalises.
  * Same 3xFP16 arithmetic and value domain as sdetr_gemm_f16x3_pre (both weights given as sdetr_split_f16_pair pairs with
  * their scales; W1 (hidden,256), W2 (256,hidden); hidden % 128 == 0).
  * x (M,256) fp32 with row pitch ldx (floats); y (M,256) contiguous, may alias x when ldx == 256;
  * gamma == beta == NULL: y = linear2(ReLU(linear1(x))) without residual / LayerNorm.
- * workspace: sdetr_ffn_fused_workspace_floats(M, hidden) floats (partial sums of panels shared by two CTAs: the persistent
- * CTAs take equal numbers of 128-hidden-unit chunks of the (panel, chunk) sequence, whatever the panel count). */
+ * workspace: sdetr_ffn_fused_workspace_floats(M, hidden) = M * (hidden + 256) floats (the hidden activations and linear2's
+ * output). */
 int64_t sdetr_ffn_fused_workspace_floats(int M, int hidden);
-/* host-side view of the work decomposition (for tests): lo[i] = first item of CTA i in the panel-major (panel, chunk) sequence,
- * lo[G] = #panels * hidden / 128; returns the CTA count G (or -G when `capacity` < G + 1, 0 for bad sizes) */
-int sdetr_ffn_fused_ranges(int M, int hidden, int64_t *lo, int capacity);
 int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *W1_hi, const void *W1_lo, float w1_scale, const float *b1,
                               const void *W2_hi, const void *W2_lo, float w2_scale, const float *b2, const float *gamma,
                               const float *beta, float eps, int M, int hidden, float *workspace, int64_t workspace_floats, float *y,
                               sdetr_stream_t stream);
-/* benchmarking knob: 1 (default) = equal chunk counts per CTA, 0 = whole panels per CTA (idle SMs when the panel count is not
- * near a multiple of the SM count).  Changes the workspace size: query it after setting. */
-int sdetr_ffn_fused_set_balance(int enable);
-/* debugging aid: CTA 0 of every sdetr_ffn_fused_layernorm launch records clock64() per pipeline event (8 x 256 int64) */
-int sdetr_ffn_fused_set_trace(long long *device_buffer);
-/* debugging / benchmarking knob: at most n persistent CTAs (0 = one per SM) */
-int sdetr_ffn_fused_set_max_ctas(int n);
-
 #ifdef __cplusplus
 }
 #endif

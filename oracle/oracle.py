@@ -481,3 +481,47 @@ def deterministic_state_dict(shapes: Dict[str, Sequence[int]], seed: int) -> Dic
             x = x / (shp[-1] ** 0.5)
         out[name] = x
     return out
+
+
+# ---- seeded inputs of the drop-in / decoder-half tests (shared by oracle/make_golden.py and the tests) -------------------------
+def dropin_msda_op_inputs():
+    """query, reference points, value, shapes, level starts, padding mask, output gradient of the MSDA operator test"""
+    shapes = torch.tensor([(30, 40), (15, 20), (8, 10), (4, 5)])
+    lsi = torch.cat([shapes.new_zeros(1), shapes.prod(1).cumsum(0)[:-1]])
+    nv, b, nq = int(shapes.prod(1).sum()), 2, 333
+    g = torch.Generator().manual_seed(1)
+    query = torch.randn(b, nq, 256, generator=g)
+    refp = torch.rand(b, nq, 4, 2, generator=g)
+    value = torch.randn(b, nv, 256, generator=g)
+    mask = torch.rand(b, nv, generator=g) < 0.1
+    gout = torch.randn(b, nq, 256, generator=g)
+    return query, refp, value, shapes, lsi, mask, gout
+
+
+def seeded_memory(shape, seed):
+    """stand-in encoder memory for the decoder test: N(0, 1) like a LayerNorm output"""
+    return torch.randn(tuple(shape), generator=torch.Generator().manual_seed(seed))
+
+
+def denoising_queries(b, nq, embed_dim, n=20, seed=4):
+    """n denoising queries + boxes ahead of nq matching queries, and the attention mask that hides them from the matching
+    queries (salience_transformer.py:218-221)"""
+    g = torch.Generator().manual_seed(seed)
+    dn_q = torch.randn(b, n, embed_dim, generator=g)
+    dn_b = torch.rand(b, n, 4, generator=g) * 0.5 + 0.25
+    mask = torch.zeros(nq + n, nq + n, dtype=torch.bool)
+    mask[n:, :n] = True
+    return dn_q, dn_b, mask
+
+
+class ConvNeck(torch.nn.Module):
+    """Stand-in for a convolutional neck between encoder and decoder (the dict-of-levels interface of the reference's necks,
+    salience_transformer.py:185-192): per level a 3x3 convolution + SiLU, weights from manual_seed(seed)."""
+
+    def __init__(self, channels, levels, seed):
+        super().__init__()
+        torch.manual_seed(seed)
+        self.convs = torch.nn.ModuleList(torch.nn.Conv2d(channels, channels, 3, padding=1) for _ in range(levels))
+
+    def forward(self, maps):
+        return {k: torch.nn.functional.silu(self.convs[k](v)) for k, v in maps.items()}

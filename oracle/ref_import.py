@@ -1,9 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- loader for the *unmodified* reference (xiuqhou/Salience-DETR).
 
-Used in the build container to (a) generate the golden fixtures under ``tests/golden/`` and
-(b) validate the oracle restatements in ``oracle/`` against the reference itself.  The
-reference tree (``/root/reference``) does not travel to the GPU box, so nothing on a product,
-bench or ``-m gpu`` path may import this module; callers must check :func:`available` first.
+Used to (a) generate the golden fixtures under ``tests/golden/`` and (b) run bench.py's reference arm against the original
+project itself, when a checkout of it is named by ``SDETR_REFERENCE_ROOT``.
+Nothing on a product path imports this module; callers must check :func:`available` first.
 
 The only accommodation made is a stub for ``util.misc`` (its real module imports ``accelerate``,
 which is not installed): ``models/bricks/salience_transformer.py:13`` needs only
@@ -16,63 +15,17 @@ import sys
 import types
 import warnings
 
-_REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BASELINE_REF = os.path.join(_REPO, "baseline", "_ref")  # git-ignored install of the reference's hot-path modules
-# the Python modules of the path (SURVEY.md 8(c)); everything else of the reference stays where it is
-PATH_MODULES = ("base_transformer.py", "basic.py", "ms_deform_attn.py", "position_encoding.py", "salience_transformer.py")
-# consumer right after the path (SURVEY.md 8(f)-3): the RepVGG neck the encoder memory is handed to, for the hand-off test
-NECK_MODULES = (("models/necks", "repnet.py"), ("models/bricks", "misc.py"))
 
 
 def _has(root: str) -> bool:
-    return os.path.isfile(os.path.join(root, "models", "bricks", "salience_transformer.py"))
+    return bool(root) and os.path.isfile(os.path.join(root, "models", "bricks", "salience_transformer.py"))
 
 
-def _resolve_root() -> str:
-    env = os.environ.get("SDETR_REFERENCE_ROOT")
-    if env:
-        return env
-    for root in ("/root/reference", BASELINE_REF):  # the tree itself in the build container, the install on the GPU box
-        if _has(root):
-            return root
-    return "/root/reference"
-
-
-REFERENCE_ROOT = _resolve_root()
+REFERENCE_ROOT = os.environ.get("SDETR_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
     return _has(REFERENCE_ROOT)
-
-
-def install(src: str = "/root/reference", dst: str = BASELINE_REF) -> bool:
-    """Install the UNMODIFIED Python modules of the path from the reference tree into the git-ignored
-    ``baseline/_ref`` (which travels to the GPU box; /root/reference does not).  The reference has no setup.py /
-    pyproject, so `pip install --target` does not apply: this copies the five files byte for byte.  The CUDA
-    extension sources (models/bricks/ops/cuda) are NOT installed: they do not compile against torch 2.11 (SURVEY.md
-    fact 2), so the reference's own `load(...)` fails, warns and falls back to its pure-PyTorch MSDA
-    (ms_deform_attn.py:13-26,361-372) -- which is the path the reference really runs on this image."""
-    import filecmp
-    import shutil
-
-    if not _has(src):
-        return _has(dst)
-    out = os.path.join(dst, "models", "bricks")
-    os.makedirs(out, exist_ok=True)
-    for name in PATH_MODULES:
-        a, b = os.path.join(src, "models", "bricks", name), os.path.join(out, name)
-        if not (os.path.exists(b) and filecmp.cmp(a, b, shallow=False)):
-            shutil.copyfile(a, b)
-    for sub, name in NECK_MODULES:
-        a, b = os.path.join(src, sub, name), os.path.join(dst, sub, name)
-        os.makedirs(os.path.dirname(b), exist_ok=True)
-        if os.path.exists(a) and not (os.path.exists(b) and filecmp.cmp(a, b, shallow=False)):
-            shutil.copyfile(a, b)
-    with open(os.path.join(dst, "README"), "w") as f:
-        f.write("Unmodified copies of xiuqhou/Salience-DETR models/bricks/{%s} (reference arm of bench.py and the\n"
-                "drop-in tests; written by oracle/ref_import.install(), git-ignored, never imported by the product).\n"
-                % ",".join(PATH_MODULES))
-    return True
 
 
 def _install_stub():
@@ -97,7 +50,7 @@ def _install_stub():
 def load():
     """Return a namespace with the reference modules of the hot path (imported unmodified)."""
     if not available():
-        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}")
+        raise RuntimeError(f"original project not found (SDETR_REFERENCE_ROOT={REFERENCE_ROOT!r})")
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)
     _install_stub()

@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE ONLY -- CPU oracle for the Salience-DETR encoder hot path.
  *
  * A plain-C restatement of the reference algorithm (xiuqhou/Salience-DETR) used as the parity
- * checker for the sm_100a kernels.  Nothing on the product path may link or call this file; only
+ * checker for the sm_90a kernels.  Nothing on the product path may link or call this file; only
  * tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs do.
  *
  * Pinning: the reference ships no tests or golden vectors (SURVEY.md section 4), so this oracle is

@@ -1,4 +1,4 @@
-"""salience-detr_b200: B200-native (sm_100a) Salience-DETR encoder hot path.
+"""salience-detr_b200: H100-native (sm_90a) Salience-DETR encoder hot path.
 
 Hierarchical salience top-k token filter + multi-scale deformable self-attention over the selected
 tokens, behind the reference's own module / operator boundary (xiuqhou/Salience-DETR,

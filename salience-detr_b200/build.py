@@ -1,4 +1,4 @@
-"""Builds the C-ABI shared library (csrc/*.cu -> lib/libsdetr_b200.so) with plain nvcc for sm_100a.
+"""Builds the C-ABI shared library (csrc/*.cu -> lib/libsdetr_b200.so) with plain nvcc for sm_90a.
 
 Deliberately NOT a torch C++ extension: the library has no torch/ATen symbols (that coupling is what
 broke the reference's extension on a newer torch, SURVEY.md fact 2) and is loaded with ctypes.
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsdetr_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc() -> str:
@@ -37,7 +37,7 @@ def is_stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into one shared library; returns its path."""
+    """Compile every CUDA source for sm_90a into one shared library; returns its path."""
     if not force and not is_stale():
         return LIB
     os.makedirs(LIBDIR, exist_ok=True)

@@ -52,8 +52,6 @@ SIGNATURES = {
     "sdetr_add_layernorm": (_i, [_vp, _vp, _vp, _vp, _f, _i64, _i, _vp, _vp]),
     "sdetr_split_tf32": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp]),
     "sdetr_gemm_3xtf32_raw": (_i, [_vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp]),
-    "sdetr_gemm_set_trace": (_i, [_vp]),
-    "sdetr_gemm_set_variant": (_i, [_i]),
     "sdetr_split_tf32_pair": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "sdetr_gemm_3xtf32": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp]),
     "sdetr_gemm_3xtf32_pre": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp]),
@@ -63,11 +61,6 @@ SIGNATURES = {
     "sdetr_mask_plan": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sdetr_sine_pos_tokens": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _vp, _vp]),
     "sdetr_split_f16_pair": (_i, [_vp, _i64, _f, _vp, _vp, _vp]),
-    "sdetr_gemm_f16x3_set_as": (_i, [_i]),
-    "sdetr_gemm_f16x3_set_cluster": (_i, [_i]),
-    "sdetr_gemm_f16x3_set_epilogue": (_i, [_i]),
-    "sdetr_gemm_f16x3_set_epilogue_warps": (_i, [_i]),
-    "sdetr_gemm_f16x3_set_trace": (_i, [_vp]),
     "sdetr_gemm_f16x3_pre": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _i64, _i, _i, _i, _i, _vp]),
     "sdetr_gemm_f16x3_scaled": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp]),
     "sdetr_split_f16_pair_dev": (_i, [_vp, _i64, _vp, _vp, _vp, _vp]),
@@ -76,12 +69,8 @@ SIGNATURES = {
     "sdetr_mask_predictor_level": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _vp, _vp, _vp, _i64, _vp, _i64, _vp]),
     "sdetr_ffn_fused_workspace_floats": (_i64, [_i, _i]),
-    "sdetr_ffn_fused_ranges": (_i, [_i, _i, _vp, _i]),
-    "sdetr_ffn_fused_set_balance": (_i, [_i]),
     "sdetr_ffn_fused_layernorm": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _i, _i, _vp, _i64, _vp, _vp]),
-    "sdetr_ffn_fused_set_trace": (_i, [_vp]),
     "sdetr_flatten_set_vectorized": (_i, [_i]),
-    "sdetr_ffn_fused_set_max_ctas": (_i, [_i]),
     "sdetr_flatten_tokens": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "sdetr_attention_small": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "sdetr_attention_qkv": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
@@ -94,13 +83,13 @@ SIGNATURES = {
 
 
 def lib():
-    """Load (once) the sm_100a library.  Raises if it has not been built (``__graft_entry__.build()``)."""
+    """Load (once) the sm_90a library.  Raises if it has not been built (``__graft_entry__.build()``)."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU or PyTorch fallback for this path.")
+                "(nvcc, sm_90a). There is no CPU or PyTorch fallback for this path.")
         cdll = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(cdll, name)
@@ -508,7 +497,7 @@ def split_tf32_pair(w):
 
 
 def gemm_3xtf32(x, w_hi, w_lo, bias=None, relu_input=0):
-    """y = act(x) @ W.T + bias on the tcgen05 tensor cores; x (..., K) with unit last stride and uniform row pitch."""
+    """y = act(x) @ W.T + bias on the wgmma tensor cores; x (..., K) with unit last stride and uniform row pitch."""
     K = x.shape[-1]
     N = w_hi.shape[0]
     if not (x.is_cuda and x.dtype == torch.float32 and x.stride(-1) == 1):
@@ -677,7 +666,7 @@ def split_f16_pair(w):
 
 
 def gemm_f16x3_pre(x, w_hi, w_lo, w_scale, bias=None, act=0, out=None):
-    """y = act(x) @ W.T + bias on the persistent tcgen05.mma.kind::f16 kernel (3xFP16, fp32-class accuracy).
+    """y = act(x) @ W.T + bias on the persistent wgmma .f16 kernel (3xFP16, fp32-class accuracy).
     ``out``: optional (M, N) fp32 destination with unit column stride (e.g. a row slice of a larger buffer)."""
     K = x.shape[-1]
     N = w_hi.shape[0]
@@ -706,7 +695,7 @@ def gemm_f16x3_pre(x, w_hi, w_lo, w_scale, bias=None, act=0, out=None):
 
 
 def ffn_fused_layernorm(x, w1, b1, w2, b2, gamma=None, beta=None, eps: float = 1e-5, out=None):
-    """y = LayerNorm(x + linear2(ReLU(linear1(x)))) by the fused tcgen05 kernel (gamma None: the bare FFN, no residual / norm).
+    """y = LayerNorm(x + linear2(ReLU(linear1(x)))) by the 3xFP16 wgmma kernel (gamma None: the bare FFN, no residual / norm).
     ``w1`` / ``w2``: (W_hi, W_lo, scale) triples of ``split_f16_pair``; x (..., 256) fp32 with unit last stride."""
     if not (x.is_cuda and x.dtype == torch.float32 and x.shape[-1] == 256 and x.stride(-1) == 1):
         raise RuntimeError("ffn_fused_layernorm needs a CUDA float32 (..., 256) input with unit last stride")

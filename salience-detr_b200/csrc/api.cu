@@ -18,10 +18,10 @@ void set_error(const char *fmt, ...) {
 int sm_count() {
     static std::atomic<int> cache[256];
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     int v = cache[dev & 255].load(std::memory_order_relaxed);
     if (!v) {
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         cache[dev & 255].store(v, std::memory_order_relaxed);
     }
     return v;

@@ -1,4 +1,4 @@
-// Shared helpers of the sm_100a kernels behind include/sdetr_b200.h.
+// Shared helpers of the sm_90a kernels behind include/sdetr_b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,388 +1,33 @@
-// Fused encoder FFN -- sdetr_ffn_fused_layernorm:   y = LayerNorm(x + linear2(ReLU(linear1(x))))
+// Encoder FFN -- sdetr_ffn_fused_layernorm:   y = LayerNorm(x + linear2(ReLU(linear1(x))))
 // (reference models/bricks/salience_transformer.py:347-351 `forward_ffn` + :391 `norm2`; C = 256, any hidden width % 128 == 0).
 //
-// As two GEMMs (gemm_f16x3.cu) the hidden activations (rows x 2048 fp32 = 186 MB at layer 0) are written to HBM and read
-// back, and both GEMMs run at the L2 -> SM fabric cap (DESIGN 3.4: 922 MB + 760 MB through the crossbar for one layer-0 FFN).
-// Here a CTA keeps one 128-row panel on chip from x to the output accumulator; only the weights stream:
-//
-//   work unit = the part of one 128-row panel inside a CTA's range of the (panel, chunk) sequence (see ffn_range_lo below;
-//              a chunk = 128 hidden units); per chunk j of the unit:
-//              G1: ACC1[128x128]   = X_hi.W1_hi^T + X_hi.W1_lo^T + X_lo.W1_hi^T      (K = 256, A and B from shared memory)
-//              cv: H = ReLU(ACC1 * 2^-(4+s1) + b1) * 16 -> split to fp16 hi / lo -> tensor memory (A operand of G2)
-//              G2: OUT[128x256]   += H_hi.W2_hi^T + H_lo.W2_hi^T + H_hi.W2_lo^T      (K = 128, N = 256 instructions)
-//   same 3xFP16 error-compensated products, scalings and accumulation as sdetr_gemm_f16x3_pre (fp32-class accuracy).
-//   The unit writes OUT * 2^-(4+s2) to its partial slot; ffn_finish_kernel adds a panel's partials (one per contributing
-//   CTA, in CTA order: deterministic), b2 and the residual and applies the LayerNorm.
-//
-//   tensor memory (512 columns): OUT [0,256) | ACC1 [256,384) | H_hi [384,448) | H_lo [448,512)   (all single-buffered: the
-//     issue order G1(j), G2(j-1), G1(j+1), ... keeps the tensor pipe busy while the converters turn ACC1(j) into H(j))
-//   shared memory: X panel, split once per unit: 4 k-blocks x {hi, lo} x (128 rows x 64 fp16, 128-byte swizzle) = 128 KB (the raw
-//     fp32 k-block lands by TMA in the 32 KB its two tiles will occupy and is split in place, while the previous unit's last G2
-//     runs); ring of 3 x 32 KB weight stages in consumption order: per chunk 4 x {W1_hi, W1_lo} k-block tiles (128 x 64 fp16
-//     each) and 4 x W2 tiles (256 x 64 fp16: k-block 0 hi, lo, k-block 1 hi, lo).
-//   warps: 0 weight producer (TMA), 1 MMA issuer, 2 TMEM allocator, 3 x producer (TMA), 4..11 converters, 12..15 epilogue.
-//   L2 -> SM traffic per panel: 128 KB of x + 4 MB of weights, against 9.4 MB for the two separate GEMMs.
-//   Measured (tools/ffn_trace.py, ncu): a chunk takes ~7000 clk in steady state = 96 MMA-equivalents of 128x128x16 at 73 clk,
-//   i.e. the measured bf16 peak of MEASURED_PEAKS.json (the SM clock sags to ~1.6 GHz under this load: power-bound).
-#include "umma.cuh"
+// Three launches on the 3xFP16 wgmma kernel of wgmma.cuh (same error-compensated products, scalings and accumulation as
+// sdetr_gemm_f16x3_pre, fp32-class accuracy):
+//   H = x W1^T + b1                       (M, hidden) fp32 in the workspace
+//   P = ReLU(H) W2^T + b2                 the ReLU is fused into the second GEMM's operand load; P goes to the workspace, or
+//                                         straight to y without LayerNorm
+//   y = LayerNorm(x + P) * gamma + beta   ffn_finish_kernel, one warp per row (x may alias y).
+// Deterministic: no atomics, a fixed reduction order per row.
+#include "wgmma.cuh"
 
 namespace sdetr {
 
-constexpr int kFD = 256;                 // model width: K of linear1, N of linear2
-constexpr int kFTile = 128 * 128;        // 16 KB: 128 rows x 128 bytes
-constexpr int kFPanel = 8 * kFTile;      // split X panel: (k-block, hi|lo) tiles
-constexpr int kFStage = 2 * kFTile;      // 32 KB
-constexpr int kFStages = 3;
-constexpr int kFRing = kFStages * kFStage;
-constexpr int kFSmem = kFPanel + kFRing + 1024 /* alignment */ + 256 /* barriers */ + 1024 /* two bias-1 slices */;
-constexpr int kFThreads = 512;
-constexpr float kFActScale = 16.f;
-constexpr uint32_t kIdescN128 = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-constexpr uint32_t kIdescN256 = (1u << 4) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-constexpr uint32_t kColOut = 0, kColAcc1 = 256, kColHhi = 384, kColHlo = 448;
+constexpr int kFD = 256;  // model width: K of linear1, N of linear2
 
-struct FfnParams {
-    const float *b1;
-    float *partial;       // [slot][128][256], slot = CTA + panel (strictly increasing along the flattened chunk sequence)
-    int M, chunks;        // chunks = hidden / 128 per panel
-    int balance;          // 1: equal chunk counts per CTA (ranges may cut panels); 0: whole panels per CTA
-    float inv1, inv2;     // 1 / (16 * weight scale), powers of two
-    long long *dbg;       // optional clock64() trace of CTA 0 (sdetr_ffn_fused_set_trace): [event][index < 256]
-};
-// Work decomposition.  All (panel, chunk) pairs in panel-major order form one sequence of `panels * chunks` items; CTA i of G
-// owns the contiguous range [lo(i), lo(i + 1)).  balance = 1: lo(i) = floor(total * i / G) -- every CTA gets the same number of
-// chunks (+-1) whatever the panel count (178 panels on 148 SMs are 19.2 chunks each, not two rounds of whole panels), at the
-// price of panels shared by two (rarely three) CTAs, each writing its partial sum of the panel's output; balance = 0: ranges
-// rounded to whole panels.  A "unit" is the part of one panel inside a CTA's range.
-__host__ __device__ inline long long ffn_range_lo(long long panels, int chunks, int G, int balance, long long i) {
-    return balance ? panels * chunks * i / G : (panels * i / G) * chunks;
-}
-struct FfnUnits {  // iteration over the units of one CTA
-    long long pos, hi;
-    int chunks;
-    __device__ FfnUnits(const FfnParams &p, int cta, int G) : chunks(p.chunks) {
-        const long long panels = (p.M + 127) / 128;
-        pos = ffn_range_lo(panels, p.chunks, G, p.balance, cta), hi = ffn_range_lo(panels, p.chunks, G, p.balance, cta + 1);
-    }
-    __device__ bool valid() const { return pos < hi; }
-    __device__ int panel() const { return (int)(pos / chunks); }
-    __device__ int c0() const { return (int)(pos % chunks); }
-    __device__ int nc() const {
-        const long long end = (long long)(panel() + 1) * chunks;
-        return (int)((hi < end ? hi : end) - pos);
-    }
-    __device__ bool has_next() const { return pos + nc() < hi; }
-    __device__ void next() { pos += nc(); }
-};
-
-#define FTRACE(ev, idx)                                                                          \
-    do {                                                                                         \
-        if (p.dbg && blockIdx.x == 0 && (idx) < 256) p.dbg[(ev) * 256 + (idx)] = clock64();      \
-    } while (0)
-
-__global__ void __launch_bounds__(kFThreads, 1)
-ffn_fused_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w1hi,
-                 const __grid_constant__ CUtensorMap map_w1lo, const __grid_constant__ CUtensorMap map_w2hi,
-                 const __grid_constant__ CUtensorMap map_w2lo, const FfnParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *panel = smem, *ring = smem + kFPanel;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kFPanel + kFRing);
-    uint64_t *full = bars, *empty = bars + kFStages;
-    uint64_t *panel_full = bars + 2 * kFStages;  // [4]: k-block kb of the unit's split x panel is written
-    uint64_t *panel_free = panel_full + 4, *acc1_full = panel_free + 1, *acc1_free = acc1_full + 1;
-    uint64_t *h_full = acc1_free + 1, *h_free = h_full + 1, *out_full = h_free + 1, *out_free = out_full + 1;
-    uint64_t *x_full = out_free + 1;  // [4]: raw x k-block kb of the unit landed in the panel region
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(x_full + 4);
-    float *sbias = reinterpret_cast<float *>(smem + kFPanel + kFRing + 256);  // 2 x 128
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kFStages; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 1);
-        mbar_init(panel_free, 1);
-        for (int kb = 0; kb < 4; ++kb) mbar_init(panel_full + kb, 256), mbar_init(x_full + kb, 1);
-        mbar_init(acc1_full, 1), mbar_init(acc1_free, 256);
-        mbar_init(h_full, 256), mbar_init(h_free, 1);
-        mbar_init(out_full, 1), mbar_init(out_free, 128);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== TMA producer: ring slots in exactly the order the converters / the MMA warp consume them =====
-        if (lane == 0) {
-            uint32_t it = 0;
-            auto slot = [&]() -> uint8_t * {
-                const int s = it % kFStages;
-                mbar_wait(empty + s, ((it / kFStages) & 1) ^ 1);
-                FTRACE(6, it);
-                mbar_expect_tx(full + s, kFStage);
-                return ring + s * kFStage;
-            };
-            for (FfnUnits un(p, blockIdx.x, gridDim.x); un.valid(); un.next()) {
-                const int c0 = un.c0(), nc = un.nc();
-                for (int j = 0; j <= nc; ++j) {
-                    if (j < nc)
-                        for (int kb = 0; kb < 4; ++kb, ++it) {  // W1 rows of chunk c0 + j, k-block kb
-                            uint8_t *st = slot();
-                            uint64_t *bar = full + it % kFStages;
-                            tma_load_2d(&map_w1hi, bar, st, kb * 64, (c0 + j) * 128);
-                            tma_load_2d(&map_w1lo, bar, st + kFTile, kb * 64, (c0 + j) * 128);
-                        }
-                    if (j > 0)
-                        for (int t = 0; t < 4; ++t, ++it) {  // W2 columns of chunk c0 + j - 1: (k-block t >> 1, hi | lo)
-                            uint8_t *st = slot();
-                            uint64_t *bar = full + it % kFStages;
-                            tma_load_2d((t & 1) ? &map_w2lo : &map_w2hi, bar, st, (c0 + j - 1) * 128 + (t >> 1) * 64, 0);
-                        }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            uint32_t it = 0, g = 0, u = 0;
-            const uint32_t t_out = tmem_base + kColOut, t_acc1 = tmem_base + kColAcc1;
-            const uint32_t t_hhi = tmem_base + kColHhi, t_hlo = tmem_base + kColHlo;
-            const uint32_t panel_addr = smem_u32(panel);
-            for (FfnUnits un(p, blockIdx.x, gridDim.x); un.valid(); un.next(), ++u) {
-                const int nc = un.nc();
-                for (int j = 0; j <= nc; ++j) {
-                    if (j < nc) {  // G1(j)
-                        const uint32_t gg = g + j;
-                        mbar_wait(acc1_free, (gg & 1) ^ 1);  // the converters have read the previous chunk's accumulator
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        for (int kb = 0; kb < 4; ++kb, ++it) {
-                            if (j == 0) mbar_wait(panel_full + kb, u & 1);
-                            const int s = it % kFStages;
-                            mbar_wait(full + s, (it / kFStages) & 1);
-                            FTRACE(0, it);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            const uint32_t st = smem_u32(ring + s * kFStage);
-                            const uint64_t a_hi = umma_desc(panel_addr + (2 * kb) * kFTile), a_lo = umma_desc(panel_addr + (2 * kb + 1) * kFTile);
-                            const uint64_t b_hi = umma_desc(st), b_lo = umma_desc(st + kFTile);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                umma_f16_ss(t_acc1, a_hi + 2 * k, b_hi + 2 * k, kIdescN128, (kb | k) != 0);
-                                umma_f16_ss(t_acc1, a_hi + 2 * k, b_lo + 2 * k, kIdescN128, 1);
-                                umma_f16_ss(t_acc1, a_lo + 2 * k, b_hi + 2 * k, kIdescN128, 1);
-                            }
-                            umma_commit(empty + s);
-                        }
-                        umma_commit(acc1_full);
-                        if (j == nc - 1) umma_commit(panel_free);  // the split panel may be rewritten for the next unit
-                    }
-                    if (j > 0) {  // G2(j - 1)
-                        const uint32_t gg = g + j - 1;
-                        mbar_wait(h_full, gg & 1);
-                        if (j == 1) mbar_wait(out_free, (u & 1) ^ 1);  // the epilogue has read the previous unit's output
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        for (int t = 0; t < 4; ++t, ++it) {
-                            const int s = it % kFStages;
-                            mbar_wait(full + s, (it / kFStages) & 1);
-                            FTRACE(1, it);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            const uint64_t b = umma_desc(smem_u32(ring + s * kFStage));
-                            const uint32_t kcol = 32u * (uint32_t)(t >> 1);
-                            if ((t & 1) == 0) {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) {
-                                    umma_f16_ts(t_out, t_hhi + kcol + 8u * k, b + 2 * k, kIdescN256, !(j == 1 && t == 0 && k == 0));
-                                    umma_f16_ts(t_out, t_hlo + kcol + 8u * k, b + 2 * k, kIdescN256, 1);
-                                }
-                            } else {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) umma_f16_ts(t_out, t_hhi + kcol + 8u * k, b + 2 * k, kIdescN256, 1);
-                            }
-                            umma_commit(empty + s);
-                        }
-                        umma_commit(h_free);
-                    }
-                }
-                umma_commit(out_full);
-                g += nc;
-            }
-        }
-    } else if (warp == 3) {
-        // ===== x producer: the unit's raw fp32 rows land IN the panel region (k-block kb: two 128 x 32 boxes = the 32 KB that its
-        // hi and lo tiles will occupy), as soon as the previous unit's last G1 has read the panel =====
-        if (lane == 0) {
-            uint32_t u = 0;
-            for (FfnUnits un(p, blockIdx.x, gridDim.x); un.valid(); un.next(), ++u) {
-                if (u > 0) mbar_wait(panel_free, (u - 1) & 1);
-                FTRACE(7, 4 * u);
-                const int m0 = un.panel() * 128;
-                for (int kb = 0; kb < 4; ++kb) {
-                    mbar_expect_tx(x_full + kb, kFStage);
-                    tma_load_2d(&map_x, x_full + kb, panel + kb * kFStage, kb * 64, m0);
-                    tma_load_2d(&map_x, x_full + kb, panel + kb * kFStage + kFTile, kb * 64 + 32, m0);
-                }
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ===== converters =====
-        const int q = warp & 3, half = (warp - 4) >> 2, r_in = q * 32 + lane, tc = threadIdx.x - 128;
-        const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-        uint32_t g = 0, u = 0;
-        // x panel of a unit, in place per k-block: raw fp32 boxes -> registers -> (all read) -> * 16, split -> the k-block's hi and lo
-        // tiles (128 rows x 64 fp16, K-major, 128-byte swizzle) over the same 32 KB
-        auto convert_x = [&](uint32_t ux /* unit ordinal */) {
-            for (int kb = 0; kb < 4; ++kb) {
-                mbar_wait(x_full + kb, ux & 1);
-                if (tc == 0 && kb == 0) FTRACE(7, 4 * ux + 1);
-                uint8_t *region = panel + kb * kFStage;
-                const uint8_t *arow = region + half * kFTile + r_in * 128;
-                float4 v[8];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) v[c] = *reinterpret_cast<const float4 *>(arow + ((c ^ (r_in & 7)) << 4));
-                named_bar_sync(2, 256);  // every converter holds its 32 floats: the boxes may be overwritten
-                uint8_t *hrow = region + r_in * 128, *lrow = hrow + kFTile;
-#pragma unroll
-                for (int c = 0; c < 8; c += 2) {  // two 16-byte chunks of floats -> one 16-byte chunk of halves
-                    uint4 h, l;
-                    split2(v[c].x * kFActScale, v[c].y * kFActScale, h.x, l.x);
-                    split2(v[c].z * kFActScale, v[c].w * kFActScale, h.y, l.y);
-                    split2(v[c + 1].x * kFActScale, v[c + 1].y * kFActScale, h.z, l.z);
-                    split2(v[c + 1].z * kFActScale, v[c + 1].w * kFActScale, h.w, l.w);
-                    const int oc = ((4 * half + (c >> 1)) ^ (r_in & 7)) << 4;
-                    *reinterpret_cast<uint4 *>(hrow + oc) = h;
-                    *reinterpret_cast<uint4 *>(lrow + oc) = l;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA's reads
-                mbar_arrive(panel_full + kb);  // G1 of the first chunk starts on k-block 0 while the others are being split
-            }
-            if (tc == 0) FTRACE(7, 4 * ux + 2);
-        };
-        FfnUnits un(p, blockIdx.x, gridDim.x);
-        if (un.valid()) convert_x(0);
-        for (; un.valid(); un.next(), ++u) {
-            const int c0 = un.c0(), nc = un.nc();
-            const bool has_next = un.has_next();
-            for (int j = 0; j < nc; ++j) {
-                const uint32_t gg = g + j;
-                const float bval = tc < 128 ? __ldg(p.b1 + (c0 + j) * 128 + tc) : 0.f;
-                mbar_wait(acc1_full, gg & 1);
-                if (tc == 0) FTRACE(2, gg);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                float *sb = sbias + (gg & 1) * 128;
-                if (tc < 128) sb[tc] = bval;
-                uint32_t r0[32], r1[32];
-                tmem_ld32(lane_base + kColAcc1 + 64u * half, r0);
-                tmem_ld32(lane_base + kColAcc1 + 64u * half + 32u, r1);
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(acc1_free);
-                named_bar_sync(2, 256);  // bias slice visible
-                uint32_t hi[32], lo[32];
-                const float *bb = sb + 64 * half;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float2 b2 = *reinterpret_cast<const float2 *>(bb + 2 * i);
-                    const float h0 = fmaxf(fmaf(__uint_as_float(r0[2 * i]), p.inv1, b2.x), 0.f) * kFActScale;
-                    const float h1 = fmaxf(fmaf(__uint_as_float(r0[2 * i + 1]), p.inv1, b2.y), 0.f) * kFActScale;
-                    split2(h0, h1, hi[i], lo[i]);
-                }
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float2 b2 = *reinterpret_cast<const float2 *>(bb + 32 + 2 * i);
-                    const float h0 = fmaxf(fmaf(__uint_as_float(r1[2 * i]), p.inv1, b2.x), 0.f) * kFActScale;
-                    const float h1 = fmaxf(fmaf(__uint_as_float(r1[2 * i + 1]), p.inv1, b2.y), 0.f) * kFActScale;
-                    split2(h0, h1, hi[16 + i], lo[16 + i]);
-                }
-                mbar_wait(h_free, (gg & 1) ^ 1);  // G2 of the previous chunk has read the slot
-                if (tc == 0) FTRACE(3, gg);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                tmem_st16u(lane_base + kColHhi + 32u * half, *reinterpret_cast<const uint32_t(*)[16]>(hi));
-                tmem_st16u(lane_base + kColHhi + 32u * half + 16u, *reinterpret_cast<const uint32_t(*)[16]>(hi + 16));
-                tmem_st16u(lane_base + kColHlo + 32u * half, *reinterpret_cast<const uint32_t(*)[16]>(lo));
-                tmem_st16u(lane_base + kColHlo + 32u * half + 16u, *reinterpret_cast<const uint32_t(*)[16]>(lo + 16));
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(h_full);
-                if (tc == 0) FTRACE(4, gg);
-            }
-            g += nc;
-            if (has_next) convert_x(u + 1);  // the next unit's x panel, while the last G2 of this one runs
-        }
-    } else if (warp >= 12) {
-        // ===== epilogue: OUT * 2^-(4+s2) -> partial[s] (each thread one row, 128 contiguous bytes per column block) =====
-        const int q = warp & 3, r_in = q * 32 + lane;
-        uint32_t u = 0;
-        for (FfnUnits un(p, blockIdx.x, gridDim.x); un.valid(); un.next(), ++u) {
-            const int row = un.panel() * 128 + r_in;
-            float *dst = p.partial + ((int64_t)(blockIdx.x + un.panel()) * 128 + r_in) * kFD;
-            mbar_wait(out_full, u & 1);
-            if (threadIdx.x == 12 * 32) FTRACE(5, u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int c = 0; c < 8; ++c) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + kColOut + (uint32_t)(c * 32), r);
-                if (c == 7) {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    mbar_arrive(out_free);
-                }
-                if (row < p.M) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        st_stream_f4(dst + c * 32 + j, make_float4(__uint_as_float(r[j]) * p.inv2, __uint_as_float(r[j + 1]) * p.inv2,
-                                                                  __uint_as_float(r[j + 2]) * p.inv2, __uint_as_float(r[j + 3]) * p.inv2));
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
-
-// y = LayerNorm(x + b2 + sum of the row's partials) (gamma != NULL), or y = b2 + sum (gamma == NULL).  One warp per row, C = 256.
-// The partials of panel p come from the CTAs whose ranges intersect [p * chunks, (p + 1) * chunks), slot = CTA + p.
-__global__ void __launch_bounds__(256) ffn_finish_kernel(const float *x /* may alias y */, int64_t ldx, const float *partial,
-                                                         int chunks, int G, int balance, const float *__restrict__ b2,
-                                                         const float *__restrict__ gamma, const float *__restrict__ beta,
-                                                         float eps, int64_t rows, float *y) {
+__global__ void __launch_bounds__(256) ffn_finish_kernel(const float *x /* may alias y */, int64_t ldx, const float *__restrict__ partial,
+                                                         const float *__restrict__ gamma, const float *__restrict__ beta, float eps,
+                                                         int64_t rows, float *y) {
     const int lane = threadIdx.x & 31;
     const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (row >= rows) return;
-    const long long panels = (rows + 127) / 128, pn = row >> 7;
-    auto cta_of = [&](long long item) {  // the CTA whose range holds `item`
-        long long i = balance ? item * G / (panels * chunks) : (item / chunks) * G / panels;
-        while (i + 1 < G && ffn_range_lo(panels, chunks, G, balance, i + 1) <= item) ++i;
-        while (i > 0 && ffn_range_lo(panels, chunks, G, balance, i) > item) --i;
-        return i;
-    };
-    const long long i0 = cta_of(pn * chunks), i1 = cta_of(pn * chunks + chunks - 1);
     float4 v[2];
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         const int c = i * 128 + lane * 4;
-        float4 a = b2 ? ldg_f4(b2 + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        for (long long k = i0; k <= i1; ++k) {
-            const float4 t = ld_stream_f4(partial + ((k + pn) * 128 + (row & 127)) * kFD + c);
-            a.x += t.x, a.y += t.y, a.z += t.z, a.w += t.w;
-        }
-        if (gamma) {
-            const float4 r = *reinterpret_cast<const float4 *>(x + row * ldx + c);
-            a.x += r.x, a.y += r.y, a.z += r.z, a.w += r.w;
-        }
-        v[i] = a;
-        s += (a.x + a.y) + (a.z + a.w);
-    }
-    if (!gamma) {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) *reinterpret_cast<float4 *>(y + row * kFD + i * 128 + lane * 4) = v[i];
-        return;
+        const float4 a = ld_stream_f4(partial + row * kFD + c), r = *reinterpret_cast<const float4 *>(x + row * ldx + c);
+        v[i] = make_float4(r.x + a.x, r.y + a.y, r.z + a.z, r.w + a.w);
+        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -411,47 +56,9 @@ __global__ void __launch_bounds__(256) ffn_finish_kernel(const float *x /* may a
 
 using namespace sdetr;
 
-static std::atomic<long long *> g_ffn_dbg{nullptr};
-
-static std::atomic<int> g_ffn_max_ctas{0};
-extern "C" int sdetr_ffn_fused_set_max_ctas(int n /* 0 = one per SM */) {
-    g_ffn_max_ctas = n > 0 ? n : 0;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_ffn_fused_set_trace(long long *device_buffer /* 8 * 256 int64, or NULL */) {
-    g_ffn_dbg = device_buffer;
-    return SDETR_OK;
-}
-
-static std::atomic<int> g_ffn_balance{1};
-extern "C" int sdetr_ffn_fused_set_balance(int enable /* 1 (default): equal chunk counts per CTA; 0: whole panels per CTA */) {
-    g_ffn_balance = enable ? 1 : 0;
-    return SDETR_OK;
-}
-
-// persistent CTAs for M rows: one per SM, but at least two chunks each (balance) / one panel each (whole panels)
-static int ffn_grid(int M, int chunks, int balance) {
-    const int cap = g_ffn_max_ctas.load();
-    const long long sms = cap > 0 && cap < persistent_ctas() ? cap : persistent_ctas();
-    const long long panels = (M + 127) / 128, most = balance ? (panels * chunks + 1) / 2 : panels;
-    return (int)(most < sms ? (most > 0 ? most : 1) : sms);
-}
-
-// host-side view of the decomposition, for tests: lo[i] = first (panel, chunk) item of CTA i, lo[G] = panels * chunks; returns G
-extern "C" int sdetr_ffn_fused_ranges(int M, int hidden, int64_t *lo, int capacity) {
-    if (M <= 0 || hidden <= 0 || hidden % 128 || !lo) return 0;
-    const int chunks = hidden / 128, balance = g_ffn_balance.load(), G = ffn_grid(M, chunks, balance);
-    if (capacity < G + 1) return -G;
-    for (int i = 0; i <= G; ++i) lo[i] = ffn_range_lo((M + 127) / 128, chunks, G, balance, i);
-    return G;
-}
-
 extern "C" int64_t sdetr_ffn_fused_workspace_floats(int M, int hidden) {
     if (M <= 0 || hidden <= 0 || hidden % 128) return 0;
-    const int balance = g_ffn_balance.load();
-    const int64_t slots = (int64_t)ffn_grid(M, hidden / 128, balance) + (M + 127) / 128;  // slot = CTA + panel
-    return slots * 128 * kFD;
+    return (int64_t)M * (hidden + kFD);  // H, then P
 }
 
 extern "C" int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *w1_hi, const void *w1_lo, float w1_scale,
@@ -466,23 +73,21 @@ extern "C" int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void
                       aligned16(w2_lo) && aligned16(workspace) && aligned16(y),
                   SDETR_ERR_INVALID_ARG, "ffn_fused: operands must be 16-byte aligned with a 16-byte row pitch");
     if (M == 0) return SDETR_OK;
-    const int chunks = hidden / 128, balance = g_ffn_balance.load(), G = ffn_grid(M, chunks, balance);
-    SDETR_REQUIRE(workspace_floats >= ((int64_t)G + (M + 127) / 128) * 128 * kFD, SDETR_ERR_INVALID_ARG,
+    SDETR_REQUIRE(workspace_floats >= (int64_t)M * (hidden + kFD), SDETR_ERR_INVALID_ARG,
                   "ffn_fused: workspace of %lld floats is smaller than sdetr_ffn_fused_workspace_floats", (long long)workspace_floats);
-    CUtensorMap mx, m1h, m1l, m2h, m2l;
-    SDETR_REQUIRE(make_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, M, kFD, ldx, 32, 128) &&
-                      make_map_2d(&m1h, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w1_hi, hidden, kFD, kFD, 64, 128) &&
-                      make_map_2d(&m1l, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w1_lo, hidden, kFD, kFD, 64, 128) &&
-                      make_map_2d(&m2h, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_hi, kFD, hidden, hidden, 64, 256) &&
-                      make_map_2d(&m2l, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_lo, kFD, hidden, hidden, 64, 256),
+    CUtensorMap m1h, m1l, m2h, m2l;
+    SDETR_REQUIRE(make_map_2d(&m1h, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w1_hi, hidden, kFD, kFD, 64, kGN) &&
+                      make_map_2d(&m1l, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w1_lo, hidden, kFD, kFD, 64, kGN) &&
+                      make_map_2d(&m2h, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_hi, kFD, hidden, hidden, 64, kGN) &&
+                      make_map_2d(&m2l, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_lo, kFD, hidden, hidden, 64, kGN),
                   SDETR_ERR_CUDA, "ffn_fused: cuTensorMapEncodeTiled failed");
-    static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, ffn_fused_kernel, kFSmem, "ffn_fused");
-    FfnParams p{b1, workspace, M, chunks, balance, 1.f / (kFActScale * w1_scale), 1.f / (kFActScale * w2_scale), g_ffn_dbg.load()};
-    ffn_fused_kernel<<<G, kFThreads, kFSmem, (cudaStream_t)stream>>>(mx, m1h, m1l, m2h, m2l, p);
-    int rc = check_launch("ffn_fused");
+    float *h = workspace, *part = gamma ? workspace + (int64_t)M * hidden : y;
+    const Gemm3xParams p1{b1, h, hidden, M, hidden, kFD, 0, kActScale, 1.f / (kActScale * w1_scale), nullptr, nullptr};
+    int rc = launch_gemm3x<true, false>(x, ldx, m1h, m1l, p1, stream, "ffn_fused/linear1");
     if (rc != SDETR_OK) return rc;
-    ffn_finish_kernel<<<(unsigned)((M + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, ldx, workspace, chunks, G, balance, b2, gamma, beta,
-                                                                                 eps, M, y);
+    const Gemm3xParams p2{b2, part, kFD, M, kFD, hidden, 1, kActScale, 1.f / (kActScale * w2_scale), nullptr, nullptr};
+    rc = launch_gemm3x<true, false>(h, hidden, m2h, m2l, p2, stream, "ffn_fused/linear2");
+    if (rc != SDETR_OK || !gamma) return rc;
+    ffn_finish_kernel<<<(unsigned)((M + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, ldx, part, gamma, beta, eps, M, y);
     return check_launch("ffn_fused/finish");
 }

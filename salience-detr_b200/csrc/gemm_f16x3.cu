@@ -1,539 +1,29 @@
-// Dense projection GEMM of the path, third generation -- sdetr_gemm_f16x3_pre ("3xFP16", fp32-class accuracy).
+// Dense projection GEMM of the path -- sdetr_gemm_f16x3_pre / _scaled ("3xFP16", fp32-class accuracy).
 //
 //   C[M,N] = act(A)[M,K] . W[N,K]^T + bias        fp32 in / fp32 out
 //
 // Same projections as gemm_tf32x3.cu (models/bricks/ms_deform_attn.py:316,322-328,375; salience_transformer.py:347-351,
-// :462, :16-47; base_transformer.py:111).  The 3xTF32 kernel there is bound by shared-memory bandwidth and by the TF32
-// tensor rate (profiles/r1_gemm_tcgen05_presplit_ncu_full.txt).  An fp16 significand is as wide as a TF32 one (11 bits),
-// so the same error-compensated product
+// :462, :16-47; base_transformer.py:111).  An fp16 significand is as wide as a TF32 one (11 bits), so the same
+// error-compensated product
 //
 //       x = hi + lo,  hi = fp16(x),  lo = fp16(x - hi)          C ~= A_hi.W_hi + A_hi.W_lo + A_lo.W_hi  (fp32 accumulate)
 //
 // keeps 22 significand bits per operand exactly like 3xTF32 (Ootomo & Yokota, "Recovering single precision accuracy from
-// Tensor Cores ...", 2022), but runs on tcgen05.mma.kind::f16: twice the K per instruction at the same issue cost and half
-// the operand bytes through shared memory.  What fp16 lacks is exponent range; it is restored with exact power-of-two
+// Tensor Cores ...", 2022), but runs on wgmma .f16: twice the K per instruction and twice the dense rate of TF32, and half
+// the weight bytes through shared memory.  What fp16 lacks is exponent range; it is restored with exact power-of-two
 // scalings: the activation is multiplied by 16 before the split (full accuracy for 2^-7 <= |x| < 4094, an ABSOLUTE error
 // floor of 2^-29 below that, inf -> NaN above: documented domain of this entry point), the weight by a per-tensor 2^s that
 // puts max|W| in [2^13, 2^14) when it is pre-split (cached per parameter), and the epilogue multiplies the accumulator by
 // the exact inverse 2^-(4+s) before adding the bias.
 //
-// Structure = the persistent kernel "P" of gemm_tf32x3.cu (one 512-thread CTA per SM walking a strided tile list; warp 0
-// TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4..11 converters, warps 12..15 epilogue; double-buffered
-// accumulator in tensor memory; TMA-store epilogue), with a k-block of 64:
-//   stage (64 KB, x3): A raw fp32 as two 128x32 boxes (16 KB each, 128-byte swizzle) + W_hi + W_lo as 128x64 fp16 tiles
-//                      (16 KB each, 128-byte rows);
-//   converters:        thread (row, half) reads its 32 floats swizzle-aware, scales, splits, packs to f16x2 and writes
-//                      16 + 16 columns of the stage's TMEM slot with tcgen05.st (A operand comes from tensor memory);
-//   MMA:               4 k-steps (K = 16) x {hi.hi, hi.lo, lo.hi} = 12 tcgen05.mma.kind::f16 of 128x128x16 per k-block;
-//   TMEM map (512):    accumulators [0,128) and [128,256); A slot s at [256 + 64 s, 256 + 64 (s+1)): 32 columns A_hi
-//                      (64 halves) then 32 columns A_lo.
-// Shared-memory traffic per 128x128x64 block: TMA 64 KB + converter reads 32 KB + MMA operand reads 48 KB = 144 KB
-// (3xTF32: 224 KB for the same K) and 12 instead of 24 MMA instructions.
+// The kernel is gemm3x_kernel<true, false> of wgmma.cuh: k-blocks of 64, stage = A as two 128x32 fp32 boxes + W_hi + W_lo
+// as 128x64 fp16 tiles (64 KB, three stages); per k-block and warpgroup 4 k-steps x {lo.hi, hi.lo, hi.hi} = 12 wgmma
+// m64n128k16 with the split activation in registers.
 #include <cuda_fp16.h>
 
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace sdetr {
-
-constexpr int kHM = 128, kHN = 128, kHK = 64;
-constexpr int kHStages = 3;
-constexpr int kHBox = 128 * 32 * 4;               // 16 KB: one A box (128 rows x 32 fp32) == one W tile (128 rows x 64 fp16)
-constexpr int kHStageBytes = 4 * kHBox;           // A box 0, A box 1, W_hi, W_lo
-constexpr int kHRingBytes = kHStages * kHStageBytes;  // 192 KB
-constexpr int kHOutBoxes = 2 * kHBox;             // two 128x32 fp32 staging boxes for the TMA stores
-constexpr int kHSmem = kHRingBytes + kHOutBoxes + 1024 /* alignment */ + 256 /* barriers */ + 1024 /* bias slices */;
-constexpr int kHThreads = 512;
-constexpr int kHConvWarps = 8;
-constexpr float kActScale = 16.f;                 // activation pre-scale (exact), see header comment
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = f32 (1 << 4), A = B = f16 (format 0), both K-major, N, M
-constexpr uint32_t kIdescF16 = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(kHN >> 3) << 17) | ((uint32_t)(kHM >> 4) << 24);
-
-struct HGemmParams {
-    const float *bias;
-    float *C;
-    int64_t ldc;
-    int M, N, K, act, use_tma_store;
-    float out_scale;  // 1 / (kActScale * weight scale), a power of two
-    const float *a_scale_dev;  // optional device scalars (powers of two): activation scale replacing kActScale (activations of
-    const float *w_scale_dev;  // unknown magnitude: gradients) and the scale the weight pair was split with (weights that change
-                               // every step: no host read of max|W|); the epilogue then uses 1 / (a * w)
-    int epilogue;     // streaming kernel: 0 = shared boxes + TMA stores, 1 = warp-private boxes + coalesced 128-bit global stores
-    long long *dbg;   // optional clock64() trace of CTA 0: [event][index < 256] (sdetr_gemm_f16x3_set_trace, tools/gemm_trace2.py; 10 events)
-};
-#define HTRACE(ev, idx)                                                                              \
-    do {                                                                                             \
-        if (p.dbg && blockIdx.x == 0 && (idx) < 256) p.dbg[(ev) * 256 + (idx)] = clock64();          \
-    } while (0)
-
-// CL = true: clusters of TWO CTAs along M.  Both CTAs of a pair work on the same 128-column tile of the output for two
-// adjacent 128-row panels, so they need the same weight k-blocks: rank 0 fetches W_hi, rank 1 fetches W_lo, and each TMA
-// load is MULTICAST into both CTAs' rings -- an SM ingests half the weight bytes per tile (the kernel is bound by the
-// L2 -> SM fabric: ncu shows ~750 MB through the crossbar at 7.4-8.8 TB/s for both FFN GEMMs,
-// profiles/r2_gemm_f16x3_ffn{1,2}_ncu_full.txt).  A ring stage is refilled only when the MMAs of BOTH CTAs have released it
-// (tcgen05.commit multicast onto both `empty` barriers, count 2).
-// EW = epilogue warps: 4 (warps 12..15, all four 32-column blocks of a tile, two alternating store boxes) or 8 (warps 12..19:
-// group 0 = column blocks 0,1, group 1 = column blocks 2,3, one store box per group).  The trace of the EW = 4 kernel at K = 256
-// (profiles/r2_gemm_f16x3_trace_epilogue_detail2.txt) shows ~6500 clk of epilogue per tile against ~4600 clk of main loop: the
-// MMA warp waits for a drained accumulator at every tile boundary; two groups halve the epilogue's critical path.
-template <bool CL, int EW>
-__global__ void __launch_bounds__(384 + 32 * EW, 1)
-gemm_f16x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
-                  const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_c,
-                  const HGemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *boxes = smem + kHRingBytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kHRingBytes + kHOutBoxes);
-    uint64_t *tma_full = bars, *conv_full = bars + kHStages, *empty = bars + 2 * kHStages;
-    uint64_t *acc_full = bars + 3 * kHStages, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    float *sbias = reinterpret_cast<float *>(smem + kHRingBytes + kHOutBoxes + 256);  // 2 x 128 floats: this tile's bias slice
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nk = p.K / kHK;
-    const int n_tiles = (p.N + kHN - 1) / kHN, m_tiles = (p.M + kHM - 1) / kHM;
-    // tile walk: CL = false: tile t = blockIdx.x + i * gridDim.x over (m, n) row-major;
-    //            CL = true : pair p = cluster + i * #clusters over (m-pair, n); this CTA's panel = 2 * m-pair + rank
-    const uint32_t rank = CL ? cluster_ctarank() : 0u;
-    const int first = CL ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, step = CL ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    const int tiles = CL ? ((m_tiles + 1) / 2) * n_tiles : n_tiles * m_tiles;
-    auto tile_m0 = [&](int t) { return (CL ? 2 * (t / n_tiles) + (int)rank : t / n_tiles) * kHM; };
-    auto tile_n0 = [&](int t) { return (t % n_tiles) * kHN; };
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kHStages; ++s) {
-            mbar_init(tma_full + s, 1);
-            mbar_init(conv_full + s, 32 * kHConvWarps);
-            mbar_init(empty + s, CL ? 2 : 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(acc_full + b, 1);
-            mbar_init(acc_empty + b, 32 * EW);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (CL) cluster_sync_all();  // the peer's barriers are initialised before any multicast / remote arrive can reach them
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int tile = first; tile < tiles; tile += step) {
-                const int m0 = tile_m0(tile), n0 = tile_n0(tile);
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % kHStages;
-                    mbar_wait(empty + s, ((it / kHStages) & 1) ^ 1);  // CL: released by the MMA warps of BOTH CTAs
-                    HTRACE(0, it);  // producer: stage free, issuing TMA
-                    uint8_t *st = smem + s * kHStageBytes;
-                    mbar_expect_tx(tma_full + s, 4 * kHBox);          // own A boxes + W_hi + W_lo (CL: one of them from the peer)
-                    tma_load_2d(&map_a, tma_full + s, st, kb * kHK, m0);
-                    tma_load_2d(&map_a, tma_full + s, st + kHBox, kb * kHK + 32, m0);
-                    if (!CL) {
-                        tma_load_2d(&map_whi, tma_full + s, st + 2 * kHBox, kb * kHK, n0);
-                        tma_load_2d(&map_wlo, tma_full + s, st + 3 * kHBox, kb * kHK, n0);
-                    } else if (rank == 0) {
-                        tma_load_2d_mc(&map_whi, tma_full + s, st + 2 * kHBox, kb * kHK, n0, 0b11);
-                    } else {
-                        tma_load_2d_mc(&map_wlo, tma_full + s, st + 3 * kHBox, kb * kHK, n0, 0b11);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            uint32_t it = 0, tc = 0;
-            for (int tile = first; tile < tiles; tile += step, ++tc) {
-                const uint32_t buf = tc & 1;
-                mbar_wait(acc_empty + buf, ((tc >> 1) & 1) ^ 1);  // the epilogue has drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc = tmem_base + buf * 128u;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % kHStages;
-                    mbar_wait(conv_full + s, (it / kHStages) & 1);
-                    HTRACE(3, it);  // MMA: operands ready, issuing
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t base = smem_u32(smem + s * kHStageBytes);
-                    const uint32_t a_hi = tmem_base + 256u + 64u * (uint32_t)s, a_lo = a_hi + 32u;
-                    const uint64_t d_hi = umma_desc(base + 2 * kHBox), d_lo = umma_desc(base + 3 * kHBox);
-#pragma unroll
-                    for (int k = 0; k < kHK / 16; ++k) {  // UMMA_K = 16 halves = 32 bytes = 2 sixteen-byte units, 8 TMEM columns
-                        umma_f16_ts(acc, a_hi + 8u * k, d_hi + 2 * k, kIdescF16, (kb | k) != 0);
-                        umma_f16_ts(acc, a_hi + 8u * k, d_lo + 2 * k, kIdescF16, 1);
-                        umma_f16_ts(acc, a_lo + 8u * k, d_hi + 2 * k, kIdescF16, 1);
-                    }
-                    if (CL) umma_commit_mc(empty + s, 0b11);  // stage reusable (in both CTAs) once these MMAs have read it
-                    else umma_commit(empty + s);
-                }
-                umma_commit(acc_full + buf);
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ===== converters: landed fp32 A boxes -> scaled, split, packed f16x2 -> TMEM slot =====
-        const int q = warp & 3, half = (warp - 4) >> 2, r_in = q * 32 + lane;
-        const float ascale = p.a_scale_dev ? __ldg(p.a_scale_dev) : kActScale;
-        uint32_t it = 0;
-        for (int tile = first; tile < tiles; tile += step) {
-            for (int kb = 0; kb < nk; ++kb, ++it) {
-                const int s = it % kHStages;
-                mbar_wait(tma_full + s, (it / kHStages) & 1);
-                if (threadIdx.x == 128) HTRACE(1, it);  // converter: TMA landed
-                const uint8_t *arow = smem + s * kHStageBytes + half * kHBox + r_in * 128;
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {  // logical 16-byte chunk c of this row sits at physical chunk c ^ (row & 7)
-                    float4 x = *reinterpret_cast<const float4 *>(arow + ((c ^ (r_in & 7)) << 4));
-                    if (p.act == 1) {
-                        x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                    } else if (p.act == 2) {
-                        x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                    }
-                    split2(x.x * ascale, x.y * ascale, hi[2 * c], lo[2 * c]);
-                    split2(x.z * ascale, x.w * ascale, hi[2 * c + 1], lo[2 * c + 1]);
-                }
-                const uint32_t slot = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + 64u * (uint32_t)s + 16u * (uint32_t)half;
-                tmem_st16u(slot, hi);
-                tmem_st16u(slot + 32u, lo);
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(conv_full + s);
-                if (threadIdx.x == 128) HTRACE(2, it);  // converter: done
-            }
-        }
-    } else if (warp >= 12) {
-        // ===== epilogue: TMEM -> registers -> * 2^-(4+s) + bias -> swizzled box -> TMA store (or direct stores) =====
-        // (a warp-private transpose box + coalesced 128-bit global stores instead of the shared boxes / TMA stores was measured
-        //  13 % slower over the projection shapes, profiles/r2_gemm_shapes_f16x3_warp_epilogue.txt: kept out)
-        const int q = warp & 3, r_in = q * 32 + lane;
-        const int grp = (warp - 12) >> 2;                                  // 0 (EW = 4) or 0 / 1 (EW = 8)
-        const bool elected = threadIdx.x == (12 + 4 * grp) * 32;           // one store-issuing thread per group
-        const bool tracer = threadIdx.x == 12 * 32;
-        constexpr int kBlocksPerGroup = (kHN / 32) / (EW / 4);
-        const int c_begin = grp * kBlocksPerGroup, c_end = c_begin + kBlocksPerGroup;
-        const float sc = p.a_scale_dev ? 1.f / (__ldg(p.a_scale_dev) * __ldg(p.w_scale_dev)) : p.out_scale;
-        uint32_t tc = 0, box_it = 0;
-        uint8_t *wbox = boxes + (warp - 12) * 4096;  // epilogue variant 1: this warp's private 32-row x 128-byte box
-        const int et = threadIdx.x - 12 * 32;        // 0 .. 32 * EW - 1 within the epilogue warps
-        for (int tile = first; tile < tiles; tile += step, ++tc) {
-            const int m0 = tile_m0(tile), n0 = tile_n0(tile);
-            const uint32_t buf = tc & 1;
-            // The tile's bias slice goes through shared memory: fetched while the accumulator is still being computed.  (Trace,
-            // profiles/r2_gemm_f16x3_trace_epilogue_detail.txt: eight dependent global bias loads per 32-column block made the
-            // "write box" phase 1000-2400 clk and the whole epilogue ~7000 clk per tile against ~4800 clk of main loop at K = 256.)
-            const float bval = (et < 128 && p.bias && n0 + et < p.N) ? __ldg(p.bias + n0 + et) : 0.f;
-            mbar_wait(acc_full + buf, (tc >> 1) & 1);
-            if (tracer) HTRACE(5, tc);  // epilogue: accumulator complete
-            float *tb = sbias + buf * 128;
-            if (et < 128) tb[et] = bval;
-            named_bar_sync(3, 32 * EW);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int row = m0 + r_in;
-#pragma unroll 1
-            for (int c = c_begin; c < c_end; ++c) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 128u + (uint32_t)(c * 32), r);
-                if (tracer) HTRACE(7, tc * 4 + c);  // epilogue detail: TMEM load done
-                if (c == c_end - 1) {  // this warp's last read of the accumulator: hand it back to the MMA warp
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    mbar_arrive(acc_empty + buf);
-                }
-                const int col0 = n0 + c * 32;
-                if (col0 >= p.N) continue;  // uniform across the CTA
-                if (p.use_tma_store && p.epilogue == 1) {  // warp-private transpose box + coalesced 128-bit global stores
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 bv = *reinterpret_cast<const float4 *>(tb + c * 32 + j);
-                        const float4 o = make_float4(fmaf(__uint_as_float(r[j]), sc, bv.x), fmaf(__uint_as_float(r[j + 1]), sc, bv.y),
-                                                     fmaf(__uint_as_float(r[j + 2]), sc, bv.z), fmaf(__uint_as_float(r[j + 3]), sc, bv.w));
-                        *reinterpret_cast<float4 *>(wbox + lane * 128 + (((j >> 2) ^ (lane & 7)) << 4)) = o;
-                    }
-                    __syncwarp();
-                    const int ch = lane & 7, gcol = col0 + 4 * ch;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int rr = 4 * i + (lane >> 3), grow = m0 + q * 32 + rr;
-                        const float4 v = *reinterpret_cast<const float4 *>(wbox + rr * 128 + ((ch ^ (rr & 7)) << 4));
-                        if (grow < p.M) {
-                            float *dst = p.C + (int64_t)grow * p.ldc + gcol;
-                            if (gcol + 3 < p.N) {
-                                st_stream_f4(dst, v);
-                            } else {
-                                if (gcol < p.N) dst[0] = v.x;
-                                if (gcol + 1 < p.N) dst[1] = v.y;
-                                if (gcol + 2 < p.N) dst[2] = v.z;
-                            }
-                        }
-                    }
-                    __syncwarp();  // the box is rewritten by the next column block
-                } else if (p.use_tma_store) {
-                    // the two staging boxes alternate per ISSUED store (a skipped column block must not advance the counter)
-                    uint8_t *box = boxes + (EW == 8 ? grp : (int)(box_it++ & 1)) * kHBox;
-                    if (elected) {  // box free again (EW = 8: one box per group, so its previous store must have been read out)
-                        if (EW == 8) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                        else asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                    }
-                    named_bar_sync(1 + grp, 128);
-                    if (tracer) HTRACE(8, tc * 4 + c);  // box free + barrier
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 bv = *reinterpret_cast<const float4 *>(tb + c * 32 + j);  // zero beyond N / without bias
-                        const float4 o = make_float4(fmaf(__uint_as_float(r[j]), sc, bv.x), fmaf(__uint_as_float(r[j + 1]), sc, bv.y),
-                                                     fmaf(__uint_as_float(r[j + 2]), sc, bv.z), fmaf(__uint_as_float(r[j + 3]), sc, bv.w));
-                        *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    named_bar_sync(1 + grp, 128);
-                    if (tracer) HTRACE(9, tc * 4 + c);  // box written + barrier
-                    if (elected) {
-                        tma_store_2d(&map_c, box, col0, m0);  // clips rows >= M and columns >= N
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
-                } else if (row < p.M) {
-                    float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (col0 + j < p.N) crow[col0 + j] = fmaf(__uint_as_float(r[j]), sc, tb[c * 32 + j]);
-                }
-            }
-            if (tracer) HTRACE(6, tc);  // epilogue: tile handed to the store engine
-        }
-        if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (CL) cluster_sync_all();  // the peer may still multicast into / arrive on this CTA's shared memory until it is done too
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
-
-// ---- "AS": activation-stationary variant for K <= 256 ---------------------------------------------------------------------
-// The streaming kernel above re-reads the activation panel for every 128-column tile of the output, and its time follows
-// the L2 -> SM traffic, not the tensor pipe: FFN-1 at layer 0 (22726 x 256 -> 2048) moves 16 x 23 MB of A, 364 MB of W and
-// 186 MB of C = 922 MB and takes 98 us, i.e. the ~9 TB/s the L2 sustains (148 SMs x ~42 B/clk, B300_MICROARCH.md "LTS
-// throughput cap"); the MMAs alone would need 30 us.  With K <= 256 the whole split activation panel of a 128-row block fits
-// in tensor memory (4 k-blocks x 64 columns = 256 columns, beside the double-buffered 2 x 128-column accumulator), so here a
-// CTA converts a panel ONCE and walks a group of up to G output tiles of that panel; per tile only the weight streams in
-// (32 KB per k-block instead of 64 KB) and the converter warps are idle instead of re-splitting the same rows.
-//   work unit  = (128-row panel, group of G consecutive 128-column tiles), units strided over the persistent CTAs;
-//   shared memory: A ring 2 x 32 KB (two fp32 boxes per k-block), W ring 4 x 32 KB (W_hi + W_lo tile), 2 store boxes;
-//   warp 0: W producer, warp 3: A producer (its own thread, so the next panel is prefetched while W streams),
-//   warp 1: MMA issuer, warps 4..11: converters (panel k-block j is rewritten as soon as the LAST tile's MMAs on k-block j
-//   have completed: per-k-block `panel_free` commits), warps 12..15: epilogue (as above).
-constexpr int kASlots = 2, kWSlots = 4;
-constexpr int kSlotBytes = 2 * kHBox;                                   // 32 KB
-constexpr int kAsRingBytes = (kASlots + kWSlots) * kSlotBytes;          // 192 KB
-constexpr int kAsSmem = kAsRingBytes + kHOutBoxes + 1024 + 256;
-constexpr int kMaxKb = 4;
-
-__global__ void __launch_bounds__(kHThreads, 1)
-gemm_f16x3_as_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
-                     const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_c,
-                     const HGemmParams p, const int group /* tiles per unit */) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *a_ring = smem, *w_ring = smem + kASlots * kSlotBytes;
-    uint8_t *boxes = smem + kAsRingBytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kAsRingBytes + kHOutBoxes);
-    uint64_t *a_full = bars, *a_empty = a_full + kASlots, *w_full = a_empty + kASlots, *w_empty = w_full + kWSlots;
-    uint64_t *panel_full = w_empty + kWSlots, *panel_free = panel_full + kMaxKb;
-    uint64_t *acc_full = panel_free + kMaxKb, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nk = p.K / kHK;  // 1..4
-    const int n_tiles = (p.N + kHN - 1) / kHN, m_tiles = (p.M + kHM - 1) / kHM;
-    const int n_groups = (n_tiles + group - 1) / group;
-    const int units = m_tiles * n_groups;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kASlots; ++s) mbar_init(a_full + s, 1), mbar_init(a_empty + s, 32 * kHConvWarps);
-        for (int s = 0; s < kWSlots; ++s) mbar_init(w_full + s, 1), mbar_init(w_empty + s, 1);
-        for (int j = 0; j < kMaxKb; ++j) mbar_init(panel_full + j, 32 * kHConvWarps), mbar_init(panel_free + j, 1);
-        for (int b = 0; b < 2; ++b) mbar_init(acc_full + b, 1), mbar_init(acc_empty + b, 128);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== W producer =====
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                const int t0 = (u % n_groups) * group, t1 = min(n_tiles, t0 + group);
-                for (int t = t0; t < t1; ++t)
-                    for (int kb = 0; kb < nk; ++kb, ++it) {
-                        const int s = it % kWSlots;
-                        mbar_wait(w_empty + s, ((it / kWSlots) & 1) ^ 1);
-                        uint8_t *st = w_ring + s * kSlotBytes;
-                        mbar_expect_tx(w_full + s, kSlotBytes);
-                        tma_load_2d(&map_whi, w_full + s, st, kb * kHK, t * kHN);
-                        tma_load_2d(&map_wlo, w_full + s, st + kHBox, kb * kHK, t * kHN);
-                    }
-            }
-        }
-    } else if (warp == 3) {
-        // ===== A producer =====
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                const int m0 = (u / n_groups) * kHM;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % kASlots;
-                    mbar_wait(a_empty + s, ((it / kASlots) & 1) ^ 1);
-                    uint8_t *st = a_ring + s * kSlotBytes;
-                    mbar_expect_tx(a_full + s, kSlotBytes);
-                    tma_load_2d(&map_a, a_full + s, st, kb * kHK, m0);
-                    tma_load_2d(&map_a, a_full + s, st + kHBox, kb * kHK + 32, m0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            uint32_t wit = 0, tc = 0, uc = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x, ++uc) {
-                const int t0 = (u % n_groups) * group, t1 = min(n_tiles, t0 + group);
-                for (int t = t0; t < t1; ++t, ++tc) {
-                    const uint32_t buf = tc & 1;
-                    mbar_wait(acc_empty + buf, ((tc >> 1) & 1) ^ 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t acc = tmem_base + buf * 128u;
-                    for (int kb = 0; kb < nk; ++kb, ++wit) {
-                        if (t == t0) mbar_wait(panel_full + kb, uc & 1);  // this unit's panel k-block has been converted
-                        const int s = wit % kWSlots;
-                        mbar_wait(w_full + s, (wit / kWSlots) & 1);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t base = smem_u32(w_ring + s * kSlotBytes);
-                        const uint32_t a_hi = tmem_base + 256u + 64u * (uint32_t)kb, a_lo = a_hi + 32u;
-                        const uint64_t d_hi = umma_desc(base), d_lo = umma_desc(base + kHBox);
-#pragma unroll
-                        for (int k = 0; k < kHK / 16; ++k) {
-                            umma_f16_ts(acc, a_hi + 8u * k, d_hi + 2 * k, kIdescF16, (kb | k) != 0);
-                            umma_f16_ts(acc, a_hi + 8u * k, d_lo + 2 * k, kIdescF16, 1);
-                            umma_f16_ts(acc, a_lo + 8u * k, d_hi + 2 * k, kIdescF16, 1);
-                        }
-                        umma_commit(w_empty + s);
-                        if (t == t1 - 1) umma_commit(panel_free + kb);  // last reader of panel k-block kb in this unit
-                    }
-                    umma_commit(acc_full + buf);
-                }
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ===== converters: one panel per unit =====
-        const int q = warp & 3, half = (warp - 4) >> 2, r_in = q * 32 + lane;
-        uint32_t it = 0, uc = 0;
-        for (int u = blockIdx.x; u < units; u += gridDim.x, ++uc) {
-            for (int kb = 0; kb < nk; ++kb, ++it) {
-                const int s = it % kASlots;
-                mbar_wait(a_full + s, (it / kASlots) & 1);
-                const uint8_t *arow = a_ring + s * kSlotBytes + half * kHBox + r_in * 128;
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    float4 x = *reinterpret_cast<const float4 *>(arow + ((c ^ (r_in & 7)) << 4));
-                    if (p.act == 1) {
-                        x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                    } else if (p.act == 2) {
-                        x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                    }
-                    split2(x.x * kActScale, x.y * kActScale, hi[2 * c], lo[2 * c]);
-                    split2(x.z * kActScale, x.w * kActScale, hi[2 * c + 1], lo[2 * c + 1]);
-                }
-                mbar_arrive(a_empty + s);                      // the fp32 boxes are in registers: the slot may be refilled
-                mbar_wait(panel_free + kb, (uc & 1) ^ 1);      // the previous unit's MMAs no longer read this k-block
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t slot = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + 64u * (uint32_t)kb + 16u * (uint32_t)half;
-                tmem_st16u(slot, hi);
-                tmem_st16u(slot + 32u, lo);
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(panel_full + kb);
-            }
-        }
-    } else if (warp >= 12) {
-        // ===== epilogue (same as the streaming kernel, tiles in the MMA warp's order) =====
-        const int q = warp & 3, r_in = q * 32 + lane;
-        const bool elected = threadIdx.x == 12 * 32;
-        const float sc = p.out_scale;
-        uint32_t tc = 0, box_it = 0;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            const int m0 = (u / n_groups) * kHM;
-            const int t0 = (u % n_groups) * group, t1 = min(n_tiles, t0 + group);
-            for (int t = t0; t < t1; ++t, ++tc) {
-                const int n0 = t * kHN;
-                const uint32_t buf = tc & 1;
-                mbar_wait(acc_full + buf, (tc >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const int row = m0 + r_in;
-#pragma unroll 1
-                for (int c = 0; c < kHN / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 128u + (uint32_t)(c * 32), r);
-                    if (c == kHN / 32 - 1) {
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                        mbar_arrive(acc_empty + buf);
-                    }
-                    const int col0 = n0 + c * 32;
-                    if (col0 >= p.N) continue;
-                    if (p.use_tma_store) {
-                        uint8_t *box = boxes + (box_it++ & 1) * kHBox;
-                        if (elected) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                        named_bar_sync(1, 128);
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            float4 o = make_float4(__uint_as_float(r[j]) * sc, __uint_as_float(r[j + 1]) * sc,
-                                                   __uint_as_float(r[j + 2]) * sc, __uint_as_float(r[j + 3]) * sc);
-                            if (p.bias && col0 + j + 3 < p.N) {
-                                const float4 bv = ldg_f4(p.bias + col0 + j);
-                                o.x += bv.x, o.y += bv.y, o.z += bv.z, o.w += bv.w;
-                            } else if (p.bias) {
-                                if (col0 + j < p.N) o.x += __ldg(p.bias + col0 + j);
-                                if (col0 + j + 1 < p.N) o.y += __ldg(p.bias + col0 + j + 1);
-                                if (col0 + j + 2 < p.N) o.z += __ldg(p.bias + col0 + j + 2);
-                            }
-                            *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                        }
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                        named_bar_sync(1, 128);
-                        if (elected) {
-                            tma_store_2d(&map_c, box, col0, m0);
-                            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                        }
-                    } else if (row < p.M) {
-                        float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (col0 + j < p.N) crow[col0 + j] = __uint_as_float(r[j]) * sc + (p.bias ? __ldg(p.bias + col0 + j) : 0.f);
-                    }
-                }
-            }
-        }
-        if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
 
 // weight split: (N,K) fp32 -> W_hi = fp16(scale * W), W_lo = fp16(scale * W - W_hi)   (scale: a power of two)
 __global__ void split_f16_pair_kernel(const float *__restrict__ w, int64_t n, float scale, __half *__restrict__ hi,
@@ -549,56 +39,6 @@ __global__ void split_f16_pair_kernel(const float *__restrict__ w, int64_t n, fl
 
 using namespace sdetr;
 
-static std::atomic<int> g_f16_cluster{0};  // 1: clusters of two CTAs share the weight k-blocks by TMA multicast (M >= 2 panels).
-// Measured (profiles/r2_gemm_shapes_f16x3_cluster.txt): bit-identical, but 3-12 % SLOWER on every shape -- the stage-by-stage
-// lockstep of the two CTAs costs more than the halved weight ingest saves -- so off by default.
-static std::atomic<long long *> g_f16_dbg{nullptr};
-static std::atomic<int> g_f16_epi{0};
-static std::atomic<int> g_f16_ew{4};  // epilogue warps of the streaming kernel: 4 or 8 (measured equal: one store box per group waits ~1200 clk for its TMA store to drain)
-static std::atomic<int> g_f16_as{0};  // 1: K <= 256 goes to the activation-stationary kernel (measured: +4 % on FFN-1, -3 % on the 6-layer value projection -- profiles/r2_gemm_shapes_f16x3_as.txt -- so off by default)
-
-extern "C" int sdetr_gemm_f16x3_set_cluster(int enable) {
-    g_f16_cluster = enable ? 1 : 0;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_gemm_f16x3_set_trace(long long *device_buffer /* 10 * 256 int64, or NULL */) {
-    g_f16_dbg = device_buffer;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_gemm_f16x3_set_epilogue(int variant) {
-    SDETR_REQUIRE(variant == 0 || variant == 1, SDETR_ERR_INVALID_ARG, "gemm_f16x3_set_epilogue: 0 or 1");
-    g_f16_epi = variant;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_gemm_f16x3_set_epilogue_warps(int warps) {
-    SDETR_REQUIRE(warps == 4 || warps == 8, SDETR_ERR_INVALID_ARG, "gemm_f16x3_set_epilogue_warps: 4 or 8");
-    g_f16_ew = warps;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_gemm_f16x3_set_as(int enable) {
-    g_f16_as = enable ? 1 : 0;
-    return SDETR_OK;
-}
-
-// tiles per work unit: the largest group whose units fill whole waves of `sms` CTAs well (>= 85 %), else the best filling
-static int pick_group(int m_tiles, int n_tiles, int sms) {
-    int best = 1;
-    double best_eff = 0.0;
-    for (int g = n_tiles; g >= 1; g = (g > 1 ? (g + 1) / 2 : 0)) {
-        const long long units = (long long)m_tiles * ((n_tiles + g - 1) / g);
-        const long long waves = (units + sms - 1) / sms;
-        const double eff = (double)units / (double)(waves * sms);
-        if (eff >= 0.85) return g;
-        if (eff > best_eff) best_eff = eff, best = g;
-        if (g == 1) break;
-    }
-    return best;
-}
-
 extern "C" int sdetr_split_f16_pair(const float *w, int64_t count, float scale, void *w_hi, void *w_lo, sdetr_stream_t stream) {
     SDETR_REQUIRE(w && w_hi && w_lo, SDETR_ERR_INVALID_ARG, "split_f16_pair: null pointer");
     SDETR_REQUIRE(scale > 0.f, SDETR_ERR_INVALID_ARG, "split_f16_pair: scale must be positive (a power of two)");
@@ -613,56 +53,20 @@ static int gemm_f16x3_impl(const float *A, int64_t lda, const void *W_hi, const 
                            const float *bias, float *C, int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream) {
     SDETR_REQUIRE(A && W_hi && W_lo && C, SDETR_ERR_INVALID_ARG, "gemm_f16x3_pre: null pointer");
     SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2, SDETR_ERR_INVALID_ARG, "gemm_f16x3_pre: bad sizes / activation");
-    SDETR_REQUIRE(K % kHK == 0, SDETR_ERR_UNSUPPORTED, "gemm_f16x3_pre: K=%d must be a multiple of %d", K, kHK);
+    SDETR_REQUIRE(K % Gemm3xShape<true>::kK == 0, SDETR_ERR_UNSUPPORTED, "gemm_f16x3_pre: K=%d must be a multiple of %d", K,
+                  Gemm3xShape<true>::kK);
     SDETR_REQUIRE(w_scale > 0.f, SDETR_ERR_INVALID_ARG, "gemm_f16x3_pre: weight scale must be positive");
     SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && aligned16(W_lo) && lda >= K && ldc >= N,
                   SDETR_ERR_INVALID_ARG, "gemm_f16x3_pre: operands must be 16-byte aligned with 16-byte row pitch");
     if (M == 0) return SDETR_OK;
-    CUtensorMap ma, mh, ml, mc;
-    SDETR_REQUIRE(make_map_2d(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, A, M, K, lda, 32, kHM) &&
-                      make_map_2d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_hi, N, K, K, kHK, kHN) &&
-                      make_map_2d(&ml, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_lo, N, K, K, kHK, kHN),
+    CUtensorMap mh, ml;
+    SDETR_REQUIRE(make_map_2d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_hi, N, K, K, 64, kGN) &&
+                      make_map_2d(&ml, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_lo, N, K, K, 64, kGN),
                   SDETR_ERR_CUDA, "gemm_f16x3_pre: cuTensorMapEncodeTiled failed");
-    const int use_tma_store = (ldc % 4 == 0) && aligned16(C) &&
-                              make_map_2d(&mc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, C, M, N, ldc, 32, kHM);
-    if (!use_tma_store) mc = ma;
-    static PerDeviceOnce once, once_as;
-    static PerDeviceOnce once_cl, once_8;
-    SDETR_OPT_IN_SMEM(once, (gemm_f16x3_kernel<false, 4>), kHSmem, "gemm_f16x3_pre");
-    SDETR_OPT_IN_SMEM(once_8, (gemm_f16x3_kernel<false, 8>), kHSmem, "gemm_f16x3_pre");
-    SDETR_OPT_IN_SMEM(once_cl, (gemm_f16x3_kernel<true, 4>), kHSmem, "gemm_f16x3_pre");
-    SDETR_OPT_IN_SMEM(once_as, gemm_f16x3_as_kernel, kAsSmem, "gemm_f16x3_pre");
-    const int sms = persistent_ctas();
-    HGemmParams p{bias, C, ldc, M, N, K, act, use_tma_store, 1.f / (kActScale * w_scale), a_scale_dev, w_scale_dev, g_f16_epi.load(), g_f16_dbg.load()};
-    const int n_tiles = (N + kHN - 1) / kHN, m_tiles = (M + kHM - 1) / kHM;
-    const int group = (g_f16_as.load() && !a_scale_dev && K <= kMaxKb * kHK) ? pick_group(m_tiles, n_tiles, sms) : 1;  // (the AS variant has the fixed activation scale only)
-    if (group >= 2) {  // a one-tile unit re-uses nothing: the streaming kernel pipelines it better
-        const long long units = (long long)m_tiles * ((n_tiles + group - 1) / group);
-        gemm_f16x3_as_kernel<<<(int)(units < sms ? units : sms), kHThreads, kAsSmem, (cudaStream_t)stream>>>(ma, mh, ml, mc, p, group);
-        return check_launch("gemm_f16x3_pre/as");
-    }
-    if (g_f16_cluster.load() && m_tiles >= 2) {
-        const int pairs = ((m_tiles + 1) / 2) * n_tiles, max_clusters = sms / 2;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(2 * (pairs < max_clusters ? pairs : max_clusters));
-        cfg.blockDim = dim3(kHThreads);
-        cfg.dynamicSmemBytes = kHSmem;
-        cfg.stream = (cudaStream_t)stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
-        cfg.attrs = at, cfg.numAttrs = 1;
-        const cudaError_t le = cudaLaunchKernelEx(&cfg, gemm_f16x3_kernel<true, 4>, ma, mh, ml, mc, p);
-        SDETR_REQUIRE(le == cudaSuccess, SDETR_ERR_CUDA, "gemm_f16x3_pre: cluster launch: %s", cudaGetErrorString(le));
-        return check_launch("gemm_f16x3_pre/cluster");
-    }
-    const int tiles = n_tiles * m_tiles;
-    if (g_f16_ew.load() == 8 && p.epilogue == 0)
-        gemm_f16x3_kernel<false, 8><<<tiles < sms ? tiles : sms, 384 + 32 * 8, kHSmem, (cudaStream_t)stream>>>(ma, mh, ml, mc, p);
-    else
-        gemm_f16x3_kernel<false, 4><<<tiles < sms ? tiles : sms, kHThreads, kHSmem, (cudaStream_t)stream>>>(ma, mh, ml, mc, p);
-    return check_launch("gemm_f16x3_pre");
+    const Gemm3xParams p{bias, C, ldc, M, N, K, act, kActScale, 1.f / (kActScale * w_scale), a_scale_dev, w_scale_dev};
+    return launch_gemm3x<true, false>(A, lda, mh, ml, p, stream, "gemm_f16x3_pre");
 }
+
 
 extern "C" int sdetr_gemm_f16x3_pre(const float *A, int64_t lda, const void *W_hi, const void *W_lo, float w_scale,
                                     const float *bias, float *C, int64_t ldc, int M, int N, int K, int act,

@@ -1,786 +1,18 @@
-// Dense projection GEMM of the path on the 5th-generation tensor cores -- sdetr_gemm_3xtf32.
+// Dense projection GEMM of the path, TF32 form -- sdetr_gemm_3xtf32 / _pre / _raw.
 //
 //   C[M,N] = act(A)[M,K] . W[N,K]^T + bias        fp32 in / fp32 out, fp32-class accuracy ("3xTF32")
 //
 // These are the only true dense GEMMs of the path (models/bricks/ms_deform_attn.py:316,322-328,375 value / offset /
 // weight / output projections; salience_transformer.py:347-351 FFN; :462 class head; :16-47 MaskPredictor;
-// base_transformer.py:111 enc_output).  Hand-written for sm_100a:
-//
-//   * operands move with TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) into a 3-stage shared-memory ring;
-//   * the weight arrives pre-split (W_hi = tf32(W), W_lo = tf32(W - W_hi), cached per parameter); the activation is
-//     split IN the kernel: four converter warps rewrite each landed A tile in place as A_hi and write A_lo next to
-//     it (element-wise, so the TMA swizzle is preserved) -- no extra HBM pass, optional ReLU fused in;
-//   * one elected thread issues tcgen05.mma.kind::tf32 (M=128, N=128, K=8): A_hi.W_hi + A_hi.W_lo + A_lo.W_hi into
-//     ONE fp32 accumulator tile in tensor memory (128 lanes x 128 columns);
-//   * tcgen05.commit signals stage release / accumulator ready through mbarriers; the converter warps then become
-//     the epilogue: tcgen05.ld (32 lanes x 32 columns per warp and step) -> + bias -> 128-bit global stores.
-//
-//   * CTAs run as clusters of two along M: both need the same W k-block, so rank 0 fetches W_hi and rank 1 fetches
-//     W_lo and each TMA load is MULTICAST into both CTAs' rings (the kernel is bound by L2->SM bandwidth: this cuts
-//     a CTA's traffic per k-block from 48 KB to 32 KB).  A ring stage is refilled only when the MMAs of BOTH CTAs
-//     have released it (tcgen05.commit multicast onto both `empty` barriers).
-//
-// Warp roles (384 threads): 0 = TMA producer, 1 = MMA issuer, 2 = TMEM allocator, 3 = idle, 4..11 = convert + epilogue.
-#include "umma.cuh"
+// base_transformer.py:111 enc_output).  The kernel is gemm3x_kernel<false, *> of wgmma.cuh: k-blocks of 32 fp32 (one
+// 128-byte swizzled row), stage = A box + W_hi + W_lo (48 KB, four stages); the activation is split into TF32 pieces in
+// registers (x = hi + lo, hi = tf32(x), lo = tf32(x - hi), optional ReLU / GELU fused in) and each warpgroup issues
+// 4 k-steps x {lo.hi, hi.lo, hi.hi} = 12 wgmma m64n128k8 .tf32 per k-block.  The weight arrives pre-split
+// (sdetr_split_tf32_pair, cached by the caller per parameter) or raw (sdetr_gemm_3xtf32_raw: the consumer warpgroups split
+// the landed W tile in place with the same arithmetic, so both forms give bit-identical results).
+#include "wgmma.cuh"
 
 namespace sdetr {
-
-constexpr int kBM = 128, kBN = 128, kBK = 32;       // tile (fp32 elements); kBK * 4 B = one 128-byte swizzle row
-constexpr int kStages = 4;                          // TMA ring: covers ~2.7k cycles of L2->smem latency
-constexpr int kLoSlots = 2;                         // A_lo ring (written by the converters, read by the MMAs)
-constexpr int kTileBytes = kBM * kBK * 4;           // 16 KB (A and W tiles have the same footprint: kBM == kBN)
-constexpr int kStageBytes = 3 * kTileBytes;         // A (raw -> hi in place), W_hi, W_lo
-constexpr int kConvWarps = 8;
-constexpr int kGemmThreads = 128 + 32 * kConvWarps; // warps 0..3: producer / MMA / TMEM / idle; 4..11: convert + epilogue
-constexpr int kTmemCols = 128;
-constexpr int kRingBytes = kStages * kStageBytes + kLoSlots * kTileBytes;  // 224 KB
-constexpr int kGemmSmem = kRingBytes + 1024 /* alignment slack */ + 256 /* barriers */;
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=tf32, both K-major, N=128, M=128
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kBN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-
-// tf32 rounding (nearest, ties away from zero) with two ALU ops -- same result as cvt.rna.tf32.f32 for finite inputs
-__device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
-
-struct GemmParams {
-    const float *bias;
-    float *C;
-    int64_t ldc;
-    int M, N, K, relu_a, use_tma_store;
-    long long *dbg;  // optional per-event clock64() trace of CTA (0,0): [role][kb] (tools/gemm_trace.py)
-};
-#define SDETR_TRACE(role, kb)                                                             \
-    do {                                                                                  \
-        if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0) p.dbg[(role) * 128 + (kb)] = clock64(); \
-    } while (0)
-
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_3xtf32_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
-                   const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_c,
-                   const GemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *lo_ring = smem + kStages * kStageBytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kRingBytes);
-    uint64_t *tma_full = bars, *conv_full = bars + kStages, *empty = bars + 2 * kStages;
-    uint64_t *lo_empty = bars + 3 * kStages, *acc_full = lo_empty + kLoSlots;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * kBN, m0 = blockIdx.y * kBM;
-    const int nk = p.K / kBK;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
-            mbar_init(tma_full + s, 1);
-            mbar_init(conv_full + s, 32 * kConvWarps);
-            mbar_init(empty + s, 2);  // released by the MMA warps of BOTH CTAs of the cluster
-        }
-        for (int s = 0; s < kLoSlots; ++s) mbar_init(lo_empty + s, 1);
-        mbar_init(acc_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(kTmemCols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();  // the peer's barriers are initialised before any multicast / remote arrive can reach them
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_acc = *tmem_slot;
-    const uint32_t rank = cluster_ctarank();
-    if (threadIdx.x == 0) SDETR_TRACE(5, 2);  // setup done
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kStages;
-                const uint32_t ph = (kb / kStages) & 1;
-                mbar_wait(empty + s, ph ^ 1);
-                SDETR_TRACE(0, kb);  // producer: stage free, issuing TMA
-                uint8_t *st = smem + s * kStageBytes;
-                mbar_expect_tx(tma_full + s, 3 * kTileBytes);  // own A + W_hi + W_lo (one of them arrives from the peer)
-                tma_load_2d(&map_a, tma_full + s, st, kb * kBK, m0);
-                if (rank == 0) tma_load_2d_mc(&map_whi, tma_full + s, st + kTileBytes, kb * kBK, n0, 0b11);
-                else tma_load_2d_mc(&map_wlo, tma_full + s, st + 2 * kTileBytes, kb * kBK, n0, 0b11);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kStages, ls = kb % kLoSlots;
-                const uint32_t ph = (kb / kStages) & 1;
-                mbar_wait(tma_full + s, ph);
-                SDETR_TRACE(1, kb);  // MMA: TMA landed
-                mbar_wait(conv_full + s, ph);
-                SDETR_TRACE(2, kb);  // MMA: converted, issuing
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t base = smem_u32(smem + s * kStageBytes);
-                const uint32_t lo_base = smem_u32(lo_ring + ls * kTileBytes);
-#pragma unroll
-                for (int k = 0; k < kBK / 8; ++k) {  // UMMA_K = 8 tf32 = 32 bytes = 2 sixteen-byte units
-                    const uint64_t a_hi = umma_desc(base) + 2 * k, a_lo = umma_desc(lo_base) + 2 * k;
-                    const uint64_t w_hi = umma_desc(base + kTileBytes) + 2 * k, w_lo = umma_desc(base + 2 * kTileBytes) + 2 * k;
-                    umma_tf32(tmem_acc, a_hi, w_hi, kIdesc, (kb | k) != 0);
-                    umma_tf32(tmem_acc, a_hi, w_lo, kIdesc, 1);
-                    umma_tf32(tmem_acc, a_lo, w_hi, kIdesc, 1);
-                }
-                umma_commit_mc(empty + s, 0b11);  // TMA stage reusable (in both CTAs) once these MMAs have read it
-                umma_commit(lo_empty + ls);   // ... and so is the A_lo slot
-            }
-            umma_commit(acc_full);            // accumulator complete
-        }
-    } else if (warp >= 4) {
-        // ===== converters: landed A tile -> A_hi (in place) + A_lo (ring) =====
-        const int t = threadIdx.x - 128;  // 0 .. 32*kConvWarps-1
-        constexpr int kPer = (kTileBytes / 16) / (32 * kConvWarps);  // 16-byte chunks per thread and stage
-        for (int kb = 0; kb < nk; ++kb) {
-            const int s = kb % kStages, ls = kb % kLoSlots;
-            const uint32_t ph = (kb / kStages) & 1, lph = (kb / kLoSlots) & 1;
-            mbar_wait(lo_empty + ls, lph ^ 1);  // A_lo slot released by the MMAs of k-block kb - kLoSlots
-            mbar_wait(tma_full + s, ph);
-            if (t == 0) SDETR_TRACE(3, kb);  // converter: start
-            float4 *a = reinterpret_cast<float4 *>(smem + s * kStageBytes);
-            float4 *alo = reinterpret_cast<float4 *>(lo_ring + ls * kTileBytes);
-            float4 v[kPer];
-#pragma unroll
-            for (int it = 0; it < kPer; ++it) v[it] = a[it * (32 * kConvWarps) + t];  // a quarter-warp = one 128-byte row
-#pragma unroll
-            for (int it = 0; it < kPer; ++it) {
-                float4 x = v[it];
-                if (p.relu_a == 1) {
-                    x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                } else if (p.relu_a == 2) {  // exact (erf) GELU, torch.nn.GELU default
-                    x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                }
-                float4 hi, lo;
-                hi.x = tf32_rn(x.x), hi.y = tf32_rn(x.y), hi.z = tf32_rn(x.z), hi.w = tf32_rn(x.w);
-                lo.x = tf32_rn(x.x - hi.x), lo.y = tf32_rn(x.y - hi.y), lo.z = tf32_rn(x.z - hi.z), lo.w = tf32_rn(x.w - hi.w);
-                a[it * (32 * kConvWarps) + t] = hi;
-                alo[it * (32 * kConvWarps) + t] = lo;
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA (async proxy)
-            mbar_arrive(conv_full + s);
-            if (t == 0) SDETR_TRACE(4, kb);  // converter: done
-        }
-        // ===== epilogue: TMEM -> registers -> (+bias) -> swizzled smem box -> TMA store (or direct stores) =====
-        mbar_wait(acc_full, 0);
-        if (t == 0) SDETR_TRACE(5, 0);  // epilogue start
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int q = warp & 3;                 // TMEM lane quadrant this warp may read
-        const int half = (warp - 4) >> 2;       // warps 4..7: column blocks 0,1; warps 8..11: column blocks 2,3
-        const int r_in = q * 32 + lane, row = m0 + r_in;
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {
-            const int c = half * 2 + cc;
-            uint32_t r[32];
-            tmem_ld32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-            const int col0 = n0 + c * 32;
-            if (p.use_tma_store) {
-                // all MMAs have completed (acc_full), so the TMA ring is free: box c lives at smem + c*16 KB,
-                // 128 rows x 128 B, 128-byte swizzle (chunk ^ (row & 7)) like the tensor map expects
-                uint8_t *box = smem + c * kTileBytes;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 o = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                           __uint_as_float(r[j + 3]));
-                    if (p.bias && col0 + j + 3 < p.N) {
-                        const float4 bv = ldg_f4(p.bias + col0 + j);
-                        o.x += bv.x, o.y += bv.y, o.z += bv.z, o.w += bv.w;
-                    } else if (p.bias) {
-                        if (col0 + j < p.N) o.x += __ldg(p.bias + col0 + j);
-                        if (col0 + j + 1 < p.N) o.y += __ldg(p.bias + col0 + j + 1);
-                        if (col0 + j + 2 < p.N) o.z += __ldg(p.bias + col0 + j + 2);
-                    }
-                    *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                named_bar_sync(1 + half, 128);  // the four warps that filled this box
-                if ((warp & 3) == 0 && lane == 0 && col0 < p.N) {
-                    tma_store_2d(&map_c, box, col0, m0);  // clips rows >= M and columns >= N
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            } else if (row < p.M) {
-                float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (col0 + j < p.N) crow[col0 + j] = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col0 + j) : 0.f);
-            }
-        }
-        if (p.use_tma_store && (warp & 3) == 0 && lane == 0)
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the bulk stores
-    }
-    if (threadIdx.x == 128) SDETR_TRACE(5, 1);  // epilogue end
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();  // the peer may still multicast into / arrive on this CTA's shared memory until it is done too
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(kTmemCols));
-    }
-}
-
-
-// ---- variant "TS": the split activation lives in TENSOR MEMORY ---------------------------------------------------------
-// The SS kernel above is bound by shared-memory bandwidth: per k-block the MMAs re-read 96 KB of operands, TMA
-// writes 48 KB and the converters move another 48 KB through the same 128 B/clk port.  Here the converters read the
-// landed A tile once (16 KB, swizzle-aware so a quarter-warp stays conflict-free) and write A_hi / A_lo with
-// tcgen05.st into TMEM slots (lane = row, column = k); the MMAs take A from TMEM ([a] operand) and only W from
-// shared memory: 112 KB instead of 192 KB of shared-memory traffic per k-block.  TMEM map (512 columns): accumulator
-// [0,128), A slot i in [128 + 64 i, 128 + 64 (i+1)): 32 columns A_hi then 32 columns A_lo, one slot per TMA stage.
-constexpr int kTsStages = 4;
-constexpr int kTsStageBytes = 3 * kTileBytes;  // A raw, W_hi, W_lo
-constexpr int kTsRingBytes = kTsStages * kTsStageBytes;
-constexpr int kTsSmem = kTsRingBytes + 1024 + 256;
-constexpr int kTsTmemCols = 512;
-
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_3xtf32_ts_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
-                      const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_c,
-                      const GemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kTsRingBytes);
-    uint64_t *tma_full = bars, *conv_full = bars + kTsStages, *empty = bars + 2 * kTsStages, *acc_full = bars + 3 * kTsStages;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * kBN, m0 = blockIdx.y * kBM;
-    const int nk = p.K / kBK;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kTsStages; ++s) {
-            mbar_init(tma_full + s, 1);
-            mbar_init(conv_full + s, 32 * kConvWarps);
-            mbar_init(empty + s, 2);
-        }
-        mbar_init(acc_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(kTsTmemCols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t rank = cluster_ctarank();
-    if (threadIdx.x == 0) SDETR_TRACE(5, 2);
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kTsStages;
-                const uint32_t ph = (kb / kTsStages) & 1;
-                mbar_wait(empty + s, ph ^ 1);  // both CTAs' MMAs have released ring stage s (and TMEM slot s)
-                SDETR_TRACE(0, kb);
-                uint8_t *st = smem + s * kTsStageBytes;
-                mbar_expect_tx(tma_full + s, 3 * kTileBytes);
-                tma_load_2d(&map_a, tma_full + s, st, kb * kBK, m0);
-                if (rank == 0) tma_load_2d_mc(&map_whi, tma_full + s, st + kTileBytes, kb * kBK, n0, 0b11);
-                else tma_load_2d_mc(&map_wlo, tma_full + s, st + 2 * kTileBytes, kb * kBK, n0, 0b11);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kTsStages;
-                const uint32_t ph = (kb / kTsStages) & 1;
-                mbar_wait(tma_full + s, ph);
-                SDETR_TRACE(1, kb);
-                mbar_wait(conv_full + s, ph);
-                SDETR_TRACE(2, kb);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t base = smem_u32(smem + s * kTsStageBytes);
-                const uint32_t a_hi = tmem_base + 128u + 64u * (uint32_t)s, a_lo = a_hi + 32u;
-#pragma unroll
-                for (int k = 0; k < kBK / 8; ++k) {
-                    const uint64_t w_hi = umma_desc(base + kTileBytes) + 2 * k, w_lo = umma_desc(base + 2 * kTileBytes) + 2 * k;
-                    umma_tf32_ts(tmem_base, a_hi + 8u * k, w_hi, kIdesc, (kb | k) != 0);
-                    umma_tf32_ts(tmem_base, a_hi + 8u * k, w_lo, kIdesc, 1);
-                    umma_tf32_ts(tmem_base, a_lo + 8u * k, w_hi, kIdesc, 1);
-                }
-                umma_commit_mc(empty + s, 0b11);
-            }
-            umma_commit(acc_full);
-        }
-    } else if (warp >= 4) {
-        const int t = threadIdx.x - 128;
-        const int q = warp & 3;             // TMEM lane quadrant of this warp
-        const int half = (warp - 4) >> 2;   // which 16 of the 32 k-columns (converter) / which column blocks (epilogue)
-        const int r_in = q * 32 + lane;     // tile row handled by this thread
-        for (int kb = 0; kb < nk; ++kb) {
-            const int s = kb % kTsStages;
-            const uint32_t ph = (kb / kTsStages) & 1;
-            mbar_wait(tma_full + s, ph);    // implies TMEM slot s is free: the refill waited for the MMAs of kb - stages
-            if (t == 0) SDETR_TRACE(3, kb);
-            const uint8_t *arow = smem + s * kTsStageBytes + r_in * 128;
-            float hi[16], lo[16];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {   // logical 16-byte chunk 4*half + c sits at physical chunk ^ (row & 7)
-                float4 x = *reinterpret_cast<const float4 *>(arow + ((((half << 2) + c) ^ (r_in & 7)) << 4));
-                if (p.relu_a == 1) {
-                    x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                } else if (p.relu_a == 2) {
-                    x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                }
-                hi[4 * c] = tf32_rn(x.x), hi[4 * c + 1] = tf32_rn(x.y), hi[4 * c + 2] = tf32_rn(x.z), hi[4 * c + 3] = tf32_rn(x.w);
-                lo[4 * c] = tf32_rn(x.x - hi[4 * c]), lo[4 * c + 1] = tf32_rn(x.y - hi[4 * c + 1]);
-                lo[4 * c + 2] = tf32_rn(x.z - hi[4 * c + 2]), lo[4 * c + 3] = tf32_rn(x.w - hi[4 * c + 3]);
-            }
-            const uint32_t slot = tmem_base + ((uint32_t)(q * 32) << 16) + 128u + 64u * (uint32_t)s + 16u * (uint32_t)half;
-            tmem_st16(slot, hi);
-            tmem_st16(slot + 32u, lo);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(conv_full + s);
-            if (t == 0) SDETR_TRACE(4, kb);
-        }
-        mbar_wait(acc_full, 0);
-        if (t == 0) SDETR_TRACE(5, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int row = m0 + r_in;
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {
-            const int c = half * 2 + cc;
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-            const int col0 = n0 + c * 32;
-            if (p.use_tma_store) {
-                uint8_t *box = smem + c * kTileBytes;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 o = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                           __uint_as_float(r[j + 3]));
-                    if (p.bias && col0 + j + 3 < p.N) {
-                        const float4 bv = ldg_f4(p.bias + col0 + j);
-                        o.x += bv.x, o.y += bv.y, o.z += bv.z, o.w += bv.w;
-                    } else if (p.bias) {
-                        if (col0 + j < p.N) o.x += __ldg(p.bias + col0 + j);
-                        if (col0 + j + 1 < p.N) o.y += __ldg(p.bias + col0 + j + 1);
-                        if (col0 + j + 2 < p.N) o.z += __ldg(p.bias + col0 + j + 2);
-                    }
-                    *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                named_bar_sync(1 + half, 128);
-                if ((warp & 3) == 0 && lane == 0 && col0 < p.N) {
-                    tma_store_2d(&map_c, box, col0, m0);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            } else if (row < p.M) {
-                float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (col0 + j < p.N) crow[col0 + j] = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col0 + j) : 0.f);
-            }
-        }
-        if (p.use_tma_store && (warp & 3) == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    if (threadIdx.x == 128) SDETR_TRACE(5, 1);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTsTmemCols));
-    }
-}
-
-
-// ---- variant "TS2": TS + weight split in the kernel + two CTAs per SM -----------------------------------------------------
-// Traces of the variants above show ~44 B/clk of TMA traffic INTO each SM as the wall (48 KB per k-block: A + W_hi +
-// W_lo), and at K = 256 the un-overlapped prologue/epilogue costs as much as the 8-k-block main loop.  This variant
-// loads the weight tile RAW (16 KB) and lets the converter warps split it as well (W_hi in place, W_lo next to it),
-// so a k-block is 32 KB of TMA traffic; and it runs with a 2-stage ring / 256 TMEM columns so that TWO CTAs share an
-// SM: one CTA's epilogue and pipeline fill overlap the other's main loop.
-constexpr int kT2Stages = 2;
-constexpr int kT2StageBytes = 3 * kTileBytes;  // A raw, W raw -> W_hi, W_lo
-constexpr int kT2RingBytes = kT2Stages * kT2StageBytes;
-constexpr int kT2Smem = kT2RingBytes + 1024 + 256;
-constexpr int kT2TmemCols = 256;               // accumulator [0,128) + 2 A slots of 64 columns
-
-__global__ void __launch_bounds__(kGemmThreads, 2)
-gemm_3xtf32_ts2_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
-                       const __grid_constant__ CUtensorMap map_c, const GemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kT2RingBytes);
-    uint64_t *tma_full = bars, *conv_full = bars + kT2Stages, *empty = bars + 2 * kT2Stages, *acc_full = bars + 3 * kT2Stages;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * kBN, m0 = blockIdx.y * kBM;
-    const int nk = p.K / kBK;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kT2Stages; ++s) {
-            mbar_init(tma_full + s, 1);
-            mbar_init(conv_full + s, 32 * kConvWarps);
-            mbar_init(empty + s, 1);
-        }
-        mbar_init(acc_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(kT2TmemCols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    if (threadIdx.x == 0) SDETR_TRACE(5, 2);
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kT2Stages;
-                const uint32_t ph = (kb / kT2Stages) & 1;
-                mbar_wait(empty + s, ph ^ 1);
-                SDETR_TRACE(0, kb);
-                uint8_t *st = smem + s * kT2StageBytes;
-                mbar_expect_tx(tma_full + s, 2 * kTileBytes);
-                tma_load_2d(&map_a, tma_full + s, st, kb * kBK, m0);
-                tma_load_2d(&map_w, tma_full + s, st + kTileBytes, kb * kBK, n0);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % kT2Stages;
-                const uint32_t ph = (kb / kT2Stages) & 1;
-                mbar_wait(conv_full + s, ph);  // converters waited for the TMA themselves
-                SDETR_TRACE(2, kb);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t base = smem_u32(smem + s * kT2StageBytes);
-                const uint32_t a_hi = tmem_base + 128u + 64u * (uint32_t)s, a_lo = a_hi + 32u;
-#pragma unroll
-                for (int k = 0; k < kBK / 8; ++k) {
-                    const uint64_t w_hi = umma_desc(base + kTileBytes) + 2 * k, w_lo = umma_desc(base + 2 * kTileBytes) + 2 * k;
-                    umma_tf32_ts(tmem_base, a_hi + 8u * k, w_hi, kIdesc, (kb | k) != 0);
-                    umma_tf32_ts(tmem_base, a_hi + 8u * k, w_lo, kIdesc, 1);
-                    umma_tf32_ts(tmem_base, a_lo + 8u * k, w_hi, kIdesc, 1);
-                }
-                umma_commit(empty + s);
-            }
-            umma_commit(acc_full);
-        }
-    } else if (warp >= 4) {
-        const int t = threadIdx.x - 128;
-        const int q = warp & 3;
-        const int half = (warp - 4) >> 2;
-        const int r_in = q * 32 + lane;
-        for (int kb = 0; kb < nk; ++kb) {
-            const int s = kb % kT2Stages;
-            const uint32_t ph = (kb / kT2Stages) & 1;
-            mbar_wait(tma_full + s, ph);
-            if (t == 0) SDETR_TRACE(3, kb);
-            uint8_t *stage = smem + s * kT2StageBytes;
-            // weight tile: element-wise split, W_hi in place, W_lo into the third buffer of the stage
-            float4 *w = reinterpret_cast<float4 *>(stage + kTileBytes), *wlo = reinterpret_cast<float4 *>(stage + 2 * kTileBytes);
-            float4 wv[4];
-#pragma unroll
-            for (int it = 0; it < 4; ++it) wv[it] = w[it * (32 * kConvWarps) + t];
-            // activation tile: this thread's row, 16 of the 32 k-columns
-            const uint8_t *arow = stage + r_in * 128;
-            float hi[16], lo[16];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                float4 x = *reinterpret_cast<const float4 *>(arow + ((((half << 2) + c) ^ (r_in & 7)) << 4));
-                if (p.relu_a == 1) {
-                    x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                } else if (p.relu_a == 2) {
-                    x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                }
-                hi[4 * c] = tf32_rn(x.x), hi[4 * c + 1] = tf32_rn(x.y), hi[4 * c + 2] = tf32_rn(x.z), hi[4 * c + 3] = tf32_rn(x.w);
-                lo[4 * c] = tf32_rn(x.x - hi[4 * c]), lo[4 * c + 1] = tf32_rn(x.y - hi[4 * c + 1]);
-                lo[4 * c + 2] = tf32_rn(x.z - hi[4 * c + 2]), lo[4 * c + 3] = tf32_rn(x.w - hi[4 * c + 3]);
-            }
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-                const float4 x = wv[it];
-                float4 h, l;
-                h.x = tf32_rn(x.x), h.y = tf32_rn(x.y), h.z = tf32_rn(x.z), h.w = tf32_rn(x.w);
-                l.x = tf32_rn(x.x - h.x), l.y = tf32_rn(x.y - h.y), l.z = tf32_rn(x.z - h.z), l.w = tf32_rn(x.w - h.w);
-                w[it * (32 * kConvWarps) + t] = h;
-                wlo[it * (32 * kConvWarps) + t] = l;
-            }
-            const uint32_t slot = tmem_base + ((uint32_t)(q * 32) << 16) + 128u + 64u * (uint32_t)s + 16u * (uint32_t)half;
-            tmem_st16(slot, hi);
-            tmem_st16(slot + 32u, lo);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(conv_full + s);
-            if (t == 0) SDETR_TRACE(4, kb);
-        }
-        mbar_wait(acc_full, 0);
-        if (t == 0) SDETR_TRACE(5, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int row = m0 + r_in;
-        // the ring (2 x 48 KB) is free now: boxes 0..3 (16 KB each) live in its first 64 KB
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {
-            const int c = half * 2 + cc;
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-            const int col0 = n0 + c * 32;
-            if (p.use_tma_store) {
-                uint8_t *box = smem + c * kTileBytes;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 o = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                           __uint_as_float(r[j + 3]));
-                    if (p.bias && col0 + j + 3 < p.N) {
-                        const float4 bv = ldg_f4(p.bias + col0 + j);
-                        o.x += bv.x, o.y += bv.y, o.z += bv.z, o.w += bv.w;
-                    } else if (p.bias) {
-                        if (col0 + j < p.N) o.x += __ldg(p.bias + col0 + j);
-                        if (col0 + j + 1 < p.N) o.y += __ldg(p.bias + col0 + j + 1);
-                        if (col0 + j + 2 < p.N) o.z += __ldg(p.bias + col0 + j + 2);
-                    }
-                    *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                named_bar_sync(1 + half, 128);
-                if ((warp & 3) == 0 && lane == 0 && col0 < p.N) {
-                    tma_store_2d(&map_c, box, col0, m0);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            } else if (row < p.M) {
-                float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (col0 + j < p.N) crow[col0 + j] = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col0 + j) : 0.f);
-            }
-        }
-        if (p.use_tma_store && (warp & 3) == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    if (threadIdx.x == 128) SDETR_TRACE(5, 1);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kT2TmemCols));
-    }
-}
-
-
-// ---- variant "P": persistent tiles, double-buffered accumulator, dedicated epilogue warps ------------------------------
-// One CTA per SM walks a strided list of 128x128 output tiles.  Roles (512 threads): warp 0 TMA producer, warp 1 MMA
-// issuer, warp 2 TMEM allocator, warps 4..11 converters (A -> TMEM slot, raw W -> W_hi/W_lo in place), warps 12..15
-// epilogue.  The accumulator is double-buffered in tensor memory (2 x 128 columns) so the epilogue of tile i
-// (tcgen05.ld -> +bias -> swizzled box -> TMA store) overlaps the main loop of tile i+1, and the 4-stage ring keeps
-// streaming across tile boundaries -- no per-tile pipeline fill, TMEM allocation or barrier initialisation.
-// TMEM map (512 columns): accumulators [0,128) and [128,256); A slot s at [256 + 64 s, 256 + 64 (s+1)).
-constexpr int kPStages = 4;
-constexpr int kPStageBytes = 3 * kTileBytes;
-constexpr int kPRingBytes = kPStages * kPStageBytes;            // 192 KB
-constexpr int kPBoxBytes = 2 * kTileBytes;                      // two 128x32 fp32 staging boxes for the TMA stores
-constexpr int kPSmem = kPRingBytes + kPBoxBytes + 1024 + 256;
-constexpr int kPThreads = 512;
-
-// kPre: the weight arrives pre-split (two TMA tiles W_hi / W_lo per stage, no in-kernel weight conversion): the stage's
-// shared-memory traffic drops from 144 KB (TMA 32 + convert read 32 + convert write 32 + MMA operand reads 48) to 112 KB.
-template <bool kPre>
-__global__ void __launch_bounds__(kPThreads, 1)
-gemm_3xtf32_p_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
-                     const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_c,
-                     const GemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *boxes = smem + kPRingBytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kPRingBytes + kPBoxBytes);
-    uint64_t *tma_full = bars, *conv_full = bars + kPStages, *empty = bars + 2 * kPStages;
-    uint64_t *acc_full = bars + 3 * kPStages, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nk = p.K / kBK;
-    const int n_tiles = (p.N + kBN - 1) / kBN, m_tiles = (p.M + kBM - 1) / kBM;
-    const int tiles = n_tiles * m_tiles;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kPStages; ++s) {
-            mbar_init(tma_full + s, 1);
-            mbar_init(conv_full + s, 32 * kConvWarps);
-            mbar_init(empty + s, 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(acc_full + b, 1);
-            mbar_init(acc_empty + b, 128);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-                const int m0 = (tile / n_tiles) * kBM, n0 = (tile % n_tiles) * kBN;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % kPStages;
-                    mbar_wait(empty + s, ((it / kPStages) & 1) ^ 1);
-                    uint8_t *st = smem + s * kPStageBytes;
-                    mbar_expect_tx(tma_full + s, (kPre ? 3 : 2) * kTileBytes);
-                    tma_load_2d(&map_a, tma_full + s, st, kb * kBK, m0);
-                    tma_load_2d(&map_w, tma_full + s, st + kTileBytes, kb * kBK, n0);
-                    if (kPre) tma_load_2d(&map_w2, tma_full + s, st + 2 * kTileBytes, kb * kBK, n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            uint32_t it = 0, tc = 0;
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tc) {
-                const uint32_t buf = tc & 1;
-                mbar_wait(acc_empty + buf, ((tc >> 1) & 1) ^ 1);  // the epilogue has drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc = tmem_base + buf * 128u;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % kPStages;
-                    mbar_wait(conv_full + s, (it / kPStages) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t base = smem_u32(smem + s * kPStageBytes);
-                    const uint32_t a_hi = tmem_base + 256u + 64u * (uint32_t)s, a_lo = a_hi + 32u;
-#pragma unroll
-                    for (int k = 0; k < kBK / 8; ++k) {
-                        const uint64_t w_hi = umma_desc(base + kTileBytes) + 2 * k, w_lo = umma_desc(base + 2 * kTileBytes) + 2 * k;
-                        umma_tf32_ts(acc, a_hi + 8u * k, w_hi, kIdesc, (kb | k) != 0);
-                        umma_tf32_ts(acc, a_hi + 8u * k, w_lo, kIdesc, 1);
-                        umma_tf32_ts(acc, a_lo + 8u * k, w_hi, kIdesc, 1);
-                    }
-                    umma_commit(empty + s);
-                }
-                umma_commit(acc_full + buf);
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ===== converters =====
-        const int t = threadIdx.x - 128;
-        const int q = warp & 3, half = (warp - 4) >> 2, r_in = q * 32 + lane;
-        uint32_t it = 0;
-        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-            for (int kb = 0; kb < nk; ++kb, ++it) {
-                const int s = it % kPStages;
-                mbar_wait(tma_full + s, (it / kPStages) & 1);
-                uint8_t *stage = smem + s * kPStageBytes;
-                float4 *w = reinterpret_cast<float4 *>(stage + kTileBytes), *wlo = reinterpret_cast<float4 *>(stage + 2 * kTileBytes);
-                float4 wv[4];
-                if (!kPre) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) wv[i] = w[i * (32 * kConvWarps) + t];
-                }
-                const uint8_t *arow = stage + r_in * 128;
-                float hi[16], lo[16];
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    float4 x = *reinterpret_cast<const float4 *>(arow + ((((half << 2) + c) ^ (r_in & 7)) << 4));
-                    if (p.relu_a == 1) {
-                        x.x = fmaxf(x.x, 0.f), x.y = fmaxf(x.y, 0.f), x.z = fmaxf(x.z, 0.f), x.w = fmaxf(x.w, 0.f);
-                    } else if (p.relu_a == 2) {
-                        x.x = gelu_erf(x.x), x.y = gelu_erf(x.y), x.z = gelu_erf(x.z), x.w = gelu_erf(x.w);
-                    }
-                    hi[4 * c] = tf32_rn(x.x), hi[4 * c + 1] = tf32_rn(x.y), hi[4 * c + 2] = tf32_rn(x.z), hi[4 * c + 3] = tf32_rn(x.w);
-                    lo[4 * c] = tf32_rn(x.x - hi[4 * c]), lo[4 * c + 1] = tf32_rn(x.y - hi[4 * c + 1]);
-                    lo[4 * c + 2] = tf32_rn(x.z - hi[4 * c + 2]), lo[4 * c + 3] = tf32_rn(x.w - hi[4 * c + 3]);
-                }
-                if (!kPre) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float4 x = wv[i];
-                        float4 h, l;
-                        h.x = tf32_rn(x.x), h.y = tf32_rn(x.y), h.z = tf32_rn(x.z), h.w = tf32_rn(x.w);
-                        l.x = tf32_rn(x.x - h.x), l.y = tf32_rn(x.y - h.y), l.z = tf32_rn(x.z - h.z), l.w = tf32_rn(x.w - h.w);
-                        w[i * (32 * kConvWarps) + t] = h;
-                        wlo[i * (32 * kConvWarps) + t] = l;
-                    }
-                }
-                const uint32_t slot = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + 64u * (uint32_t)s + 16u * (uint32_t)half;
-                tmem_st16(slot, hi);
-                tmem_st16(slot + 32u, lo);
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(conv_full + s);
-            }
-        }
-    } else if (warp >= 12) {
-        // ===== epilogue =====
-        const int q = warp & 3, r_in = q * 32 + lane;
-        const bool elected = threadIdx.x == 12 * 32;
-        uint32_t tc = 0, box_it = 0;
-        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tc) {
-            const int m0 = (tile / n_tiles) * kBM, n0 = (tile % n_tiles) * kBN;
-            const uint32_t buf = tc & 1;
-            mbar_wait(acc_full + buf, (tc >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int row = m0 + r_in;
-#pragma unroll 1
-            for (int c = 0; c < kBN / 32; ++c) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 128u + (uint32_t)(c * 32), r);
-                if (c == kBN / 32 - 1) {  // last read of this accumulator: hand it back to the MMA warp
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    mbar_arrive(acc_empty + buf);
-                }
-                const int col0 = n0 + c * 32;
-                if (col0 >= p.N) continue;  // uniform across the CTA
-                if (p.use_tma_store) {
-                    // the two staging boxes alternate per ISSUED store (skipped column blocks must not advance the
-                    // counter, or one box would be refilled while its previous store is still reading it)
-                    uint8_t *box = boxes + (box_it++ & 1) * kTileBytes;
-                    if (elected) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");  // box free again
-                    named_bar_sync(1, 128);
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 o = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                               __uint_as_float(r[j + 3]));
-                        if (p.bias && col0 + j + 3 < p.N) {
-                            const float4 bv = ldg_f4(p.bias + col0 + j);
-                            o.x += bv.x, o.y += bv.y, o.z += bv.z, o.w += bv.w;
-                        } else if (p.bias) {
-                            if (col0 + j < p.N) o.x += __ldg(p.bias + col0 + j);
-                            if (col0 + j + 1 < p.N) o.y += __ldg(p.bias + col0 + j + 1);
-                            if (col0 + j + 2 < p.N) o.z += __ldg(p.bias + col0 + j + 2);
-                        }
-                        *reinterpret_cast<float4 *>(box + r_in * 128 + (((j >> 2) ^ (r_in & 7)) << 4)) = o;
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    named_bar_sync(1, 128);
-                    if (elected) {
-                        tma_store_2d(&map_c, box, col0, m0);
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
-                } else if (row < p.M) {
-                    float *crow = p.C + (int64_t)row * p.ldc;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (col0 + j < p.N) crow[col0 + j] = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col0 + j) : 0.f);
-                }
-            }
-        }
-        if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
 
 // weight split: (N,K) -> W_hi, W_lo (both (N,K), TF32-representable)
 __global__ void split_pair_kernel(const float *__restrict__ w, int64_t n, float *__restrict__ hi, float *__restrict__ lo) {
@@ -790,13 +22,28 @@ __global__ void split_pair_kernel(const float *__restrict__ w, int64_t n, float 
     hi[i] = h, lo[i] = tf32_rn(x - h);
 }
 
-// ---- host side --------------------------------------------------------------------------------------------------------
-// 2-D fp32 tensor (rows, cols) with row stride ld (floats); box = (kBK cols, box_rows rows), 128-byte swizzle
-static std::atomic<long long *> g_gemm_dbg{nullptr};
-static std::atomic<int> g_raw_persistent{1};  // sdetr_gemm_3xtf32_raw: 1 = persistent kernel "P", 0 = "TS2"
-static std::atomic<int> g_gemm_variant{0};  // 0 = SS (operands from shared memory), 1 = TS (split activation in tensor memory)
-static bool make_map(CUtensorMap *m, const float *base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
-    return make_map_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, rows, cols, ld, kBK, box_rows);
+// 2-D fp32 tensor (rows, cols) with row stride ld (floats); box = 32 cols x 128 rows, 128-byte swizzle
+static bool make_map(CUtensorMap *m, const float *base, int64_t rows, int64_t cols, int64_t ld) {
+    return make_map_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, rows, cols, ld, 32, kGN);
+}
+
+static int gemm_3xtf32_impl(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, float *C,
+                            int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream, const char *what) {
+    const bool raw = W_lo == nullptr;  // sdetr_gemm_3xtf32_raw: W_hi is the raw weight
+    SDETR_REQUIRE(A && W_hi && C, SDETR_ERR_INVALID_ARG, "%s: null pointer", what);
+    SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2, SDETR_ERR_INVALID_ARG, "%s: bad sizes / activation", what);
+    SDETR_REQUIRE(K % Gemm3xShape<false>::kK == 0, SDETR_ERR_UNSUPPORTED, "%s: K=%d must be a multiple of %d", what, K,
+                  Gemm3xShape<false>::kK);
+    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && (raw || aligned16(W_lo)) && lda >= K && ldc >= N,
+                  SDETR_ERR_INVALID_ARG, "%s: operands must be 16-byte aligned with 16-byte row pitch", what);
+    if (M == 0) return SDETR_OK;
+    CUtensorMap mh, ml;
+    SDETR_REQUIRE(make_map(&mh, W_hi, N, K, K) && (raw || make_map(&ml, W_lo, N, K, K)), SDETR_ERR_CUDA,
+                  "%s: cuTensorMapEncodeTiled failed", what);
+    if (raw) ml = mh;
+    const Gemm3xParams p{bias, C, ldc, M, N, K, act, 1.f, 1.f, nullptr, nullptr};
+    return raw ? launch_gemm3x<false, true>(A, lda, mh, ml, p, stream, what)
+               : launch_gemm3x<false, false>(A, lda, mh, ml, p, stream, what);
 }
 
 }  // namespace sdetr
@@ -805,43 +52,8 @@ using namespace sdetr;
 
 extern "C" int sdetr_gemm_3xtf32_raw(const float *A, int64_t lda, const float *W, const float *bias, float *C, int64_t ldc,
                                      int M, int N, int K, int act, sdetr_stream_t stream) {
-    SDETR_REQUIRE(A && W && C, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_raw: null pointer");
-    SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_raw: bad sizes / activation");
-    SDETR_REQUIRE(K % kBK == 0, SDETR_ERR_UNSUPPORTED, "gemm_3xtf32_raw: K=%d must be a multiple of %d", K, kBK);
-    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W) && lda >= K && ldc >= N, SDETR_ERR_INVALID_ARG,
-                  "gemm_3xtf32_raw: operands must be 16-byte aligned with 16-byte row pitch");
-    if (M == 0) return SDETR_OK;
-    CUtensorMap ma, mw, mc;
-    SDETR_REQUIRE(make_map(&ma, A, M, K, lda, kBM) && make_map(&mw, W, N, K, K, kBN), SDETR_ERR_CUDA,
-                  "gemm_3xtf32_raw: cuTensorMapEncodeTiled failed");
-    const int use_tma_store = (ldc % 4 == 0) && aligned16(C) && make_map(&mc, C, M, N, ldc, kBM);
-    if (!use_tma_store) mc = ma;
-    static PerDeviceOnce once_t2, once_p;
-    SDETR_OPT_IN_SMEM(once_t2, gemm_3xtf32_ts2_kernel, kT2Smem, "gemm_3xtf32_raw");
-    SDETR_OPT_IN_SMEM(once_p, gemm_3xtf32_p_kernel<false>, kPSmem, "gemm_3xtf32_raw");
-    const int sms = sm_count();
-    GemmParams p{bias, C, ldc, M, N, K, act, use_tma_store, g_gemm_dbg.load()};
-    if (g_raw_persistent) {
-        const int tiles = ((N + kBN - 1) / kBN) * ((M + kBM - 1) / kBM);
-        gemm_3xtf32_p_kernel<false><<<tiles < sms ? tiles : sms, kPThreads, kPSmem, (cudaStream_t)stream>>>(ma, mw, mw, mc, p);
-        return check_launch("gemm_3xtf32_raw");
-    }
-    dim3 grid((N + kBN - 1) / kBN, (M + kBM - 1) / kBM);
-    gemm_3xtf32_ts2_kernel<<<grid, kGemmThreads, kT2Smem, (cudaStream_t)stream>>>(ma, mw, mc, p);
-    return check_launch("gemm_3xtf32_raw");
-}
-
-extern "C" int sdetr_gemm_set_variant(int variant) {
-    // 0 / 1: sdetr_gemm_3xtf32 uses "SS" / "TS";   2 / 3: sdetr_gemm_3xtf32_raw uses "TS2" / persistent "P"
-    SDETR_REQUIRE(variant >= 0 && variant <= 3, SDETR_ERR_INVALID_ARG, "gemm_set_variant: 0..3");
-    if (variant <= 1) g_gemm_variant = variant;
-    else g_raw_persistent = variant - 2;
-    return SDETR_OK;
-}
-
-extern "C" int sdetr_gemm_set_trace(long long *device_buffer /* 6*128 int64, or NULL */) {
-    g_gemm_dbg = device_buffer;
-    return SDETR_OK;
+    SDETR_REQUIRE(W, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_raw: null pointer");
+    return gemm_3xtf32_impl(A, lda, W, nullptr, bias, C, ldc, M, N, K, act, stream, "gemm_3xtf32_raw");
 }
 
 extern "C" int sdetr_split_tf32_pair(const float *w, int64_t count, float *w_hi, float *w_lo, sdetr_stream_t stream) {
@@ -853,57 +65,12 @@ extern "C" int sdetr_split_tf32_pair(const float *w, int64_t count, float *w_hi,
 
 extern "C" int sdetr_gemm_3xtf32(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias,
                                  float *C, int64_t ldc, int M, int N, int K, int relu_a, sdetr_stream_t stream) {
-    SDETR_REQUIRE(A && W_hi && W_lo && C, SDETR_ERR_INVALID_ARG, "gemm_3xtf32: null pointer");
-    SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && relu_a >= 0 && relu_a <= 2, SDETR_ERR_INVALID_ARG, "gemm_3xtf32: bad sizes / activation");
-    SDETR_REQUIRE(K % kBK == 0, SDETR_ERR_UNSUPPORTED, "gemm_3xtf32: K=%d must be a multiple of %d", K, kBK);
-    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && aligned16(W_lo) && lda >= K && ldc >= N,
-                  SDETR_ERR_INVALID_ARG, "gemm_3xtf32: operands must be 16-byte aligned with 16-byte row pitch");
-    if (M == 0) return SDETR_OK;
-    CUtensorMap ma, mh, ml, mc;
-    SDETR_REQUIRE(make_map(&ma, A, M, K, lda, kBM) && make_map(&mh, W_hi, N, K, K, kBN) && make_map(&ml, W_lo, N, K, K, kBN),
-                  SDETR_ERR_CUDA, "gemm_3xtf32: cuTensorMapEncodeTiled failed");
-    // the epilogue leaves through TMA bulk stores when C's rows are 16-byte aligned (else plain stores, e.g. N = 91)
-    const int use_tma_store = (ldc % 4 == 0) && aligned16(C) && make_map(&mc, C, M, N, ldc, kBM);
-    if (!use_tma_store) mc = ma;
-    static PerDeviceOnce once_ss, once_ts;
-    SDETR_OPT_IN_SMEM(once_ss, gemm_3xtf32_kernel, kGemmSmem, "gemm_3xtf32");
-    SDETR_OPT_IN_SMEM(once_ts, gemm_3xtf32_ts_kernel, kTsSmem, "gemm_3xtf32");
-    GemmParams p{bias, C, ldc, M, N, K, relu_a, use_tma_store, g_gemm_dbg.load()};
-    const int mtiles = (M + kBM - 1) / kBM;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((N + kBN - 1) / kBN, (mtiles + 1) & ~1);  // clusters of 2 along M (an odd tail tile is all out-of-bounds)
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = g_gemm_variant ? kTsSmem : kGemmSmem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 1, at[0].val.clusterDim.y = 2, at[0].val.clusterDim.z = 1;
-    cfg.attrs = at, cfg.numAttrs = 1;
-    cudaError_t le = g_gemm_variant ? cudaLaunchKernelEx(&cfg, gemm_3xtf32_ts_kernel, ma, mh, ml, mc, p)
-                                    : cudaLaunchKernelEx(&cfg, gemm_3xtf32_kernel, ma, mh, ml, mc, p);
-    SDETR_REQUIRE(le == cudaSuccess, SDETR_ERR_CUDA, "gemm_3xtf32: launch: %s", cudaGetErrorString(le));
-    return check_launch("gemm_3xtf32");
+    SDETR_REQUIRE(W_lo, SDETR_ERR_INVALID_ARG, "gemm_3xtf32: null pointer");
+    return gemm_3xtf32_impl(A, lda, W_hi, W_lo, bias, C, ldc, M, N, K, relu_a, stream, "gemm_3xtf32");
 }
 
-// Persistent kernel on a pre-split weight (W_hi, W_lo from sdetr_split_tf32_pair, cached by the caller per parameter).
 extern "C" int sdetr_gemm_3xtf32_pre(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias,
                                      float *C, int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream) {
-    SDETR_REQUIRE(A && W_hi && W_lo && C, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_pre: null pointer");
-    SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_pre: bad sizes / activation");
-    SDETR_REQUIRE(K % kBK == 0, SDETR_ERR_UNSUPPORTED, "gemm_3xtf32_pre: K=%d must be a multiple of %d", K, kBK);
-    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && aligned16(W_lo) && lda >= K && ldc >= N,
-                  SDETR_ERR_INVALID_ARG, "gemm_3xtf32_pre: operands must be 16-byte aligned with 16-byte row pitch");
-    if (M == 0) return SDETR_OK;
-    CUtensorMap ma, mh, ml, mc;
-    SDETR_REQUIRE(make_map(&ma, A, M, K, lda, kBM) && make_map(&mh, W_hi, N, K, K, kBN) && make_map(&ml, W_lo, N, K, K, kBN),
-                  SDETR_ERR_CUDA, "gemm_3xtf32_pre: cuTensorMapEncodeTiled failed");
-    const int use_tma_store = (ldc % 4 == 0) && aligned16(C) && make_map(&mc, C, M, N, ldc, kBM);
-    if (!use_tma_store) mc = ma;
-    static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, gemm_3xtf32_p_kernel<true>, kPSmem, "gemm_3xtf32_pre");
-    const int sms = sm_count();
-    GemmParams p{bias, C, ldc, M, N, K, act, use_tma_store, g_gemm_dbg.load()};
-    const int tiles = ((N + kBN - 1) / kBN) * ((M + kBM - 1) / kBM);
-    gemm_3xtf32_p_kernel<true><<<tiles < sms ? tiles : sms, kPThreads, kPSmem, (cudaStream_t)stream>>>(ma, mh, ml, mc, p);
-    return check_launch("gemm_3xtf32_pre");
+    SDETR_REQUIRE(W_lo, SDETR_ERR_INVALID_ARG, "gemm_3xtf32_pre: null pointer");
+    return gemm_3xtf32_impl(A, lda, W_hi, W_lo, bias, C, ldc, M, N, K, act, stream, "gemm_3xtf32_pre");
 }

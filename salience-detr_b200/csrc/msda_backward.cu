@@ -1,4 +1,4 @@
-// MSDA core backward for sm_100a -- sdetr_msda_backward.
+// MSDA core backward for sm_90a -- sdetr_msda_backward.
 //
 // Reference semantics: models/bricks/ops/cuda/ms_deform_im2col_cuda.cuh:76-148 (bilinear backward helper)
 // and :290-392 (the kernel variant selected at head_dim 32, `case 32` :1129-1150), host wrapper

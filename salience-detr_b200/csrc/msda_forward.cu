@@ -1,4 +1,4 @@
-// MSDA core forward for sm_100a -- sdetr_msda_forward / _ex / sdetr_msda_fused_forward.
+// MSDA core forward for sm_90a -- sdetr_msda_forward / _ex / sdetr_msda_fused_forward.
 //
 // Reference semantics: models/bricks/ops/cuda/ms_deform_im2col_cuda.cuh:22-73,226-288 (kernel) and
 // models/bricks/ms_deform_attn.py:322-344 (softmax + sampling-location arithmetic, fused variant).
@@ -307,10 +307,9 @@ __global__ void __launch_bounds__(THREADS, MINB) msda_fwd_kernel(const MsdaFwdPa
 }
 
 // ---- "W32": one WARP per (image, query, head), one lane per channel (D = 32, L = 4, P = 4, head-major schedule) ------------
-// Measured on the kernel above (profiles/r2_msda_probe_v1.txt): even when every gather hits in L1 it needs ~125 clk per
-// (query, head) per SM, twice the 64 clk that 64 corner rows x 128 B cost at 128 B/clk.  Its LDG.128 instructions touch four
-// different 128-byte lines each (one per 8-lane group), and a multi-line request is replayed at ~2 clk per line
-// (B300_MICROARCH.md: 1.0 clk per wavefront across instructions, 2.07 within one).  Here every corner row is ONE fully
+// The kernel above issues LDG.128 instructions that touch four different 128-byte lines each (one per 8-lane group), and a
+// multi-line request is replayed line by line in the L1 tag stage, so even all-hit gathers cost more than their 128 B per row
+// of data movement.  Here every corner row is ONE fully
 // coalesced 128-byte LDG.32 -- a single line, a single wavefront -- issued by the whole warp:
 //   * lane e (and its mirror e + 16) owns sampling point e of the (query, head): softmax over 16 lanes by shuffles,
 //     location, corner index and the four weights are computed once per point and published in 320 bytes of shared memory

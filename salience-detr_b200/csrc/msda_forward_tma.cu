@@ -2,9 +2,8 @@
 //
 // Reference semantics as msda_forward.cu (ms_deform_im2col_cuda.cuh:226-288; ms_deform_attn.py:322-349 for the fused part).
 //
-// Why: the L1 gather of msda_forward.cu is bounded by the cache's tag stage, not its data stage -- with EVERY access an L1
-// hit it still needs ~125 clk per (query, head) per SM for 64 corner rows, i.e. ~2 clk per 128-byte line
-// (profiles/r2_msda_probe_v1.txt, "allhit"); a shared-memory row costs one 128-byte wavefront, 1 clk.  So this variant
+// Why: the L1 gather of msda_forward.cu can be bounded by the cache's tag stage rather than its data stage (multi-line
+// requests are replayed line by line even when every access hits); a shared-memory row costs one 128-byte wavefront.  So this variant
 // stages, per CTA, the part of every level's value map that its queries sample into shared memory with TMA and gathers
 // from there:
 //   * CTA = one head x `chunk` consecutive queries of the spatial tile order (as the head-major schedule of

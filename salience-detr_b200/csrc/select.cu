@@ -1,4 +1,4 @@
-// Hierarchical salience token filter for sm_100a -- sdetr_salience_select, sdetr_order_prefixes,
+// Hierarchical salience token filter for sm_90a -- sdetr_salience_select, sdetr_order_prefixes,
 // sdetr_topk_desc.
 //
 // Reference semantics: models/bricks/salience_transformer.py:146-168 (masked_fill with the batch-global
@@ -704,7 +704,7 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
     int rc = check_launch("salience_select/level_min");
     if (rc) return rc;
     const int64_t total = (int64_t)batch * num_value;
-    const int64_t fg_blocks = (total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8;
+    const int64_t fg_cap = 8 * (int64_t)sm_count(), fg_blocks = (total + 255) / 256 < fg_cap ? (total + 255) / 256 : fg_cap;
     foreground_kernel<<<(unsigned)fg_blocks, 256, 0, s>>>(raw_score, mask, lmin, num_levels, total, foreground_score);
     if ((rc = check_launch("salience_select/foreground"))) return rc;
     if (K == 0) return SDETR_OK;

@@ -1,4 +1,4 @@
-// Token movement and small fused elementwise kernels around the encoder layers (sm_100a).
+// Token movement and small fused elementwise kernels around the encoder layers (sm_90a).
 //
 // Reference semantics: models/bricks/salience_transformer.py:134-143 (score modulation), :366 (mc score),
 // :390-391/:349-350 (residual + LayerNorm), :417-432 + :454-461 (reference points + four gathers),
@@ -541,7 +541,7 @@ extern "C" int sdetr_gelu_colmean(float *z, int batch, int num_rows, int channel
     // pass 1 is a read-modify-write stream: up to 8 resident CTAs per SM so enough loads are in flight;
     // pass 2 only stores (and every CTA re-adds the partials), one wave is enough
     int chunks1 = (num_rows + 31) / 32, chunks2 = (num_rows + 63) / 64;
-    const int cap1 = 592 / batch > 0 ? 592 / batch : 1, cap2 = 148 / batch > 0 ? 148 / batch : 1;
+    const int sms = sm_count(), cap1 = 4 * sms / batch > 0 ? 4 * sms / batch : 1, cap2 = sms / batch > 0 ? sms / batch : 1;
     if (chunks1 > cap1) chunks1 = cap1;
     if (chunks2 > cap2) chunks2 = cap2;
     cudaStream_t s = (cudaStream_t)stream;

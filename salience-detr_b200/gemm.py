@@ -2,12 +2,12 @@
 
 These are true dense GEMMs, the only place of the path where tensor cores belong.  ``MODE``:
 
-* ``"auto"`` (default): the hand-written persistent tcgen05 kernels on a pre-split weight -- ``OWN_KERNEL = "f16x3"``:
-  ``sdetr_gemm_f16x3_pre`` (3xFP16 on ``tcgen05.mma.kind::f16``: same 22-bit operands as 3xTF32 at twice the MMA rate, for
+* ``"auto"`` (default): the hand-written persistent wgmma kernels on a pre-split weight -- ``OWN_KERNEL = "f16x3"``:
+  ``sdetr_gemm_f16x3_pre`` (3xFP16 on ``wgmma`` .f16: same 22-bit operands as 3xTF32 at twice the MMA rate, for
   K % 64 == 0); ``"tf32x3"`` (or K % 64 != 0): ``sdetr_gemm_3xtf32_pre`` -- except GEMMs with at most ``SMALL_M`` rows (the
   coarse levels of the MaskPredictor), which are latency-bound and go to cuBLAS fp32.
-* ``"tcgen05"``: the hand-written sm_100a GEMM (``sdetr_gemm_3xtf32``: TMA -> in-kernel TF32 split of the activation
-  -> tcgen05.mma.kind::tf32 into TMEM -> epilogue), same 3xTF32 arithmetic without the separate split pass.
+* ``"tcgen05"`` (name kept for existing callers): the hand-written sm_90a 3xTF32 GEMM (``sdetr_gemm_3xtf32_pre``: TMA ->
+  TF32 split of the activation in registers -> wgmma .tf32 -> epilogue), same arithmetic without the separate split pass.
 * ``"3xtf32"``: each operand is split into two TF32 pieces by ``sdetr_split_tf32`` and ONE cuBLAS TF32
   GEMM over K' = 3K accumulates A_hi.B_hi + A_hi.B_lo + A_lo.B_hi in fp32 -- tensor-core speed with fp32-class
   accuracy (error ~2^-21 relative per product, same order as fp32 summation-order noise; measured in
@@ -138,7 +138,7 @@ def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input:
             if PRESPLIT_PERSISTENT:
                 w_hi, w_lo = split_weight_pair(weight)
                 return cabi.gemm_3xtf32_pre(x, w_hi, w_lo, bias, relu_input)
-            # short reductions: both operands split in the kernel, A in TMEM, two CTAs per SM (variant "TS2")
+            # both operands split in the kernel
             return cabi.gemm_3xtf32_raw(x, weight if weight.is_contiguous() else weight.contiguous(), bias, relu_input)
     if MODE == "fp32" or k % 4 != 0:
         return F.linear(_act_torch(x, relu_input), weight, bias)

@@ -1,4 +1,4 @@
-"""Drop-in mirror of the reference's ``models/bricks/ms_deform_attn.py`` on top of the sm_100a C-ABI.
+"""Drop-in mirror of the reference's ``models/bricks/ms_deform_attn.py`` on top of the sm_90a C-ABI.
 
 Same public names, constructor arguments, parameter names and ``forward`` signature as the reference
 (``MultiScaleDeformableAttention`` ms_deform_attn.py:215-377, ``MultiScaleDeformableAttnFunction`` :35-84,
@@ -74,7 +74,7 @@ class MultiScaleDeformableAttnFunction(Function):
 
 
 class MultiScaleDeformableAttention(nn.Module):
-    """Multi-scale deformable attention (Deformable-DETR), B200-native core."""
+    """Multi-scale deformable attention (Deformable-DETR), H100-native core."""
 
     def __init__(self, embed_dim: int = 256, num_levels: int = 4, num_heads: int = 8, num_points: int = 4,
                  img2col_step: int = 64):
@@ -166,7 +166,7 @@ class MultiScaleDeformableAttention(nn.Module):
         b, nq, _ = query.shape
         nv = value.shape[1]
         if not value.is_cuda:
-            raise RuntimeError("MultiScaleDeformableAttention (B200) needs CUDA tensors; there is no CPU path")
+            raise RuntimeError("MultiScaleDeformableAttention needs CUDA tensors; there is no CPU path")
         M, L, P, D = self.num_heads, self.num_levels, self.num_points, self.embed_dim // self.num_heads
         v = self.project_value(value, key_padding_mask)
         needs_grad = torch.is_grad_enabled() and (query.requires_grad or v.requires_grad or

@@ -2,7 +2,7 @@
 
 Same constructor arguments and buffers (``dim_tx`` / ``dim_ty``) and the same ``forward(mask) -> (b, 2F, H, W)``.
 In the detector the embedding is a pure function of the padding mask (models/detectors/salience_detr.py:172-176), so the
-B200 path never moves it over PCIe and never materialises it per level in NCHW: ``tokens()`` writes it once per mask
+H100 path never moves it over PCIe and never materialises it per level in NCHW: ``tokens()`` writes it once per mask
 geometry, directly in the (b,Nv,C) token layout the encoder consumes, from the normalised coordinates that
 ``sdetr_mask_plan`` produces (two launches instead of ~15 ATen launches per level)."""
 from __future__ import annotations
@@ -45,7 +45,7 @@ class PositionEmbeddingSine(nn.Module):
     def forward(self, mask: Tensor) -> Tensor:
         """Reference signature: (b,H,W) bool padding mask -> (b,2F,H,W).  CUDA masks run the fused kernels."""
         if not mask.is_cuda:
-            raise RuntimeError("PositionEmbeddingSine (B200) needs a CUDA mask; there is no CPU path")
+            raise RuntimeError("PositionEmbeddingSine needs a CUDA mask; there is no CPU path")
         b, h, w = mask.shape
         if not self.normalize:  # RT-DETR style un-normalised variant: not on this path, plain torch ops
             nm = (~mask.bool()).to(torch.float32)

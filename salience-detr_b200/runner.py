@@ -1,7 +1,7 @@
 """EncoderRunner: the sync-free, CUDA-graph way to call the encoder half for a fixed batch geometry.
 
 The reference forces ~40 host synchronisations and ~1000 tiny launches per encoder forward (SURVEY.md 3a);
-on a B200 the algorithmic time of the path is ~0.1-1 ms, so launch latency would dominate.  The runner builds
+on an H100 the algorithmic time of the path is ~0.1-1 ms, so launch latency would dominate.  The runner builds
 the ``EncoderPlan`` once, captures ``SalienceTransformer.forward_encoder`` into one CUDA graph over static
 device buffers and replays it; ``run_host`` adds the pinned-host <-> device copies on the same stream."""
 from __future__ import annotations

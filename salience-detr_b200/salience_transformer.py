@@ -6,7 +6,7 @@ Same class names, constructor arguments, sub-module / parameter names and ``forw
 (``strict=False`` skips the decoder keys) and reference configs can instantiate these classes in place
 of the originals.  The decoder half (:194-295, :500-674) is out of scope for this round (SURVEY.md 8(f)-1).
 
-How the path is laid out for a B200 (none of this is a translation of the reference's op chain):
+How the path is laid out for an H100 (none of this is a translation of the reference's op chain):
 
 * one ``EncoderPlan`` per batch geometry holds everything derived from the padding masks (token budgets,
   level tables, valid ratios, keep mask).  Building it costs ONE host round trip; the reference syncs
@@ -33,11 +33,11 @@ from . import cabi, gemm
 from .ms_deform_attn import MultiScaleDeformableAttention
 
 OVERLAP_VALUE_PROJ = True  # all-layer value projection as a parallel branch (graph capture) / on a side stream (eager) beside the salience filter
-OVERLAP_VALUE_PROJ_EAGER = __import__("os").environ.get("SDETR_OVERLAP_EAGER", "0") != "0"  # eager too: measured on the fresh-mask
-# pipeline, 760 vs 781-795 images/s -- the extra stream operations cost the (host-bound) eager path more than the overlap returns: off
-VALUE_PROJ_PER_LAYER = False  # (measured, profiles/r2_msda_probe_v1.txt: L2-warm value buys the sampling kernel 2 %; one N=1536 GEMM is 1.5x cheaper than six N=256 ones)
+OVERLAP_VALUE_PROJ_EAGER = __import__("os").environ.get("SDETR_OVERLAP_EAGER", "0") != "0"  # eager too: off by default,
+# because the extra stream operations cost the (host-bound) eager path of the fresh-mask pipeline more than the overlap returns
+VALUE_PROJ_PER_LAYER = False  # (off: one N=1536 GEMM is cheaper than six N=256 ones)
 # each layer's value_proj as its own GEMM on a side stream beside that layer's (latency-bound)
-# pre-attention, joined right before the sampling kernel: the 45.7 MB it writes are still in the 126 MB L2 when the
+# pre-attention, joined right before the sampling kernel: the 45.7 MB it writes may still be in L2 when the
 # sampling kernel gathers from them (one 6-layer GEMM up front writes 274 MB, which L2 cannot hold), and the value rows
 # are 1 KB apart instead of 6 KB
 FUSED_GELU_MEAN = True     # MaskPredictor: GELU + token-mean of the global half as two fused launches (else torch ops)
@@ -52,14 +52,12 @@ OVERLAP_PROJ = False  # (measured: 763 vs 773 images/s, e2e 918 vs 942 -- the ex
 FUSED_SMALL_PREDICTOR = __import__("os").environ.get("SDETR_FUSED_SMALL_PREDICTOR", "1") != "0"  # score modulation + MaskPredictor of a
 # level with at most PREDICTOR_SMALL_ROWS token rows as two fp32 kernels (csrc/predictor_small.cu) instead of ~15 latency-bound launches
 PREDICTOR_SMALL_ROWS = 4096
-FUSED_FFN = __import__("os").environ.get("SDETR_FUSED_FFN", "1") != "0"  # C = 256: linear1 -> ReLU -> linear2 -> +residual -> norm2 as ONE
-# tensor-core kernel that keeps the hidden activations in tensor memory (csrc/ffn_fused.cu) + a row kernel, instead of two GEMMs
-# writing / reading the (rows x d_ffn) hidden tensor and an add+LayerNorm launch
-FFN_CHUNK_ROWS = int(__import__("os").environ.get("SDETR_FFN_CHUNK", "0"))  # FFN in row chunks: the hidden activations of a chunk (6144 x 2048 fp32 = 50 MB) are produced and consumed
-# inside the 126 MB L2 and their buffer is reused by the next chunk, so most of the hidden tensor (186 MB at layer 0) is never
-# written to / read back from HBM -- the K = 256 GEMMs with outputs larger than L2 are bound by the HBM write stream (DESIGN 3.4).
-# 0 (default) = one GEMM pair over all rows.  MEASURED (profiles/r2_ffn_chunk_sweep.txt): 811 images/s unchunked vs 798 / 772 / 680
-# with chunks of 9216 / 6144 / 4096 rows -- the per-launch prologue and tail of the smaller GEMMs cost more than the HBM traffic saves.
+FUSED_FFN = __import__("os").environ.get("SDETR_FUSED_FFN", "1") != "0"  # C = 256: linear1 -> ReLU -> linear2 -> +residual -> norm2
+# through sdetr_ffn_fused_layernorm (csrc/ffn_fused.cu: two 3xFP16 GEMMs, the ReLU fused into the second's operand load, + a row kernel)
+# instead of two gemm.linear calls and an add+LayerNorm launch
+FFN_CHUNK_ROWS = int(__import__("os").environ.get("SDETR_FFN_CHUNK", "0"))  # FFN in row chunks: the hidden activations of a chunk are
+# produced and consumed while they can still sit in L2 and their buffer is reused by the next chunk.  0 (default) = one GEMM pair
+# over all rows.
 TILE_CELL_PX = 64   # edge (image pixels) of the spatial cells that define the MSDA processing order
 MSDA_SCHEDULE = 1   # 0 = query-major, 1 = head-major chunks (see include/sdetr_b200.h)
 

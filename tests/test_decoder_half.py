@@ -1,19 +1,21 @@
-"""Decoder half (SURVEY.md 8(f)-1) against the UNMODIFIED reference modules (baseline/_ref, see test_dropin_reference.py):
-two-stage proposal selection (salience_transformer.py:194-212, 249-295) and the decoder (:498-674) with 4-d reference boxes
-through the fused sampling kernel."""
+"""Decoder half (SURVEY.md 8(f)-1) against the UNMODIFIED reference modules: two-stage proposal selection
+(salience_transformer.py:194-212, 249-295) and the decoder (:498-674) with 4-d reference boxes through the fused sampling kernel.
+What the reference computes is stored in tests/golden/{nms_topk,decoder_half_even,decoder_half_ragged}.npz (oracle/make_golden.py
+runs the original project on the same deterministic weights -- oracle.deterministic_state_dict -- and seeded inputs)."""
+import json
+import os
+
+import numpy as np
 import pytest
 import torch
 
+from conftest import GOLDEN
+from oracle import make_golden as mg
 from oracle import oracle as orc
-from oracle import ref_import
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-GEO = dict(embed_dim=256, d_ffn=512, n_heads=8, n_levels=4, n_points=4, num_layers=2, num_classes=17,
-           level_filter_ratio=(0.4, 0.8, 1.0, 1.0), layer_filter_ratio=(1.0, 0.5), topk_sa=100, max_num_embedding=100,
-           num_proposals=300)
-DEC_LAYERS = 3
+GEO = mg.HALF
 
 
 @pytest.fixture(scope="module")
@@ -21,13 +23,6 @@ def pkg():
     import salience_detr_b200 as p
     p.cabi.lib()
     return p
-
-
-@pytest.fixture(scope="module")
-def ref():
-    if not ref_import.available():
-        pytest.skip("baseline/_ref not installed (run __graft_entry__.build() where /root/reference exists)")
-    return ref_import.load()
 
 
 @pytest.fixture(autouse=True)
@@ -39,60 +34,44 @@ def _fp32(pkg):
     pkg.gemm.MODE = mode
 
 
-def _reference(ref, seed=2):
-    st = ref.st
-    torch.manual_seed(seed)
-    relu = torch.nn.ReLU(inplace=True)
-    enc = st.SalienceTransformerEncoder(st.SalienceTransformerEncoderLayer(GEO["embed_dim"], GEO["d_ffn"], 0.0, GEO["n_heads"], relu,
-                                                                           4, 4, topk_sa=GEO["topk_sa"]), GEO["num_layers"],
-                                        max_num_embedding=GEO["max_num_embedding"])
-    dec = st.SalienceTransformerDecoder(st.SalienceTransformerDecoderLayer(GEO["embed_dim"], GEO["d_ffn"], GEO["n_heads"], 0.0, relu,
-                                                                           4, 4), DEC_LAYERS, GEO["num_classes"])
-    tr = st.SalienceTransformer(enc, None, dec, GEO["num_classes"], 4, GEO["num_proposals"], GEO["level_filter_ratio"],
-                                GEO["layer_filter_ratio"])
-    with torch.no_grad():  # non-trivial heads: the reference zero-initialises the last bbox layers and the offset weights
-        for layer in list(tr.encoder.layers) + list(tr.decoder.layers):
-            attn = layer.self_attn if hasattr(layer, "pre_attention") else layer.cross_attn
-            attn.sampling_offsets.weight.normal_(0, 0.03)
-            attn.attention_weights.weight.normal_(0, 0.5)
-        for head in list(tr.decoder.bbox_head) + [tr.encoder_bbox_head]:
-            head.layers[-1].weight.normal_(0, 0.02)
-        tr.encoder_class_head.weight.normal_(0, 0.05)
-    return tr.to(DEV).eval()
+def _golden(ragged):
+    z = np.load(os.path.join(GOLDEN, "decoder_half_%s.npz" % ("ragged" if ragged else "even")), allow_pickle=False)
+    return {k: torch.from_numpy(z[k]) for k in z.files if k != "shapes_json"}, json.loads(str(z["shapes_json"]))
 
 
-def _ours(pkg, tr):
+def _ours(pkg, shapes):
+    """this package's transformer with a GEO["dec_layers"]-layer decoder and the fixture's weights (every reference key)"""
     relu = torch.nn.ReLU(inplace=True)
     enc = pkg.SalienceTransformerEncoder(pkg.SalienceTransformerEncoderLayer(GEO["embed_dim"], GEO["d_ffn"], 0.0, GEO["n_heads"], relu,
                                                                             4, 4, topk_sa=GEO["topk_sa"]), GEO["num_layers"],
                                          GEO["max_num_embedding"])
     dec = pkg.SalienceTransformerDecoder(pkg.SalienceTransformerDecoderLayer(GEO["embed_dim"], GEO["d_ffn"], GEO["n_heads"], 0.0, relu,
-                                                                            4, 4), DEC_LAYERS, GEO["num_classes"])
+                                                                            4, 4), GEO["dec_layers"], GEO["num_classes"])
     ours = pkg.SalienceTransformer(enc, None, dec, GEO["num_classes"], 4, GEO["num_proposals"], GEO["level_filter_ratio"],
                                    GEO["layer_filter_ratio"])
-    ours.load_state_dict(tr.state_dict(), strict=True)  # every reference key, decoder half included
+    res = ours.load_state_dict(orc.deterministic_state_dict(shapes, mg.HALF_SEED), strict=False)
+    assert not res.unexpected_keys and all(k.endswith("_filter_ratio") for k in res.missing_keys)
     return ours.to(DEV).eval()
 
 
 def _inputs(ragged):
-    sizes = [(480, 640), (400, 500)] if ragged else [(480, 640), (480, 640)]
-    feats, masks, pos = orc.synthetic_inputs(sizes, (480, 640), GEO["embed_dim"], seed=13)
+    feats, masks, pos = orc.synthetic_inputs(mg.image_sizes(ragged), (480, 640), GEO["embed_dim"], seed=mg.HALF_INPUT_SEED)
     return [f.to(DEV) for f in feats], [m.to(DEV) for m in masks], [p.to(DEV) for p in pos]
 
 
-def test_nms_on_topk_index_matches_torchvision(pkg, ref):
-    """sdetr_nms_topk_index vs the reference's own nms_on_topk_index (torchvision.ops.batched_nms), index for index."""
-    tr = _reference(ref)
+def test_nms_on_topk_index_matches_torchvision(pkg):
+    """sdetr_nms_topk_index vs the reference's own nms_on_topk_index (torchvision.ops.batched_nms), index for index: its
+    kept lists for the same seeded candidates are stored in tests/golden/nms_topk.npz (oracle/make_golden.py)."""
+    z = np.load(os.path.join(GOLDEN, "nms_topk.npz"))
     g = torch.Generator().manual_seed(0)
-    for shapes, k in [([(60, 80), (30, 40), (15, 20), (8, 10)], 1200), ([(100, 168), (50, 84), (25, 42), (13, 21)], 3600),
-                      ([(20, 20), (10, 10)], 450)]:
+    for i, (shapes, k) in enumerate([([(60, 80), (30, 40), (15, 20), (8, 10)], 1200),
+                                     ([(100, 168), (50, 84), (25, 42), (13, 21)], 3600), ([(20, 20), (10, 10)], 450)]):
         st = torch.tensor(shapes, device=DEV)
         lsi = torch.cat([st.new_zeros(1), st.prod(1).cumsum(0)[:-1]])
         nv = int(st.prod(1).sum())
         scores = torch.rand(2, nv, generator=g).to(DEV)  # distinct with probability 1: the order is unambiguous
         topk_scores, topk_index = torch.topk(scores, k, dim=1)
-        tr.two_stage_num_proposals = 900
-        want = tr.nms_on_topk_index(topk_scores, topk_index, st, lsi, iou_threshold=0.3)
+        want = torch.from_numpy(z[f"kept{i}"]).to(DEV)
         kept, count, flag = pkg.cabi.nms_topk_index(topk_index.contiguous(), shapes, 0.3)
         n = want.shape[1]
         assert int(count.min()) >= n and torch.equal(kept[:, :n], want)
@@ -104,62 +83,52 @@ def test_nms_on_topk_index_matches_torchvision(pkg, ref):
 
 
 @pytest.mark.parametrize("ragged", [False, True])
-def test_decoder_on_reference_inputs(pkg, ref, ragged):
-    """The decoder alone on the reference's own memory / proposals (identical inputs on both sides): class logits and boxes of
-    every layer within 1e-3, in the strict fp32-GEMM mode and in the default tensor-core mode."""
-    tr = _reference(ref)
-    ours = _ours(pkg, tr)
-    feats, masks, pos = _inputs(ragged)
-    cap = {}
-    dec_fwd = tr.decoder.forward
-
-    def spy(**kw):
-        cap.update(kw)
-        cap["out"] = dec_fwd(**kw)
-        return cap["out"]
-
-    tr.decoder.forward = spy
-    with torch.no_grad():
-        want = tr(feats, masks, pos, None, None, None)
-    del tr.decoder.forward
-    kw = {k: v for k, v in cap.items() if k != "out"}
+def test_decoder_on_reference_inputs(pkg, ragged):
+    """The decoder alone on identical inputs on both sides (the reference filter's padding mask, valid ratios and proposal boxes,
+    seeded memory, the learned target queries): class logits and boxes of every layer within 1e-3 / 1e-4 of the reference
+    decoder's, in the strict fp32-GEMM mode and in the default tensor-core mode; then with denoising queries and their attention
+    mask (salience_transformer.py:218-221)."""
+    g, shapes = _golden(ragged)
+    ours = _ours(pkg, shapes)
+    b = g["reference_points"].shape[0]
+    kw = dict(query=ours.tgt_embed.weight.expand(b, -1, -1),
+              value=orc.seeded_memory((b, int(g["key_padding_mask"].shape[1]), GEO["embed_dim"]), mg.HALF_VALUE_SEED).to(DEV),
+              key_padding_mask=g["key_padding_mask"].to(DEV), reference_points=g["reference_points"].to(DEV),
+              spatial_shapes=g["spatial_shapes"].to(DEV), level_start_index=g["level_start_index"].to(DEV),
+              valid_ratios=g["valid_ratios"].to(DEV), attn_mask=None)
     for mode in ("fp32", "auto"):
         pkg.gemm.MODE = mode
         n0 = pkg.cabi.launch_count()
         with torch.no_grad():
             cls, box = ours.decoder(**kw)
-        assert pkg.cabi.launch_count() > n0 + 3 * DEC_LAYERS
-        assert cls.shape == want[0].shape and box.shape == want[1].shape
-        assert (cls - cap["out"][0]).abs().max() < 1e-3, mode
-        assert (box - cap["out"][1]).abs().max() < 1e-4, mode
-    # denoising queries + attention mask pass through like in the reference (salience_transformer.py:218-221)
-    b, nq = kw["query"].shape[:2]
-    g = torch.Generator().manual_seed(4)
-    dn_q = torch.randn(b, 20, GEO["embed_dim"], generator=g).to(DEV)
-    dn_b = torch.rand(b, 20, 4, generator=g).to(DEV) * 0.5 + 0.25
-    mask = torch.zeros(nq + 20, nq + 20, dtype=torch.bool, device=DEV)
-    mask[20:, :20] = True
-    kw2 = dict(kw, query=torch.cat([dn_q, kw["query"]], 1), reference_points=torch.cat([dn_b, kw["reference_points"]], 1), attn_mask=mask)
+        assert pkg.cabi.launch_count() > n0 + 3 * GEO["dec_layers"]
+        assert cls.shape == g["dec_cls"].shape and box.shape == g["dec_box"].shape
+        assert (cls.cpu() - g["dec_cls"]).abs().max() < 1e-3, mode
+        assert (box.cpu() - g["dec_box"]).abs().max() < 1e-4, mode
+    dn_q, dn_b, mask = orc.denoising_queries(b, kw["query"].shape[1], GEO["embed_dim"])
+    kw2 = dict(kw, query=torch.cat([dn_q.to(DEV), kw["query"]], 1), reference_points=torch.cat([dn_b.to(DEV), kw["reference_points"]], 1),
+               attn_mask=mask.to(DEV))
     with torch.no_grad():
-        w2 = tr.decoder(**kw2)
         pkg.gemm.MODE = "auto"
         g2 = ours.decoder(**kw2)
-    assert (g2[0] - w2[0]).abs().max() < 1e-3 and (g2[1] - w2[1]).abs().max() < 1e-4
+    assert (g2[0].cpu() - g["dn_cls"]).abs().max() < 1e-3 and (g2[1].cpu() - g["dn_box"]).abs().max() < 1e-4
 
 
 @pytest.mark.parametrize("ragged", [False, True])
-def test_full_transformer_forward_vs_reference(pkg, ref, ragged):
+def test_full_transformer_forward_vs_reference(pkg, ragged):
     """Whole ``SalienceTransformer.forward`` (filter + encoder + two-stage selection + decoder), reference call signature and
     5-tuple of outputs.  Encoder memories differ by round-off, so near-tied proposals may swap: the proposal SETS must agree
     except for a few entries, and every query whose proposal agrees in position must agree in its outputs."""
-    tr = _reference(ref)
-    ours = _ours(pkg, tr)
+    g, shapes = _golden(ragged)
+    ours = _ours(pkg, shapes)
     feats, masks, pos = _inputs(ragged)
+    want = [g[f"full{i}"] for i in range(4)] + [[g[f"full_score{i}"] for i in range(len([k for k in g if k.startswith("full_score")]))]]
     with torch.no_grad():
-        want = tr(feats, masks, pos, None, None, None)
         pkg.gemm.MODE = "fp32"
         got = ours(feats, masks, pos, None, None, None)
+    got = [t.cpu() for t in got[:4]] + [[t.cpu() for t in got[4]]]
     assert len(got) == 5 and got[0].shape == want[0].shape and got[1].shape == want[1].shape
+    assert len(got[4]) == len(want[4])
     for a, w in zip(got[4], want[4]):  # salience score maps
         assert a.shape == w.shape and (a - w).abs().max() < 1e-4
     same = ((got[3] - want[3]).abs().amax(-1) < 1e-4)            # proposals equal position by position
@@ -169,48 +138,41 @@ def test_full_transformer_forward_vs_reference(pkg, ref, ragged):
         assert (got[0] - want[0]).abs().max() < 2e-3 and (got[1] - want[1]).abs().max() < 2e-4
 
 
-def test_neck_handoff_with_reference_repvgg(pkg, ref):
-    """SURVEY.md 8(f)-3: the encoder memory is handed to the RepVGG neck in per-level NCHW maps and comes back as tokens
-    (salience_transformer.py:185-192).  Layout kernels: exact round trip; then the reference's own RepVGGPluXNetwork
-    (models/necks/repnet.py:125-245, eval mode) plugged into OUR transformer against the reference transformer with the same
-    neck and weights: the memory that leaves the neck (captured at the decoder's `value` input) within 2e-3."""
-    if ref.repnet is None:
-        pytest.skip("baseline/_ref has no models/necks/repnet.py (re-run __graft_entry__.build())")
+def test_neck_handoff_vs_reference(pkg):
+    """SURVEY.md 8(f)-3: the encoder memory is handed to a convolutional neck in per-level NCHW maps and comes back as tokens
+    (salience_transformer.py:185-192).  Layout kernels: exact round trip; then a neck (oracle.ConvNeck, the reference's
+    dict-of-levels interface) plugged into OUR transformer against the reference transformer with the same neck and weights:
+    the memory that leaves the neck (captured at the decoder's `value` input) within 2e-3."""
     shapes = [(60, 80), (30, 40), (15, 20), (8, 10)]
-    g = torch.Generator().manual_seed(1)
-    tok = torch.randn(2, sum(h * w for h, w in shapes), 96, generator=g).to(DEV)
+    gen = torch.Generator().manual_seed(1)
+    tok = torch.randn(2, sum(h * w for h, w in shapes), 96, generator=gen).to(DEV)
     maps = pkg.cabi.tokens_to_maps(tok, shapes)
     want = [t.transpose(1, 2).reshape(2, 96, h, w) for t, (h, w) in zip(tok.split([h * w for h, w in shapes], 1), shapes)]
     assert all(torch.equal(a, b) for a, b in zip(maps, want))
     assert torch.equal(pkg.cabi.maps_to_tokens(maps), tok)
 
-    tr = _reference(ref)
-    torch.manual_seed(3)
-    neck = ref.repnet.RepVGGPluXNetwork([GEO["embed_dim"]] * 4, [GEO["embed_dim"]] * 4, norm_layer=torch.nn.BatchNorm2d,
-                                       activation=torch.nn.SiLU, groups=4).to(DEV).eval()
-    tr.neck = neck
-    ours = _ours(pkg, _reference(ref))      # same seed -> same weights as `tr` (the state_dict now also has neck.* keys)
-    ours.neck = neck
+    g, sd_shapes = _golden(False)
+    ours = _ours(pkg, sd_shapes)
+    ours.neck = orc.ConvNeck(GEO["embed_dim"], 4, seed=3).to(DEV).eval()
     feats, masks, pos = _inputs(False)
     cap = {}
 
-    def grab(store):
-        def spy(**kw):
-            store["value"] = kw["value"]
-            raise ref_import._Stop()
-        return spy
+    class _Stop(Exception):
+        pass
 
-    for model, key in ((tr, "ref"), (ours, "ours")):
-        cap[key] = {}
-        model.decoder.forward = grab(cap[key])
-        try:
-            with torch.no_grad():
-                if key == "ours":
-                    pkg.gemm.MODE = "fp32"
-                model(feats, masks, pos, None, None, None)
-        except ref_import._Stop:
-            pass
-        finally:
-            del model.decoder.forward
-    a, w = cap["ours"]["value"], cap["ref"]["value"]
-    assert a.shape == w.shape and (a - w).abs().max() < 2e-3 * max(1.0, w.abs().max().item())
+    def grab(**kw):
+        cap["value"] = kw["value"]
+        raise _Stop()
+
+    ours.decoder.forward = grab
+    try:
+        with torch.no_grad():
+            pkg.gemm.MODE = "fp32"
+            ours(feats, masks, pos, None, None, None)
+    except _Stop:
+        pass
+    finally:
+        del ours.decoder.forward
+    idx = g["neck_rows_index"].to(DEV)
+    a = torch.gather(cap["value"], 1, idx[..., None].expand(-1, -1, cap["value"].shape[2])).cpu()
+    assert (a - g["neck_rows"]).abs().max() < 2e-3 * max(1.0, float(g["neck_value_absmax"]))

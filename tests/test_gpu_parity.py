@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels (called through the C-ABI via salience_detr_b200.cabi) against the
+"""GPU parity tests: the sm_90a kernels (called through the C-ABI via salience_detr_b200.cabi) against the
 CPU oracle on identical seeded inputs, against the golden fixtures made from the reference, and -- at
 BASELINE.json's full sizes -- through size-independent properties.
 
@@ -34,13 +34,8 @@ def _restore_global_state(pkg):
     yield
     pkg.gemm.MODE = mode
     pkg.gemm.OWN_KERNEL = os.environ.get("SDETR_GEMM_KERNEL", "f16x3")
-    pkg.cabi.lib().sdetr_gemm_f16x3_set_as(0)
-    pkg.cabi.lib().sdetr_gemm_f16x3_set_cluster(0)
-    pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue(0)
-    pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue_warps(4)
+    pkg.cabi.lib().sdetr_set_persistent_ctas(0)
     pkg.cabi.set_option("msda_smem_broadcast", 1)
-    pkg.cabi.lib().sdetr_gemm_set_variant(0)
-    pkg.cabi.lib().sdetr_gemm_set_variant(3)
 
 
 def _msda_inputs(b, shapes, m, d, nq, p, seed):
@@ -563,7 +558,7 @@ def test_gemm_persistent_many_tiles_ragged_n(pkg):
 
 
 def test_gemm_tcgen05_3xtf32(pkg):
-    """Hand-written tcgen05 GEMM (TMA + in-kernel TF32 split + TMEM accumulator) against an fp64 reference."""
+    """Hand-written 3xTF32 wgmma GEMM (TMA + in-kernel TF32 split + register accumulator) against an fp64 reference."""
     g = torch.Generator().manual_seed(1)
     for rows, K, N, relu in [(128, 32, 128, False), (300, 256, 384, False), (4097, 256, 256, False), (1000, 2048, 256, True),
                              (333, 256, 91, False), (50, 64, 1, False), (22726, 256, 1536, False), (513, 128, 64, False)]:
@@ -576,17 +571,13 @@ def test_gemm_tcgen05_3xtf32(pkg):
         torch.cuda.synchronize()
         ref = torch.nn.functional.linear((x.relu() if relu else x).double(), w.double(), b.double())
         err = (y.double() - ref).abs().max().item()
-        assert err < 3e-4, (rows, K, N, err)  # TMEM accumulation truncates: grows with K (2e-4 at K = 2048)
+        assert err < 3e-4, (rows, K, N, err)  # tensor-core accumulation truncates: grows with K
         # no bias, strided rows (a column slice of a wider buffer)
         wide = torch.randn(rows, K + 32, generator=g).to(DEV)
         y2 = pkg.cabi.gemm_3xtf32(wide[:, 32:], w_hi, w_lo)
         ref2 = wide[:, 32:].double() @ w.double().t()
         assert (y2.double() - ref2).abs().max() < 1e-4
-        # the variants: TS (split activation in TMEM) and TS2 (both operands split in the kernel, 2 CTAs/SM)
-        pkg.cabi.lib().sdetr_gemm_set_variant(1)
-        y3 = pkg.cabi.gemm_3xtf32(x, w_hi, w_lo, b, relu)
-        pkg.cabi.lib().sdetr_gemm_set_variant(0)
-        assert torch.equal(y3, y)
+        # the raw-weight form (W split in the kernel) and the pre-split persistent entry point: same arithmetic
         y4 = pkg.cabi.gemm_3xtf32_raw(x, w, b, int(relu))
         assert y4.shape == y.shape and (y4.double() - ref).abs().max() < 3e-4
         y5 = pkg.cabi.gemm_3xtf32_pre(x, w_hi, w_lo, b, int(relu))  # persistent kernel, pre-split weight: same arithmetic
@@ -603,7 +594,7 @@ def test_gemm_tcgen05_3xtf32(pkg):
 
 
 def test_gemm_f16x3_accuracy_and_range(pkg):
-    """3xFP16 persistent kernel (tcgen05.mma.kind::f16 on hi/lo fp16 pairs, power-of-two range scalings) against an fp64
+    """3xFP16 persistent kernel (wgmma .f16 on hi/lo fp16 pairs, power-of-two range scalings) against an fp64
     reference: the same fp32-class error as 3xTF32 / SGEMM on O(1) data, across the documented activation range
     (2^-7 .. 4094 relative accuracy, absolute floor below), with the fused input activations, ragged N, strided rows,
     many tiles per CTA, and bit-reproducible."""
@@ -626,47 +617,24 @@ def test_gemm_f16x3_accuracy_and_range(pkg):
         e32 = (pkg.gemm.linear(x if act is None else (F.relu(x) if act == "relu" else F.gelu(x)), w, b).double() - ref).abs().max().item()
         assert err < 3e-4 and err < 32 * e32 + 1e-6, (rows, K, N, err, e32)
         assert torch.equal(pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, {None: 0, "relu": 1, "gelu": 2}[act]), y)
-    # activation-stationary variant (K <= 256, several output tiles per work unit): the same MMA sequence per tile as the
-    # streaming kernel, so the results are bit-identical
+    # the benched shapes and the awkward ones: wide N, long K, one-panel problems, ragged N, many tiles per CTA (also with
+    # the persistent grid capped at a few CTAs); bit-reproducible whatever the grid
     for rows, K, N, act in [(22726, 256, 2048, 0), (4544, 256, 2048, 1), (44646, 256, 1536, 0), (20000, 128, 640, 2),
-                            (19000, 64, 384, 0), (18180, 256, 384, 0), (40000, 192, 300, 0)]:
+                            (19000, 64, 384, 0), (18180, 256, 384, 0), (40000, 192, 300, 0), (22726, 2048, 256, 1), (129, 64, 128, 0),
+                            (385, 256, 91, 0), (100, 128, 256, 0), (36264, 256, 91, 2), (4544, 256, 384, 0)]:
         x = torch.randn(rows, K, generator=g).to(DEV)
         w = (torch.randn(N, K, generator=g) / K ** 0.5).to(DEV)
         b = torch.randn(N, generator=g).to(DEV)
         w_hi, w_lo, sc = pkg.cabi.split_f16_pair(w)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_as(0)
         y0 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_as(1)
-        y1 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
         xa = x.double() if act == 0 else (F.relu(x.double()) if act == 1 else F.gelu(x.double()))
-        assert (y1.double() - F.linear(xa, w.double(), b.double())).abs().max() < 1e-4, (rows, K, N)
-        assert torch.equal(y0, y1), (rows, K, N)
-        assert torch.equal(pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act), y1)
-    # cluster-of-two variant (weight k-blocks multicast to two adjacent panels): same MMA sequence per tile -> bit-identical;
-    # odd panel counts (a dummy out-of-range panel), one-panel problems (plain launch), ragged N, long K, many tiles per CTA
-    for rows, K, N, act in [(22726, 256, 2048, 0), (22726, 2048, 256, 1), (44646, 256, 1536, 0), (129, 64, 128, 0), (385, 256, 91, 0),
-                            (100, 128, 256, 0), (36264, 256, 91, 2), (19000, 64, 384, 0), (4544, 256, 384, 0)]:
-        x = torch.randn(rows, K, generator=g).to(DEV)
-        w = (torch.randn(N, K, generator=g) / K ** 0.5).to(DEV)
-        b = torch.randn(N, generator=g).to(DEV)
-        w_hi, w_lo, sc = pkg.cabi.split_f16_pair(w)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_cluster(0)
-        y0 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_cluster(1)
+        assert (y0.double() - F.linear(xa, w.double(), b.double())).abs().max() < 1e-4, (rows, K, N)
+        pkg.cabi.lib().sdetr_set_persistent_ctas(7)
         y1 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
+        pkg.cabi.lib().sdetr_set_persistent_ctas(0)
         assert torch.equal(y0, y1), (rows, K, N)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_cluster(0)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue(1)   # warp-private store epilogue: same values, different store path
-        y2 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue(0)
-        assert torch.equal(y0, y2), (rows, K, N)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue_warps(8)  # two groups of four epilogue warps instead of one
-        y3 = pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_epilogue_warps(4)
-        assert torch.equal(y0, y3), (rows, K, N)
-        pkg.cabi.lib().sdetr_gemm_f16x3_set_cluster(1)
         for _ in range(3):
-            assert torch.equal(pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act), y1)
+            assert torch.equal(pkg.cabi.gemm_f16x3_pre(x, w_hi, w_lo, sc, b, act), y0)
     # range: tiny, huge and mixed-magnitude activations; relative error of the result stays fp32-class
     K, N = 256, 256
     w = (torch.randn(N, K, generator=g) / 16).to(DEV)
@@ -1036,8 +1004,6 @@ def test_full_size_config2_properties(pkg):
     assert torch.equal(ic, wi) and torch.equal(sc, ws) and torch.equal(fg.cpu(), wf)
 
 
-# The reference itself at its real width; observed green on the driver's B200 at the end of round 1 (GPUTEST_r01: xpassed),
-# so it is a plain test now.
 def test_encoder_half_c256_vs_reference_golden(pkg):
     """The reference itself at its real width (C = 256, 8 heads of 32, 4080 tokens per image; fixture made by
     oracle/make_golden.py, weights / inputs regenerated from seeds): this geometry takes the paths specialised for the
@@ -1207,9 +1173,9 @@ def test_salience_targets_kernel_vs_reference_golden(pkg):
 
 
 def test_ffn_fused_layernorm(pkg):
-    """Fused FFN (hidden activations kept in tensor memory, sdetr_ffn_fused_layernorm) against an fp64 reference and against
-    the two-GEMM path: CTA ranges that cut panels (balanced) and whole-panel ranges, few / many CTAs (several units per CTA,
-    panels shared by three CTAs), ragged last panel, strided input rows, bare-FFN mode, in-place output, bit-reproducible."""
+    """Encoder FFN + LayerNorm (sdetr_ffn_fused_layernorm) against an fp64 reference and against the two-GEMM path: the full
+    grid and grids capped at a few CTAs (many tiles per CTA), ragged last panel, strided input rows, bare-FFN mode, in-place
+    output, bit-reproducible."""
     g = torch.Generator().manual_seed(11)
     F = torch.nn.functional
     lib = pkg.cabi.lib()
@@ -1227,17 +1193,15 @@ def test_ffn_fused_layernorm(pkg):
             ref = F.layer_norm(x.double() + f64, (256,), gamma.double(), beta.double(), 1e-5)
             two = pkg.cabi.gemm_f16x3_pre(pkg.cabi.gemm_f16x3_pre(x, *s1, b1, 0), *s2, b2, 1)
             e_two = (two.double() - f64).abs().max().item()
-            for balance, ctas in [(1, 0), (0, 0), (1, 7), (0, 5), (1, 97), (1, 1)]:
-                lib.sdetr_ffn_fused_set_balance(balance)
-                lib.sdetr_ffn_fused_set_max_ctas(ctas)
+            for ctas in (0, 7, 97, 1):
+                lib.sdetr_set_persistent_ctas(ctas)
                 bare = pkg.cabi.ffn_fused_layernorm(x, s1, b1, s2, b2)
                 err = (bare.double() - f64).abs().max().item()
-                assert err < 1e-4 and err < 4 * e_two + 1e-6, (rows, hidden, balance, ctas, err, e_two)
+                assert err < 1e-4 and err < 4 * e_two + 1e-6, (rows, hidden, ctas, err, e_two)
                 y = pkg.cabi.ffn_fused_layernorm(x, s1, b1, s2, b2, gamma, beta, 1e-5)
-                assert (y.double() - ref).abs().max().item() < 1e-4, (rows, hidden, balance, ctas)
+                assert (y.double() - ref).abs().max().item() < 1e-4, (rows, hidden, ctas)
                 assert torch.equal(pkg.cabi.ffn_fused_layernorm(x, s1, b1, s2, b2, gamma, beta, 1e-5), y)
-            lib.sdetr_ffn_fused_set_balance(1)
-            lib.sdetr_ffn_fused_set_max_ctas(0)
+            lib.sdetr_set_persistent_ctas(0)
             # in place (the layer's use) and strided input rows
             xin = x.clone()
             pkg.cabi.ffn_fused_layernorm(xin, s1, b1, s2, b2, gamma, beta, 1e-5, out=xin)
@@ -1252,8 +1216,7 @@ def test_ffn_fused_layernorm(pkg):
         bare = pkg.cabi.ffn_fused_layernorm(x, s1, b1, s2, b2)
         assert ((bare.double() - f64).abs().max() / f64.abs().max()).item() < 2e-6
     finally:
-        lib.sdetr_ffn_fused_set_balance(1)
-        lib.sdetr_ffn_fused_set_max_ctas(0)
+        lib.sdetr_set_persistent_ctas(0)
 
 
 def test_mask_predictor_level(pkg):

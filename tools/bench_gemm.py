@@ -1,4 +1,4 @@
-"""Per-shape timing of the dense projections: hand-written tcgen05 3xTF32 GEMM vs cuBLAS 3xTF32 (split pass + TF32
+"""Per-shape timing of the dense projections: hand-written wgmma 3xTF32 GEMM vs cuBLAS 3xTF32 (split pass + TF32
 GEMM) vs cuBLAS fp32 SGEMM, on the GEMM shapes of the bench workload (layer 0 and layer 5 query counts)."""
 import os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

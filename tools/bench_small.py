@@ -1,5 +1,5 @@
 """Latency of the small (launch-bound) pieces with a warm L2, as they run inside a step: small-M dense projections
-(hand-written tcgen05 kernel vs cuBLAS fp32) and the 300-token pre-attention (fused kernels vs library path)."""
+(hand-written wgmma kernel vs cuBLAS fp32) and the 300-token pre-attention (fused kernels vs library path)."""
 import os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -39,7 +39,7 @@ def graph_time(fn, reps=20, inner=20):
     return statistics.median(ts)
 
 
-print("small dense projections, per call inside a CUDA graph (us): own tcgen05 kernel | cuBLAS fp32")
+print("small dense projections, per call inside a CUDA graph (us): own wgmma kernel | cuBLAS fp32")
 for name, M, K, N, act in [("mask l3 fc1", 546, 256, 256, None), ("mask l3 fc2", 546, 256, 128, None), ("mask l3 fc3", 546, 128, 64, "gelu"),
                            ("mask l3 fc4", 546, 64, 1, "gelu"), ("mask l2 fc1", 2100, 256, 256, None), ("mask l2 fc3", 2100, 128, 64, "gelu"),
                            ("mask l1 fc1", 8400, 256, 256, None), ("mask l1 fc2", 8400, 256, 128, None), ("mask l1 fc3", 8400, 128, 64, "gelu"),

@@ -1,5 +1,5 @@
 // Kernel-to-kernel gap inside a CUDA graph on this GPU, with and without programmatic dependent launch, for small kernels and
-// for kernels that opt into the maximum dynamic shared memory (carve-out switches).  nvcc -arch=sm_100a -o launch_gap launch_gap.cu
+// for kernels that opt into the maximum dynamic shared memory (carve-out switches).  nvcc -arch=sm_90a -o launch_gap launch_gap.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <vector>
@@ -75,14 +75,14 @@ int main() {
     const int n = 200;
     for (int pdl = 0; pdl < 2; ++pdl) {
         printf("pdl=%d  small 1 CTA:            %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int) { launch_attr(small_kernel, 1, 32, 0, s, pdl, p, pdl); }));
-        printf("pdl=%d  small 148 CTAs x 256:   %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int) { launch_attr(small_kernel, 148, 256, 0, s, pdl, p, pdl); }));
-        printf("pdl=%d  227 KB smem 148 x 512:  %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int) { launch_attr(big_kernel, 148, 512, big, s, pdl, p, pdl); }));
+        printf("pdl=%d  small 132 CTAs x 256:   %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int) { launch_attr(small_kernel, 132, 256, 0, s, pdl, p, pdl); }));
+        printf("pdl=%d  227 KB smem 132 x 512:  %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int) { launch_attr(big_kernel, 132, 512, big, s, pdl, p, pdl); }));
         printf("pdl=%d  alternating small/227KB: %.2f us per node\n", pdl, time_graph(n, [&](cudaStream_t s, int i) {
-            if (i & 1) launch_attr(big_kernel, 148, 512, big, s, pdl, p, pdl); else launch_attr(small_kernel, 148, 256, 0, s, pdl, p, pdl); }));
+            if (i & 1) launch_attr(big_kernel, 132, 512, big, s, pdl, p, pdl); else launch_attr(small_kernel, 132, 256, 0, s, pdl, p, pdl); }));
         for (int iters : {2000, 20000}) {
-            printf("pdl=%d  busy(%d iters) 227 KB 148 x 512: %.2f us per node\n", pdl, iters, time_graph(n, [&](cudaStream_t s, int) { launch_attr(busy_kernel, 148, 512, big, s, pdl, p, pdl, iters); }));
+            printf("pdl=%d  busy(%d iters) 227 KB 132 x 512: %.2f us per node\n", pdl, iters, time_graph(n, [&](cudaStream_t s, int) { launch_attr(busy_kernel, 132, 512, big, s, pdl, p, pdl, iters); }));
             printf("pdl=%d  busy(%d iters) alternating with small: %.2f us per PAIR\n", pdl, iters, 2 * time_graph(n, [&](cudaStream_t s, int i) {
-                if (i & 1) launch_attr(busy_kernel, 148, 512, big, s, pdl, p, pdl, iters); else launch_attr(small_kernel, 148, 256, 0, s, pdl, p, pdl); }));
+                if (i & 1) launch_attr(busy_kernel, 132, 512, big, s, pdl, p, pdl, iters); else launch_attr(small_kernel, 132, 256, 0, s, pdl, p, pdl); }));
         }
     }
     return 0;

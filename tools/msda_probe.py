@@ -86,5 +86,5 @@ for spec in variants:
     err = max((o - r).abs().max().item() for o, r in zip(outs, ref_out))
     for mode in ("cold", "warm", "allhit"):
         t = run(mode)
-        cyc = sum(t) * 1e-6 * 1.965e9 * 148 / sum(items)
+        cyc = sum(t) * 1e-6 * 1.98e9 * torch.cuda.get_device_properties(0).multi_processor_count / sum(items)  # at the H100 SXM max SM clock
         print(f"{name:18s} {mode:6s} | " + " ".join(f"{x:6.1f}" for x in t) + f" | {sum(t):7.1f} | {sum(byts) / sum(t) / 1e3:7.1f} | {cyc:6.1f} | {err:.1e}")

@@ -1,9 +1,9 @@
 """One encoder-half forward at the bench workload inside cudaProfilerStart/Stop, for ncu:
 
   ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv \
-      --log-file gpurun_out/launches.csv python tools/profile_step.py
+      --log-file out/launches.csv python tools/profile_step.py
   ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:msda_fwd \
-      -o gpurun_out/msda python tools/profile_step.py
+      -o out/msda python tools/profile_step.py
 """
 import argparse
 import os

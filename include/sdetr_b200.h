@@ -391,14 +391,15 @@ int sdetr_mask_predictor_level(const float *mem, int64_t mem_batch_stride, int b
 
 /* ---- encoder FFN: y = LayerNorm(x + linear2(ReLU(linear1(x)))) ------------------------------------------------------------
  * Replaces `forward_ffn` + `norm2` of the encoder layer (models/bricks/salience_transformer.py:347-351, :391) for embed_dim 256:
- * linear1 and linear2 (the ReLU fused into its operand load) on the 3xFP16 kernel, then a row kernel adds the residual and
- * normalises.
+ * one persistent kernel computes linear1, ReLU and linear2 per 64-row panel with the hidden activations kept in shared memory,
+ * and adds the residual and normalises in its epilogue; panels whose hidden chunks are spread over several CTAs are summed
+ * (in a fixed order: bit-reproducible) and normalised by a second, row-wise launch.
  * Same 3xFP16 arithmetic and value domain as sdetr_gemm_f16x3_pre (both weights given as sdetr_split_f16_pair pairs with
  * their scales; W1 (hidden,256), W2 (256,hidden); hidden % 128 == 0).
  * x (M,256) fp32 with row pitch ldx (floats); y (M,256) contiguous, may alias x when ldx == 256;
- * gamma == beta == NULL: y = linear2(ReLU(linear1(x))) without residual / LayerNorm.
- * workspace: sdetr_ffn_fused_workspace_floats(M, hidden) = M * (hidden + 256) floats (the hidden activations and linear2's
- * output). */
+ * gamma == beta == NULL: y = linear2(ReLU(linear1(x))) without residual / LayerNorm.  b2 == NULL: linear2 without bias.
+ * workspace: sdetr_ffn_fused_workspace_floats(M, hidden) = M * (hidden + 256) floats, an upper bound (per-CTA partial sums of
+ * shared panels; the grid is narrowed to what it holds). */
 int64_t sdetr_ffn_fused_workspace_floats(int M, int hidden);
 int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *W1_hi, const void *W1_lo, float w1_scale, const float *b1,
                               const void *W2_hi, const void *W2_lo, float w2_scale, const float *b2, const float *gamma,

@@ -1,54 +1,347 @@
 // Encoder FFN -- sdetr_ffn_fused_layernorm:   y = LayerNorm(x + linear2(ReLU(linear1(x))))
 // (reference models/bricks/salience_transformer.py:347-351 `forward_ffn` + :391 `norm2`; C = 256, any hidden width % 128 == 0).
 //
-// Three launches on the 3xFP16 wgmma kernel of wgmma.cuh (same error-compensated products, scalings and accumulation as
-// sdetr_gemm_f16x3_pre, fp32-class accuracy):
-//   H = x W1^T + b1                       (M, hidden) fp32 in the workspace
-//   P = ReLU(H) W2^T + b2                 the ReLU is fused into the second GEMM's operand load; P goes to the workspace, or
-//                                         straight to y without LayerNorm
-//   y = LayerNorm(x + P) * gamma + beta   ffn_finish_kernel, one warp per row (x may alias y).
-// Deterministic: no atomics, a fixed reduction order per row.
+// One persistent sm_90a kernel keeps the hidden activations on chip: only the weights stream from L2.  The arithmetic is
+// that of sdetr_gemm_f16x3_pre applied twice (3xFP16 error-compensated products, exact power-of-two scalings, every
+// 64-wide k-block's tensor-core product added into the fp32 sum with a round-to-nearest add):
+//   H = acc1 * 2^-(4+s1) + b1  ->  ReLU  ->  x16  ->  fp16 hi / lo        per 128-wide hidden chunk, in shared memory
+//   OUT += H . W2[:, chunk]^T                                             fp32 registers, 64 rows x 256 per CTA
+//   y = LayerNorm(x + OUT * 2^-(4+s2) + b2) * gamma + beta                (or y = OUT * 2^-(4+s2) + b2 without gamma / beta)
+//
+// Work: a unit is one (64-row panel, hidden chunk); CTA i of G takes units [U i / G, U (i+1) / G) of U = panels * chunks,
+// so small layers still fill the GPU.  A panel whose chunks all fall to one CTA is finished in that CTA's epilogue (x may
+// alias y: only that CTA reads those rows).  A panel shared by several CTAs gets per-CTA raw sums in the workspace; a
+// second launch (ffn_finish_kernel) adds them in CTA order and applies bias, residual and LayerNorm.  No atomics: the
+// result is bit-reproducible at a given grid.
+//
+// CTA: warpgroup 0, one thread, is the TMA producer of a ring of 32 KB weight stages (W hi + lo, 128 rows x 64 k each:
+// per chunk 4 stages of W1 (K = 256), then W2 k-blocks 0 and 1 for output columns 0-127 and 128-255).  Warpgroups 1 and 2
+// share the 64 rows of the panel and split the columns: for linear1 each computes 64 of the chunk's 128 hidden columns
+// (m64n64, x hi / lo read from shared memory, where it was split once per panel), writes them as hi / lo fp16 into a
+// double-buffered H tile, and after a barrier between the two computes its 128 output columns of linear2 (m64n128, H from
+// shared memory).  Registers: setmaxnreg moves them from the producer warpgroup (40) to the consumers (232 each).
 #include "wgmma.cuh"
 
 namespace sdetr {
 
-constexpr int kFD = 256;  // model width: K of linear1, N of linear2
+constexpr int kFD = 256;                          // model width: K of linear1, N of linear2
+constexpr int kFM = 64;                           // rows of a panel
+constexpr int kFTile = kFM * 128;                 // 8 KB: 64 rows x 64 fp16, SWIZZLE_128B
+constexpr int kFXBytes = 2 * (kFD / 64) * kFTile; // x hi, x lo: 4 k-block tiles each
+constexpr int kFHBytes = 4 * kFTile;              // one H chunk buffer: hi tiles 0, 1 then lo tiles 0, 1
+constexpr int kFStageBytes = 2 * kGBox;           // W hi, W lo boxes of 128 rows x 64 fp16
+constexpr int kFStages = 3;
+constexpr int kFSlot = kFM * kFD;                 // floats of one partial panel in the workspace
+constexpr int kFSmem = kFXBytes + 2 * kFHBytes + kFStages * kFStageBytes + 1024 /* alignment */ + 1024 /* barriers, row sums */;
 
-__global__ void __launch_bounds__(256) ffn_finish_kernel(const float *x /* may alias y */, int64_t ldx, const float *__restrict__ partial,
-                                                         const float *__restrict__ gamma, const float *__restrict__ beta, float eps,
-                                                         int64_t rows, float *y) {
+struct FfnParams {
+    const float *x;  // may alias y
+    int64_t ldx;
+    const float *b1, *b2, *gamma, *beta;
+    float eps, out1, out2;  // out1, out2: 1 / (kActScale * w_scale) of linear1, linear2
+    int M, chunks, units;
+    float *part;  // CTA i's partial panels: slot 2i (its first panel) and 2i + 1 (its last)
+    float *y;
+};
+
+__host__ __device__ inline int ffn_range_lo(int i, int units, int ctas) { return (int)((int64_t)units * i / ctas); }
+
+__device__ __forceinline__ void proxy_fence_and_sync() {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> wgmma operand reads
+    named_bar_sync(1, 256);
+}
+
+__global__ void __launch_bounds__(kGThreads, 1)
+    ffn_fused_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constant__ CUtensorMap m1l,
+                     const __grid_constant__ CUtensorMap m2h, const __grid_constant__ CUtensorMap m2l, const FfnParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *xs = smem, *hs = smem + kFXBytes, *ring = hs + 2 * kFHBytes;
+    uint64_t *full = reinterpret_cast<uint64_t *>(ring + kFStages * kFStageBytes), *empty = full + kFStages;
+    float *red = reinterpret_cast<float *>(empty + kFStages + 2);  // [2 warpgroups][64 rows]
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kFStages; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 8);  // 8 consumer warps release
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const int lo = ffn_range_lo(blockIdx.x, p.units, gridDim.x), hi = ffn_range_lo(blockIdx.x + 1, p.units, gridDim.x);
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+
+    if (wg == 0) {  // ---- producer
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (tid == 0) {
+            int s = 0;
+            uint32_t ph = 0;
+            for (int u = lo; u < hi; ++u) {
+                const int h0 = (u % p.chunks) * 128;
+                for (int t = 0; t < 8; ++t) {
+                    mbar_wait(empty + s, ph ^ 1);
+                    uint8_t *st = ring + s * kFStageBytes;
+                    mbar_expect_tx(full + s, 2 * kGBox);
+                    if (t < 4) {  // W1 rows [h0, h0 + 128), k-block t
+                        tma_load_2d(&m1h, full + s, st, t * 64, h0);
+                        tma_load_2d(&m1l, full + s, st + kGBox, t * 64, h0);
+                    } else {      // W2 rows (output columns) [128 half, +128), k-block kb of the chunk
+                        const int kb = (t - 4) >> 1, half = (t - 4) & 1;
+                        tma_load_2d(&m2h, full + s, st, h0 + kb * 64, half * 128);
+                        tma_load_2d(&m2l, full + s, st + kGBox, h0 + kb * 64, half * 128);
+                    }
+                    if (++s == kFStages) s = 0, ph ^= 1;
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- consumers: warpgroup cw = wg - 1 owns hidden columns [64 cw, 64 cw + 64) of every chunk and output columns
+    // [128 cw, 128 cw + 128)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1, ctid = threadIdx.x - 128;
+    const int warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    const int r0 = warp * 16 + g;  // this thread's fragment rows: r0, r0 + 8
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[64], d[64], acc1[32], d1[32];
+    for (int u = lo; u < hi;) {
+        const int pnl = u / p.chunks, c_begin = u % p.chunks, c_end = min(p.chunks, c_begin + (hi - u));
+        const int64_t m0 = (int64_t)pnl * kFM;
+        // x panel -> x16, hi / lo fp16, swizzled k-block tiles (the previous panel's readers passed the last chunk barrier)
+        for (int i = ctid; i < kFM * kFD / 4; i += 256) {
+            const int r = i >> 6, c4 = i & 63;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (m0 + r < p.M) v = *reinterpret_cast<const float4 *>(p.x + (m0 + r) * p.ldx + 4 * c4);
+            uint2 h, l;
+            split2(v.x * kActScale, v.y * kActScale, h.x, l.x);
+            split2(v.z * kActScale, v.w * kActScale, h.y, l.y);
+            const int off = (c4 >> 4) * kFTile + r * 128 + ((((c4 & 15) >> 1) ^ (r & 7)) << 4) + (c4 & 1) * 8;
+            *reinterpret_cast<uint2 *>(xs + off) = h;
+            *reinterpret_cast<uint2 *>(xs + kFXBytes / 2 + off) = l;
+        }
+        proxy_fence_and_sync();
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int c = c_begin; c < c_end; ++c) {
+            // linear1: H[:, 64 cw .. +64) of chunk c, K = 256 in 4 k-blocks
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
+            for (int kb = 0; kb < 4; ++kb) {
+                mbar_wait(full + s, ph);
+                const uint32_t bh = smem_u32(ring + s * kFStageBytes) + cw * kFTile, bl = bh + kGBox;
+                const uint32_t xh = smem_u32(xs) + kb * kFTile, xl = xh + kFXBytes / 2;
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    wgmma_f16_ss_n64(d1, wgmma_desc(xl + kk * 32), wgmma_desc(bh + kk * 32), kk);
+                    wgmma_f16_ss_n64(d1, wgmma_desc(xh + kk * 32), wgmma_desc(bl + kk * 32), 1);
+                    wgmma_f16_ss_n64(d1, wgmma_desc(xh + kk * 32), wgmma_desc(bh + kk * 32), 1);
+                }
+                wgmma_commit();
+                wgmma_wait_all();
+                if (lane == 0) mbar_arrive(empty + s);
+                if (++s == kFStages) s = 0, ph ^= 1;
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc1[i] += d1[i];
+            }
+            // H = acc1 * out1 + b1 -> ReLU -> x16 -> hi / lo into H tile cw of buffer c & 1 (its readers of chunk c - 2
+            // passed the barrier of chunk c - 1)
+            uint8_t *hb = hs + (c & 1) * kFHBytes;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int col = c * 128 + cw * 64 + 8 * j + 2 * q;
+                const float bb0 = __ldg(p.b1 + col), bb1 = __ldg(p.b1 + col + 1);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const float v0 = fmaxf(acc1[4 * j + 2 * h] * p.out1 + bb0, 0.f) * kActScale;
+                    const float v1 = fmaxf(acc1[4 * j + 2 * h + 1] * p.out1 + bb1, 0.f) * kActScale;
+                    uint32_t vh, vl;
+                    split2(v0, v1, vh, vl);
+                    const int off = cw * kFTile + r * 128 + ((j ^ (r & 7)) << 4) + 4 * q;
+                    *reinterpret_cast<uint32_t *>(hb + off) = vh;
+                    *reinterpret_cast<uint32_t *>(hb + 2 * kFTile + off) = vl;
+                }
+            }
+            proxy_fence_and_sync();
+            // linear2: OUT[:, 128 cw .. +128) += H(chunk c) . W2^T, 2 k-blocks; the other warpgroup's stages are released
+            // unread
+            const uint32_t ah0 = smem_u32(hb);
+            for (int t = 0; t < 4; ++t) {
+                const int kb = t >> 1;
+                mbar_wait(full + s, ph);
+                if ((t & 1) == cw) {
+                    const uint32_t bh = smem_u32(ring + s * kFStageBytes), bl = bh + kGBox;
+                    const uint32_t ah = ah0 + kb * kFTile, al = ah + 2 * kFTile;
+                    wgmma_fence();
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+                        wgmma_f16_ss(d, wgmma_desc(al + kk * 32), wgmma_desc(bh + kk * 32), kk);
+                        wgmma_f16_ss(d, wgmma_desc(ah + kk * 32), wgmma_desc(bl + kk * 32), 1);
+                        wgmma_f16_ss(d, wgmma_desc(ah + kk * 32), wgmma_desc(bh + kk * 32), 1);
+                    }
+                    wgmma_commit();
+                    wgmma_wait_all();
+                }
+                if (lane == 0) mbar_arrive(empty + s);
+                if (++s == kFStages) s = 0, ph ^= 1;
+                if ((t & 1) == cw) {
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) acc[i] += d[i];
+                }
+            }
+        }
+        // epilogue: acc[4j + {0,1}] = (row r0, cols 128 cw + 8j + 2q + {0,1}), acc[4j + {2,3}] = (row r0 + 8, same cols)
+        if (c_begin == 0 && c_end == p.chunks) {
+            float b2v[32];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int col = cw * 128 + 8 * j + 2 * q;
+                b2v[2 * j] = p.b2 ? __ldg(p.b2 + col) : 0.f, b2v[2 * j + 1] = p.b2 ? __ldg(p.b2 + col + 1) : 0.f;
+            }
+            if (p.gamma) {
+                float sum[2] = {0.f, 0.f};
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t row = m0 + r0 + 8 * h;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int col = cw * 128 + 8 * j + 2 * q;
+                        float2 xv = make_float2(0.f, 0.f);
+                        if (row < p.M) xv = *reinterpret_cast<const float2 *>(p.x + row * p.ldx + col);
+                        float &a0 = acc[4 * j + 2 * h], &a1 = acc[4 * j + 2 * h + 1];
+                        a0 = xv.x + (a0 * p.out2 + b2v[2 * j]);
+                        a1 = xv.y + (a1 * p.out2 + b2v[2 * j + 1]);
+                        sum[h] += a0 + a1;
+                    }
+                }
+                float mean[2], rstd[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+                    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+                    if (q == 0) red[cw * kFM + r0 + 8 * h] = sum[h];
+                }
+                named_bar_sync(1, 256);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) mean[h] = (red[r0 + 8 * h] + red[kFM + r0 + 8 * h]) / (float)kFD;
+                named_bar_sync(1, 256);
+                float ss[2] = {0.f, 0.f};
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const float e0 = acc[4 * j + 2 * h] - mean[h], e1 = acc[4 * j + 2 * h + 1] - mean[h];
+                        ss[h] += e0 * e0 + e1 * e1;
+                    }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 1);
+                    ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 2);
+                    if (q == 0) red[cw * kFM + r0 + 8 * h] = ss[h];
+                }
+                named_bar_sync(1, 256);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    rstd[h] = rsqrtf((red[r0 + 8 * h] + red[kFM + r0 + 8 * h]) / (float)kFD + p.eps);
+                named_bar_sync(1, 256);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t row = m0 + r0 + 8 * h;
+                    if (row >= p.M) continue;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int col = cw * 128 + 8 * j + 2 * q;
+                        const float2 gm = *reinterpret_cast<const float2 *>(p.gamma + col);
+                        const float2 bt = *reinterpret_cast<const float2 *>(p.beta + col);
+                        *reinterpret_cast<float2 *>(p.y + row * kFD + col) =
+                            make_float2((acc[4 * j + 2 * h] - mean[h]) * rstd[h] * gm.x + bt.x,
+                                        (acc[4 * j + 2 * h + 1] - mean[h]) * rstd[h] * gm.y + bt.y);
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t row = m0 + r0 + 8 * h;
+                    if (row >= p.M) continue;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int col = cw * 128 + 8 * j + 2 * q;
+                        *reinterpret_cast<float2 *>(p.y + row * kFD + col) =
+                            make_float2(acc[4 * j + 2 * h] * p.out2 + b2v[2 * j], acc[4 * j + 2 * h + 1] * p.out2 + b2v[2 * j + 1]);
+                    }
+                }
+            }
+        } else {  // raw partial sums of a shared panel
+            float *dst = p.part + (int64_t)(2 * blockIdx.x + (u == lo ? 0 : 1)) * kFSlot;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    *reinterpret_cast<float2 *>(dst + (r0 + 8 * h) * kFD + cw * 128 + 8 * j + 2 * q) =
+                        make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+        u += c_end - c_begin;
+    }
+}
+
+// Rows of panels shared by several CTAs: OUT = the CTAs' partial sums in CTA order, y = LayerNorm(x + OUT * out2 + b2) (or
+// OUT * out2 + b2 without gamma / beta).  One warp per row; rows of panels finished in the fused kernel return at once.
+__global__ void __launch_bounds__(256) ffn_finish_kernel(const FfnParams p, int ctas) {
     const int lane = threadIdx.x & 31;
     const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (row >= rows) return;
-    float4 v[2];
+    if (row >= p.M) return;
+    const int pnl = (int)(row / kFM), u0 = pnl * p.chunks, u1 = u0 + p.chunks - 1;
+    int i0 = (int)((int64_t)u0 * ctas / p.units);
+    while (ffn_range_lo(i0 + 1, p.units, ctas) <= u0) ++i0;
+    int i1 = i0;
+    while (ffn_range_lo(i1 + 1, p.units, ctas) <= u1) ++i1;
+    if (i0 == i1) return;
+    float4 v[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+    for (int i = i0; i <= i1; ++i) {
+        const int first = ffn_range_lo(i, p.units, ctas) / p.chunks;
+        const float *src = p.part + (int64_t)(2 * i + (pnl == first ? 0 : 1)) * kFSlot + (row % kFM) * kFD;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const float4 a = *reinterpret_cast<const float4 *>(src + k * 128 + lane * 4);
+            v[k].x += a.x, v[k].y += a.y, v[k].z += a.z, v[k].w += a.w;
+        }
+    }
     float s = 0.f;
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const int c = i * 128 + lane * 4;
-        const float4 a = ld_stream_f4(partial + row * kFD + c), r = *reinterpret_cast<const float4 *>(x + row * ldx + c);
-        v[i] = make_float4(r.x + a.x, r.y + a.y, r.z + a.z, r.w + a.w);
-        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    for (int k = 0; k < 2; ++k) {
+        const int c = k * 128 + lane * 4;
+        const float4 b = p.b2 ? ldg_f4(p.b2 + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[k].x = v[k].x * p.out2 + b.x, v[k].y = v[k].y * p.out2 + b.y, v[k].z = v[k].z * p.out2 + b.z, v[k].w = v[k].w * p.out2 + b.w;
+        if (p.gamma) {
+            const float4 r = *reinterpret_cast<const float4 *>(p.x + row * p.ldx + c);
+            v[k].x += r.x, v[k].y += r.y, v[k].z += r.z, v[k].w += r.w;
+        }
+        s += (v[k].x + v[k].y) + (v[k].z + v[k].w);
+    }
+    if (!p.gamma) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) *reinterpret_cast<float4 *>(p.y + row * kFD + k * 128 + lane * 4) = v[k];
+        return;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const float mean = s / (float)kFD;
     float ss = 0.f;
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const float dx = v[i].x - mean, dy = v[i].y - mean, dz = v[i].z - mean, dw = v[i].w - mean;
+    for (int k = 0; k < 2; ++k) {
+        const float dx = v[k].x - mean, dy = v[k].y - mean, dz = v[k].z - mean, dw = v[k].w - mean;
         ss += (dx * dx + dy * dy) + (dz * dz + dw * dw);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    const float rstd = rsqrtf(ss / (float)kFD + eps);
+    const float rstd = rsqrtf(ss / (float)kFD + p.eps);
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const int c = i * 128 + lane * 4;
-        const float4 g = ldg_f4(gamma + c), bt = ldg_f4(beta + c);
+    for (int k = 0; k < 2; ++k) {
+        const int c = k * 128 + lane * 4;
+        const float4 gm = ldg_f4(p.gamma + c), bt = ldg_f4(p.beta + c);
         float4 o;
-        o.x = (v[i].x - mean) * rstd * g.x + bt.x, o.y = (v[i].y - mean) * rstd * g.y + bt.y;
-        o.z = (v[i].z - mean) * rstd * g.z + bt.z, o.w = (v[i].w - mean) * rstd * g.w + bt.w;
-        *reinterpret_cast<float4 *>(y + row * kFD + c) = o;
+        o.x = (v[k].x - mean) * rstd * gm.x + bt.x, o.y = (v[k].y - mean) * rstd * gm.y + bt.y;
+        o.z = (v[k].z - mean) * rstd * gm.z + bt.z, o.w = (v[k].w - mean) * rstd * gm.w + bt.w;
+        *reinterpret_cast<float4 *>(p.y + row * kFD + c) = o;
     }
 }
 
@@ -58,7 +351,7 @@ using namespace sdetr;
 
 extern "C" int64_t sdetr_ffn_fused_workspace_floats(int M, int hidden) {
     if (M <= 0 || hidden <= 0 || hidden % 128) return 0;
-    return (int64_t)M * (hidden + kFD);  // H, then P
+    return (int64_t)M * (hidden + kFD);  // an upper bound: the kernel uses at most two 64 x 256 slots per CTA
 }
 
 extern "C" int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *w1_hi, const void *w1_lo, float w1_scale,
@@ -81,13 +374,23 @@ extern "C" int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void
                       make_map_2d(&m2h, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_hi, kFD, hidden, hidden, 64, kGN) &&
                       make_map_2d(&m2l, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, w2_lo, kFD, hidden, hidden, 64, kGN),
                   SDETR_ERR_CUDA, "ffn_fused: cuTensorMapEncodeTiled failed");
-    float *h = workspace, *part = gamma ? workspace + (int64_t)M * hidden : y;
-    const Gemm3xParams p1{b1, h, hidden, M, hidden, kFD, 0, kActScale, 1.f / (kActScale * w1_scale), nullptr, nullptr};
-    int rc = launch_gemm3x<true, false>(x, ldx, m1h, m1l, p1, stream, "ffn_fused/linear1");
-    if (rc != SDETR_OK) return rc;
-    const Gemm3xParams p2{b2, part, kFD, M, kFD, hidden, 1, kActScale, 1.f / (kActScale * w2_scale), nullptr, nullptr};
-    rc = launch_gemm3x<true, false>(h, hidden, m2h, m2l, p2, stream, "ffn_fused/linear2");
-    if (rc != SDETR_OK || !gamma) return rc;
-    ffn_finish_kernel<<<(unsigned)((M + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, ldx, part, gamma, beta, eps, M, y);
+    const int chunks = hidden / 128, units = ((M + kFM - 1) / kFM) * chunks;
+    int ctas = persistent_ctas();
+    if (ctas > units) ctas = units;
+    // The grid is narrowed to the CTAs whose two 64 x 256 partial panels fit in the workspace of M * (hidden + 256) floats.
+    // That only binds for small M: at hidden 2048 it allows about M / 14 CTAs (M = 64: 4), which passes an H100's SM count
+    // from about 1900 rows on.
+    const int64_t slot_ctas = workspace_floats / (2 * kFSlot);
+    if (chunks > 1 && ctas > slot_ctas) ctas = slot_ctas > 1 ? (int)slot_ctas : 1;
+    const FfnParams p{x, ldx, b1, b2, gamma, beta, eps, 1.f / (kActScale * w1_scale), 1.f / (kActScale * w2_scale),
+                      M, chunks, units, workspace, y};
+    static PerDeviceOnce once;
+    SDETR_OPT_IN_SMEM(once, ffn_fused_kernel, kFSmem, "ffn_fused");
+    ffn_fused_kernel<<<ctas, kGThreads, kFSmem, (cudaStream_t)stream>>>(m1h, m1l, m2h, m2l, p);
+    int rc = check_launch("ffn_fused");
+    bool shared_panel = false;  // some CTA's range starts inside a panel
+    for (int i = 1; i < ctas && !shared_panel; ++i) shared_panel = ffn_range_lo(i, units, ctas) % chunks != 0;
+    if (rc != SDETR_OK || !shared_panel) return rc;
+    ffn_finish_kernel<<<(unsigned)((M + 7) / 8), 256, 0, (cudaStream_t)stream>>>(p, ctas);
     return check_launch("ffn_fused/finish");
 }

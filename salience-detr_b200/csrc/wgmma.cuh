@@ -101,6 +101,32 @@ __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[64], const uint32_t (&a
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
 }
 
+#define SDETR_WGMMA_D32                                                                                                           \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, " \
+    "%27, %28, %29, %30, %31}, "
+#define SDETR_WGMMA_D32_OPS(d)                                                                                                    \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),       \
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),      \
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),      \
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// d (64 x 128 fp32 per warpgroup) = (accumulate ? d : 0) + a (64 x 16 fp16) . b (16 x 128 fp16), both K-major in shared memory
+__device__ __forceinline__ void wgmma_f16_ss(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " SDETR_WGMMA_D64
+                 "%64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : SDETR_WGMMA_D64_OPS(d)
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// d (64 x 64 fp32 per warpgroup) = (accumulate ? d : 0) + a (64 x 16 fp16) . b (16 x 64 fp16), both K-major in shared memory
+__device__ __forceinline__ void wgmma_f16_ss_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " SDETR_WGMMA_D32
+                 "%32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : SDETR_WGMMA_D32_OPS(d)
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
 // (x0, x1) -> packed hi (f16x2: x0 in the low half = the lower k index) and packed lo of the residuals
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_t &lo) {
     const __half2 h = __floats2half2_rn(x0, x1);

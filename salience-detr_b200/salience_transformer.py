@@ -53,11 +53,10 @@ FUSED_SMALL_PREDICTOR = __import__("os").environ.get("SDETR_FUSED_SMALL_PREDICTO
 # level with at most PREDICTOR_SMALL_ROWS token rows as two fp32 kernels (csrc/predictor_small.cu) instead of ~15 latency-bound launches
 PREDICTOR_SMALL_ROWS = 4096
 FUSED_FFN = __import__("os").environ.get("SDETR_FUSED_FFN", "1") != "0"  # C = 256: linear1 -> ReLU -> linear2 -> +residual -> norm2
-# through sdetr_ffn_fused_layernorm (csrc/ffn_fused.cu: two 3xFP16 GEMMs, the ReLU fused into the second's operand load, + a row kernel)
+# through sdetr_ffn_fused_layernorm (csrc/ffn_fused.cu: one persistent 3xFP16 kernel that keeps the hidden activations on chip)
 # instead of two gemm.linear calls and an add+LayerNorm launch
-FFN_CHUNK_ROWS = int(__import__("os").environ.get("SDETR_FFN_CHUNK", "0"))  # FFN in row chunks: the hidden activations of a chunk are
-# produced and consumed while they can still sit in L2 and their buffer is reused by the next chunk.  0 (default) = one GEMM pair
-# over all rows.
+FFN_CHUNK_ROWS = int(__import__("os").environ.get("SDETR_FFN_CHUNK", "0"))  # FFN in row chunks of this many rows, one FFN call
+# each.  0 (default) = one call over all rows.
 TILE_CELL_PX = 64   # edge (image pixels) of the spatial cells that define the MSDA processing order
 MSDA_SCHEDULE = 1   # 0 = query-major, 1 = head-major chunks (see include/sdetr_b200.h)
 

@@ -128,6 +128,36 @@ int sdetr_msda_backward(const float *value, const int64_t *spatial_shapes, const
                         int num_value, int num_heads, int head_dim, int num_levels, int num_query,
                         int num_points, sdetr_stream_t stream);
 
+/* Deterministic MSDA core backward: the contract of sdetr_msda_backward (same arguments, checks and head dims
+ * {4,8,16,32,64,128}), and grad_value is BIT-IDENTICAL for identical inputs whatever the launch order, the grid or the order
+ * of the queries.  grad_sampling_loc and grad_attn_weight are computed by the same code as sdetr_msda_backward's and are
+ * bit-identical to its results.
+ * grad_value accumulates in fixed point: each corner contribution (w_corner * attn) * grad_out is multiplied by one exact
+ * power of two 2^s, rounded to int64 and added with integer atomics (associative: the order of additions cannot matter).
+ * s is computed on the device (no host read; the call can be captured in a CUDA graph) so that
+ * max|grad_out| * max|attn| * num_query * num_points * 2^s <= 2^62 with both maxima rounded up to powers of two; no sum can
+ * overflow.  The absolute error of a grad_value entry is at most (its number of contributions / 2 + 1) * 2^-s.
+ * Non-finite values: a non-finite sampling location contributes exactly 0 (as in sdetr_msda_backward); a NaN or infinity
+ * anywhere in grad_output or attn_weight makes EVERY grad_value entry NaN.
+ * workspace: sdetr_msda_backward_deterministic_workspace() bytes, 16-byte aligned = the int64 accumulator
+ * (8 * b*Nv*M*D bytes) and 32 bytes of scale / flag / reduction state; zeroed on `stream` by the call.  Too small:
+ * SDETR_ERR_WORKSPACE.  Cost: four 8-byte integer reductions per lane and corner where the fp32 path issues one 16-byte one. */
+size_t sdetr_msda_backward_deterministic_workspace(int batch, int num_value, int num_heads, int head_dim);
+int sdetr_msda_backward_deterministic(const float *value, const int64_t *spatial_shapes, const int64_t *level_start_index,
+                                      const float *sampling_loc, const float *attn_weight, const float *grad_output,
+                                      float *grad_value, float *grad_sampling_loc, float *grad_attn_weight, int batch,
+                                      int num_value, int num_heads, int head_dim, int num_levels, int num_query,
+                                      int num_points, void *workspace, size_t workspace_bytes, sdetr_stream_t stream);
+
+/* Backward of the coarse-to-fine score upsample F.interpolate(mode="bilinear", align_corners=True) from (planes, Hc, Wc) to
+ * (planes, H, W) (salience_transformer.py:134-143), deterministic: in gather form, each coarse cell sums the weighted
+ * gradients of the fine pixels whose stencil contains it, in row-major order, and is written once (no atomics; torch's
+ * CUDA backward of the op scatters with atomics).  The stencil uses the fp32 quantities of torch's forward:
+ * scale = (in-1)/(out-1), src = scale*dst, i0 = (int)src, i1 = i0 + (i0 < in-1), lambda = src - i0.
+ * grad_fine (planes,H,W) -> grad_coarse (planes,Hc,Wc), fully written. */
+int sdetr_upsample_bilinear_ac_backward(const float *grad_fine, int planes, int H, int W, int Hc, int Wc, float *grad_coarse,
+                                        sdetr_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Hierarchical salience token filter (models/bricks/salience_transformer.py:146-168), one call:
  *   per level l: v = where(mask, min over the whole (b,HW_l) score tensor, score)       (:146)

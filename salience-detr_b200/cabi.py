@@ -36,6 +36,9 @@ SIGNATURES = {
     "sdetr_msda_set_host_shapes": (_i, [_i, _vp, _vp]),
     "sdetr_nms_topk_index": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp]),
     "sdetr_msda_backward": (_i, [_vp] * 9 + [_i] * 7 + [_vp]),
+    "sdetr_msda_backward_deterministic_workspace": (_sz, [_i] * 4),
+    "sdetr_msda_backward_deterministic": (_i, [_vp] * 9 + [_i] * 7 + [_vp, _sz, _vp]),
+    "sdetr_upsample_bilinear_ac_backward": (_i, [_vp] + [_i] * 5 + [_vp, _vp]),
     "sdetr_salience_select_workspace": (_sz, [_i, _i, _i]),
     "sdetr_salience_select": (_i, [_vp] * 7 + [_i] * 4 + [_vp] * 5 + [_sz, _vp]),
     "sdetr_order_prefixes": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
@@ -255,6 +258,38 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
         gv.data_ptr(), gl.data_ptr(), ga.data_ptr(), b, nv, m, d, L, nq, P, _stream())
     _check(rc, "sdetr_msda_backward")
     return gv, gl, ga
+
+
+def msda_backward_deterministic(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output):
+    """Same contract as :func:`msda_backward`; grad_value is bit-reproducible (fixed-point accumulation, whatever the order of
+    the queries), grad_sampling_loc / grad_attn_weight are bit-identical to msda_backward's.  The int64 accumulator comes from
+    the caching allocator (8 bytes per value element)."""
+    b, nv, m, d = value.shape
+    nq, L, P = sampling_loc.shape[1], sampling_loc.shape[3], sampling_loc.shape[4]
+    gv = torch.empty_like(value)
+    gl = torch.empty_like(sampling_loc)
+    ga = torch.empty_like(attn_weight)
+    need = lib().sdetr_msda_backward_deterministic_workspace(b, nv, m, d)
+    ws = torch.empty(max(need, 16), device=value.device, dtype=torch.uint8)
+    rc = lib().sdetr_msda_backward_deterministic(
+        _req(value, "value", torch.float32), _req(spatial_shapes, "spatial_shapes", torch.int64),
+        _req(level_start_index, "level_start_index", torch.int64), _req(sampling_loc, "sampling_loc", torch.float32),
+        _req(attn_weight, "attn_weight", torch.float32), _req(grad_output, "grad_output", torch.float32),
+        gv.data_ptr(), gl.data_ptr(), ga.data_ptr(), b, nv, m, d, L, nq, P, ws.data_ptr(), ws.numel(), _stream())
+    _check(rc, "sdetr_msda_backward_deterministic")
+    return gv, gl, ga
+
+
+def upsample_bilinear_ac_backward(grad_fine, Hc: int, Wc: int):
+    """Backward of ``F.interpolate(x, size=(H, W), mode="bilinear", align_corners=True)`` for x (..., Hc, Wc):
+    grad_fine (..., H, W) -> grad (..., Hc, Wc), deterministic (gather form, no atomics)."""
+    H, W = grad_fine.shape[-2:]
+    planes = grad_fine.numel() // max(H * W, 1)
+    out = torch.empty(*grad_fine.shape[:-2], Hc, Wc, device=grad_fine.device, dtype=torch.float32)
+    rc = lib().sdetr_upsample_bilinear_ac_backward(_req(grad_fine, "grad_fine", torch.float32), planes, H, W, Hc, Wc,
+                                                   out.data_ptr(), _stream())
+    _check(rc, "sdetr_upsample_bilinear_ac_backward")
+    return out
 
 
 # ---- salience filter --------------------------------------------------------------------------------------

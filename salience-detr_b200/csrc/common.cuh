@@ -1,6 +1,7 @@
 // Shared helpers of the sm_90a kernels behind include/sdetr_b200.h.
 #pragma once
 #include <cuda_runtime.h>
+#include <float.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -74,6 +75,42 @@ __device__ __forceinline__ void st_stream_f4(float *p, const float4 &v) {
     asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
                  "f"(v.w)
                  : "memory");
+}
+
+// ---- max|x| in one launch (sdetr_pow2_scale, the deterministic MSDA backward's scale) ----------------------------------
+// This thread's grid-stride share of max|x[0, n)|.  fmaxf skips NaN: `nonfinite` is set when a NaN or an infinity is seen.
+// 16-byte aligned x is read with 128-bit streaming loads, any other x element by element.
+__device__ __forceinline__ float thread_absmax(const float *__restrict__ x, int64_t n, bool &nonfinite) {
+    float m = 0.f;
+    bool bad = false;
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = (int64_t)gridDim.x * blockDim.x;
+    if ((reinterpret_cast<uintptr_t>(x) & 15u) == 0) {
+        for (int64_t i = t * 4; i < n; i += nt * 4) {
+            if (i + 3 < n) {
+                const float4 v = ld_stream_f4(x + i);
+                m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+                bad |= !(fabsf(v.x) <= FLT_MAX) | !(fabsf(v.y) <= FLT_MAX) | !(fabsf(v.z) <= FLT_MAX) | !(fabsf(v.w) <= FLT_MAX);
+            } else {
+                for (int64_t j = i; j < n; ++j) m = fmaxf(m, fabsf(x[j])), bad |= !(fabsf(x[j]) <= FLT_MAX);
+            }
+        }
+    } else {
+        for (int64_t i = t; i < n; i += nt) m = fmaxf(m, fabsf(x[i])), bad |= !(fabsf(x[i]) <= FLT_MAX);
+    }
+    nonfinite |= bad;
+    return m;
+}
+// Maximum of m over the block, in thread 0 (blockDim.x a multiple of 32).  Safe to call repeatedly in one kernel.
+__device__ __forceinline__ float block_max(float m) {
+    __shared__ float wm[32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    __syncthreads();  // wm may still be read by an earlier call
+    if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, wm[w]);
+    return m;
 }
 
 // fp32 -> uint32 whose ascending order is the DESCENDING order of the floats (-0 == +0, NaN first).

@@ -106,24 +106,10 @@ namespace sdetr {
 __global__ void __launch_bounds__(256) pow2_scale_kernel(const float *__restrict__ x, int64_t n, int target_log2,
                                                          unsigned int *__restrict__ state /* [0] max bits, [1] blocks done */,
                                                          float *__restrict__ scale) {
-    float m = 0.f;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
-    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
-        if (i + 3 < n) {
-            const float4 v = ld_stream_f4(x + i);
-            m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
-        } else {
-            for (int64_t j = i; j < n; ++j) m = fmaxf(m, fabsf(x[j]));
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    __shared__ float wm[8];
+    bool nonfinite = false;  // not needed here: NaN / inf propagate through the GEMM whatever the scale
+    float m = block_max(thread_absmax(x, n, nonfinite));
     __shared__ bool last;
-    if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
-    __syncthreads();
     if (threadIdx.x == 0) {
-        for (int w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
         if (!(m <= 3.0e38f)) m = 3.0e38f;                 // NaN / inf: the GEMM propagates them whatever the scale
         atomicMax(state, __float_as_uint(m));             // non-negative floats order like their bit patterns
         __threadfence();

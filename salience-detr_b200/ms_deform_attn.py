@@ -41,11 +41,16 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
 
 def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
                             im2col_step=64):
-    """Operator-level replacement of ``_C.ms_deform_attn_backward`` (ms_deform_attn_cuda.cu:75-145)."""
+    """Operator-level replacement of ``_C.ms_deform_attn_backward`` (ms_deform_attn_cuda.cu:75-145).
+
+    Under ``torch.use_deterministic_algorithms(True)`` (either ``warn_only``) grad_value comes from the fixed-point kernel
+    (``sdetr_msda_backward_deterministic``): bit-reproducible, with the same grad_sampling_loc / grad_attn_weight bits.
+    Otherwise it is accumulated with fp32 atomics, like the reference's."""
     step = min(value.shape[0], im2col_step)
     if value.shape[0] % step != 0:
         raise RuntimeError(f"batch({value.shape[0]}) must divide im2col_step({step})")
-    return list(cabi.msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output))
+    fn = cabi.msda_backward_deterministic if torch.are_deterministic_algorithms_enabled() else cabi.msda_backward
+    return list(fn(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output))
 
 
 # what `from models.bricks.ms_deform_attn import _C` gives the reference code

@@ -151,6 +151,22 @@ class EncoderPlan:
     scratch: Dict[str, Tensor] = field(default_factory=dict)
 
 
+class UpsampleBilinearAC(torch.autograd.Function):
+    """``F.interpolate(x, size, mode="bilinear", align_corners=True)`` with a deterministic backward
+    (``sdetr_upsample_bilinear_ac_backward``, gather form).  torch's CUDA backward of the op accumulates with atomics and
+    raises under ``torch.use_deterministic_algorithms(True)``; the forward is the same torch call, so its bits do not change."""
+
+    @staticmethod
+    def forward(ctx, x, size):
+        ctx.in_hw = tuple(x.shape[-2:])
+        return F.interpolate(x, size=size, mode="bilinear", align_corners=True)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        return cabi.upsample_bilinear_ac_backward(grad.contiguous(), *ctx.in_hw), None
+
+
 def flatten_levels(xs: Sequence[Tensor]) -> Tensor:
     """(b,[C],H_l,W_l) per level -> (b,Nv,[C]) tokens (base_transformer.py:21-26)."""
     y = torch.cat([e.flatten(-2) for e in xs], -1)
@@ -639,8 +655,11 @@ class SalienceTransformer(nn.Module):
                 hc, wc = plan.shapes_list[lvl + 1]
                 s1 = plan.level_start[lvl + 1]
                 if grad:
-                    up = F.interpolate(prev.transpose(1, 2).reshape(b, 1, hc, wc), size=(h, w), mode="bilinear",
-                                       align_corners=True)
+                    coarse = prev.transpose(1, 2).reshape(b, 1, hc, wc)
+                    if torch.are_deterministic_algorithms_enabled():  # torch's backward of the resize is not deterministic
+                        up = UpsampleBilinearAC.apply(coarse, (h, w))
+                    else:
+                        up = F.interpolate(coarse, size=(h, w), mode="bilinear", align_corners=True)
                     m_l = m_l + m_l * up.view(b, 1, h * w).transpose(1, 2) * self.alpha[lvl]
                 else:
                     m_l = cabi.score_modulate(mem, s0, h, w, raw[:, s1:s1 + hc * wc], hc, wc, self.alpha, lvl)

@@ -1,5 +1,6 @@
 """MSDA core forward / backward (the `_C` operator boundary) at the config-2 layer shapes: time per launch and the
-fraction of the HBM roofline on algorithmic bytes.  Results summarised under profiles/."""
+fraction of the HBM roofline on algorithmic bytes, and the deterministic (fixed-point) backward next to the atomic one
+("det us", "det/bwd").  Results summarised under profiles/."""
 import json
 import os
 import statistics
@@ -23,7 +24,8 @@ b, m, d, L, P = 2, 8, 32, 4, 4
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 g = torch.Generator(device="cpu").manual_seed(0)
 print("MSDA core at config 2 (b=2, Nv=%d, M=8, D=32, L=4, P=4); HBM peak %.0f GB/s" % (nv, peak))
-print("%8s | %10s %10s %8s | %10s %10s %8s" % ("Nq", "fwd us", "fwd GB/s", "frac", "bwd us", "bwd GB/s", "frac"))
+print("%8s | %10s %10s %8s | %10s %10s %8s | %10s %8s" % ("Nq", "fwd us", "fwd GB/s", "frac", "bwd us", "bwd GB/s", "frac",
+                                                         "det us", "det/bwd"))
 for nq in (11363, 9090, 6817, 4545, 2272):
     value = torch.randn(b, nv, m, d, generator=g).to(dev)
     # sampling locations as the encoder produces them: reference point + small learned offsets
@@ -31,7 +33,7 @@ for nq in (11363, 9090, 6817, 4545, 2272):
     loc = (ref + torch.randn(b, nq, m, L, P, 2, generator=g) * 0.03).to(dev)
     attn = torch.randn(b, nq, m, L * P, generator=g).softmax(-1).view(b, nq, m, L, P).to(dev)
     gout = torch.randn(b, nq, m * d, generator=g).to(dev)
-    tf, tb = [], []
+    tf, tb, td = [], [], []
     for _ in range(12):
         flush.zero_()
         e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
@@ -43,10 +45,18 @@ for nq in (11363, 9090, 6817, 4545, 2272):
         torch.cuda.synchronize()
         tf.append(e[0].elapsed_time(e[1]) * 1e3)
         tb.append(e[1].elapsed_time(e[2]) * 1e3)
-    tf, tb = statistics.median(tf[2:]), statistics.median(tb[2:])
+        flush.zero_()
+        e = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        e[0].record()
+        pkg.cabi.msda_backward_deterministic(value, st, lsi, loc, attn, gout)  # workspace allocation included (cached)
+        e[1].record()
+        torch.cuda.synchronize()
+        td.append(e[0].elapsed_time(e[1]) * 1e3)
+    tf, tb, td = statistics.median(tf[2:]), statistics.median(tb[2:]), statistics.median(td[2:])
     c = m * d
     fwd_bytes = b * (4 * nv * c + nq * (12 * m * L * P + 4 * c))                      # SURVEY 8(d) C_msda
     bwd_bytes = b * (4 * nv * c + nq * (12 * m * L * P + 4 * c)                       # value, loc, attn, grad_out in
                      + 4 * nv * c + nq * 12 * m * L * P)                              # grad_value, grad_loc, grad_attn out
-    print("%8d | %10.1f %10.1f %8.3f | %10.1f %10.1f %8.3f" % (nq, tf, fwd_bytes / tf / 1e3, fwd_bytes / tf / 1e3 / peak,
-                                                               tb, bwd_bytes / tb / 1e3, bwd_bytes / tb / 1e3 / peak))
+    print("%8d | %10.1f %10.1f %8.3f | %10.1f %10.1f %8.3f | %10.1f %8.2f" % (
+        nq, tf, fwd_bytes / tf / 1e3, fwd_bytes / tf / 1e3 / peak, tb, bwd_bytes / tb / 1e3, bwd_bytes / tb / 1e3 / peak,
+        td, td / tb))

@@ -435,6 +435,35 @@ int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *W1_hi, co
                               const void *W2_hi, const void *W2_lo, float w2_scale, const float *b2, const float *gamma,
                               const float *beta, float eps, int M, int hidden, float *workspace, int64_t workspace_floats, float *y,
                               sdetr_stream_t stream);
+
+/* ---- RepVGG-PluX neck in token layout (models/necks/repnet.py:125-245; RepVGGPluXNetwork.forward_tokens) ------------------
+ * Operands are token rows: pixel (py, px) of image n, channel c at base + n * pitch + (py * W + px) * ld + c (floats), so a
+ * level slice of a (b, Nv, C) tensor is an operand as it is.
+ *
+ * Convolution y = act(conv(x, W) + bias), kernel ksize x ksize (1 or 3), padding ksize / 2, stride 1 or 2, `groups` groups;
+ * act 0 none, 3 SiLU.  Implicit GEMM on wgmma with the 3xFP16 arithmetic of sdetr_gemm_f16x3_scaled: x is multiplied by the
+ * power-of-two device scalar *a_scale_dev (sdetr_pow2_scale with target 12) before its hi / lo split, W (Cout, ksize, ksize,
+ * Cin / groups) row-major was split with *w_scale_dev (sdetr_split_f16_pair_dev), the epilogue divides both out.
+ * Cin / groups and Cout / groups multiples of 64 (else SDETR_ERR_UNSUPPORTED); x, x_pitch, ldx 16-byte aligned; y, y_pitch,
+ * ldy 8-byte aligned; Ho = (H + 2 (ksize / 2) - ksize) / stride + 1, likewise Wo.  bias may be NULL. */
+int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin, const float *a_scale_dev,
+                       const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, int Cout, int groups,
+                       int ksize, int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
+/* Context gate of a RepVggPluXBlock (SqueezeAndExcitation, models/bricks/basic.py:29-54, plus the block's residual), per image
+ * of HW pixels: p = softmax over the pixels of (y . w_mask + *b_mask); ctx = sum p y; gate = sigmoid(W2 ReLU(W1 ctx)) with
+ * w1 (R, C), w2 (C, R) row-major; out = gate * y + x (+ z when z is not NULL).  Three launches; every reduction is summed in a
+ * fixed order (bit-reproducible).  C % 4 == 0; all row operands 16-byte aligned; out may alias x or z.
+ * workspace: sdetr_context_gate_workspace_floats(batch, HW, C) floats, 16-byte aligned. */
+int64_t sdetr_context_gate_workspace_floats(int batch, int HW, int C);
+int sdetr_context_gate(const float *y, int64_t y_pitch, int64_t ldy, const float *x, int64_t x_pitch, int64_t ldx, const float *z,
+                       int64_t z_pitch, int64_t ldz, int batch, int HW, int C, const float *w_mask, const float *b_mask,
+                       const float *w1, const float *w2, int R, float *workspace, int64_t workspace_floats, float *out,
+                       int64_t out_pitch, int64_t ldo, sdetr_stream_t stream);
+/* dst[:, :, 0:C] = nearest-upsampled hi (Hi, Wi) -> (Ho, Wo) with torch's index rule src = min(floor(dst * (float)in / out),
+ * in - 1); dst[:, :, C:2C] = lo (Ho, Wo).  C % 4 == 0; all row operands 16-byte aligned. */
+int sdetr_upsample_nearest_concat(const float *hi, int64_t hi_pitch, int64_t ldh, int Hi, int Wi, const float *lo, int64_t lo_pitch,
+                                  int64_t ldl, int Ho, int Wo, int batch, int C, float *dst, int64_t dst_pitch, int64_t ldd,
+                                  sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -27,6 +27,13 @@ from .decoder import (  # noqa: F401
     get_sine_pos_embed,
     inverse_sigmoid,
 )
+from .neck import (  # noqa: F401
+    Conv2dNormActivation,
+    CSPRepPluXLayer,
+    RepVGGPluXNetwork,
+    RepVggPluXBlock,
+    SqueezeAndExcitation,
+)
 from .salience_transformer import (  # noqa: F401
     EncoderPlan,
     MaskPredictor,

@@ -82,6 +82,11 @@ SIGNATURES = {
     "sdetr_rows_gather": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "sdetr_rows_gather_add": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sdetr_rows_scatter": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "sdetr_conv2d_f16x3": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
+    "sdetr_context_gate_workspace_floats": (_i64, [_i, _i, _i]),
+    "sdetr_context_gate": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp,
+                                _i64, _i64, _vp]),
+    "sdetr_upsample_nearest_concat": (_i, [_vp, _i64, _i64, _i, _i, _vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
 }
 
 
@@ -873,3 +878,72 @@ def gelu_colmean_(z, half: int):
     rc = lib().sdetr_gelu_colmean(_req(z, "z", torch.float32), b, n, c, half, ws.data_ptr(), ws.numel(), _stream())
     _check(rc, "sdetr_gelu_colmean")
     return z
+
+
+# ---- RepVGG-PluX neck in token layout (neck.RepVGGPluXNetwork.forward_tokens) --------------------------------------------
+def _token_rows(t, name):
+    """(b, HW, C) fp32 CUDA view with unit channel stride -> (pointer, image pitch, row stride) in floats"""
+    if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 3 and t.stride(2) == 1):
+        raise RuntimeError(f"{name} must be a CUDA float32 (b, HW, C) tensor with unit channel stride")
+    if t.device.index != _current_device():
+        raise RuntimeError(f"{name} lives on {t.device} but cuda:{_current_device()} is current")
+    return t.data_ptr(), t.stride(0), t.stride(1)
+
+
+ACT_SILU = 3
+
+
+def conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, w_scale, bias, groups: int, ksize: int, stride: int, act: int = 0, out=None):
+    """y = act(conv2d(x, W) + bias) on token rows.  x: (b, H*W, Cin) view (e.g. a level slice of the encoder memory), hw = (H, W);
+    W given as the (Cout, k, k, Cin / groups) pair of split_f16_pair_dev and its device scale; a_scale: pow2_scale of x (target 12).
+    out: optional (b, Ho*Wo, Cout) view to write; returns it (or a new contiguous tensor)."""
+    H, W = hw
+    b, hw_in, cin = x.shape
+    if hw_in != H * W:
+        raise RuntimeError(f"conv2d_f16x3: x has {hw_in} rows per image, the map is {H}x{W}")
+    cout = w_hi.shape[0]
+    pad = ksize // 2
+    ho, wo = (H + 2 * pad - ksize) // stride + 1, (W + 2 * pad - ksize) // stride + 1
+    y = out if out is not None else torch.empty(b, ho * wo, cout, device=x.device, dtype=torch.float32)
+    if tuple(y.shape) != (b, ho * wo, cout):
+        raise RuntimeError(f"conv2d_f16x3: out must be ({b}, {ho * wo}, {cout})")
+    xp, xpitch, ldx = _token_rows(x, "x")
+    yp, ypitch, ldy = _token_rows(y, "out")
+    rc = lib().sdetr_conv2d_f16x3(xp, xpitch, ldx, b, H, W, cin, _req(a_scale, "a_scale", torch.float32),
+                                  _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
+                                  _req(w_scale, "w_scale", torch.float32),
+                                  _req(bias, "bias", torch.float32) if bias is not None else None, cout, int(groups), int(ksize),
+                                  int(stride), int(act), yp, ypitch, ldy, _stream())
+    _check(rc, "sdetr_conv2d_f16x3")
+    return y
+
+
+def context_gate(y, x, w_mask, b_mask, w1, w2, z=None, out=None):
+    """out = sigmoid(W2 ReLU(W1 ctx)) * y + x (+ z), ctx = softmax over each image's pixels of (y . w_mask + b_mask) . y.
+    y, x, z, out: (b, HW, C) views; w_mask (C), b_mask (1) device tensors, w1 (C / r, C), w2 (C, C / r)."""
+    b, hw, c = y.shape
+    r = w1.shape[0]
+    out = out if out is not None else torch.empty(b, hw, c, device=y.device, dtype=torch.float32)
+    ops = [_token_rows(t, n) for t, n in ((y, "y"), (x, "x"), (out, "out"))]
+    zp = _token_rows(z, "z") if z is not None else (None, 0, 0)
+    if any(tuple(t.shape) != (b, hw, c) for t in (x, out) + ((z,) if z is not None else ())):
+        raise RuntimeError("context_gate: y, x, z and out must have the same shape")
+    ws = torch.empty(max(int(lib().sdetr_context_gate_workspace_floats(b, hw, c)), 4), device=y.device, dtype=torch.float32)
+    rc = lib().sdetr_context_gate(*ops[0], *ops[1], *zp, b, hw, c, _req(w_mask, "w_mask", torch.float32),
+                                  _req(b_mask, "b_mask", torch.float32), _req(w1, "w1", torch.float32), _req(w2, "w2", torch.float32),
+                                  r, ws.data_ptr(), ws.numel(), *ops[2], _stream())
+    _check(rc, "sdetr_context_gate")
+    return out
+
+
+def upsample_nearest_concat(hi, hi_hw, lo, lo_hw, out=None):
+    """(b, Ho*Wo, 2C) = [nearest(hi) | lo]: hi (b, Hi*Wi, C), lo (b, Ho*Wo, C) views; torch's nearest index rule."""
+    b, _, c = hi.shape
+    ho, wo = lo_hw
+    out = out if out is not None else torch.empty(b, ho * wo, 2 * c, device=hi.device, dtype=torch.float32)
+    if tuple(lo.shape) != (b, ho * wo, c) or tuple(out.shape) != (b, ho * wo, 2 * c) or hi.shape[1] != hi_hw[0] * hi_hw[1]:
+        raise RuntimeError("upsample_nearest_concat: shapes do not match")
+    rc = lib().sdetr_upsample_nearest_concat(*_token_rows(hi, "hi"), int(hi_hw[0]), int(hi_hw[1]), *_token_rows(lo, "lo"), int(ho),
+                                             int(wo), b, c, *_token_rows(out, "out"), _stream())
+    _check(rc, "sdetr_upsample_nearest_concat")
+    return out

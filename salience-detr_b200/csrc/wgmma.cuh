@@ -127,6 +127,16 @@ __device__ __forceinline__ void wgmma_f16_ss_n64(float (&d)[32], uint64_t desc_a
                  : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
+// d (64 x 64 fp32 per warpgroup) = (accumulate ? d : 0) + a (64 x 16 fp16, registers) . b (16 x 64 fp16, K-major in shared
+// memory)
+__device__ __forceinline__ void wgmma_f16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " SDETR_WGMMA_D32
+                 "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+                 : SDETR_WGMMA_D32_OPS(d)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
+
 // (x0, x1) -> packed hi (f16x2: x0 in the low half = the lower k index) and packed lo of the residuals
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_t &lo) {
     const __half2 h = __floats2half2_rn(x0, x1);

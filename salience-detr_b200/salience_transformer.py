@@ -778,8 +778,11 @@ class SalienceTransformer(nn.Module):
         salience = [aux["raw_score"][:, s:s + h * w].reshape(b, 1, h, w) for s, (h, w) in zip(plan.level_start, plan.shapes_list)]
         if self.decoder is None and self.neck is None:
             return memory, salience
-        if self.neck is not None:  # :185-192 (the RepVGG neck itself is outside the path: any nn.Module taking {i: NCHW})
-            if memory.is_cuda and not (torch.is_grad_enabled() and memory.requires_grad):
+        if self.neck is not None:  # :185-192 (any nn.Module taking {i: NCHW}; neck.RepVGGPluXNetwork also runs in token layout)
+            tokens_ok = getattr(self.neck, "tokens_supported", None)
+            if tokens_ok is not None and hasattr(self.neck, "forward_tokens") and tokens_ok(memory, plan.shapes_list):
+                memory = self.neck.forward_tokens(memory, plan.shapes_list)
+            elif memory.is_cuda and not (torch.is_grad_enabled() and memory.requires_grad):
                 feats = dict(enumerate(cabi.tokens_to_maps(memory.contiguous(), plan.shapes_list)))   # one launch each way
                 feats = list(self.neck(feats).values())
                 memory = cabi.maps_to_tokens([f.float().contiguous() for f in feats])

@@ -308,12 +308,9 @@ int sdetr_sine_pos_tokens(const float *ynorm, const float *xnorm, const float *d
                           int num_pos_feats, float *pos_tokens, sdetr_stream_t stream);
 
 /* Dense self-attention core of the 300-token pre-attention (salience_transformer.py:372-376; the attention inside
- * nn.MultiheadAttention): out = softmax(Q K^T / sqrt(d)) V per (image, head).  qk (b,n,2,heads,d): projected queries
- * then keys; v (b,n,heads,d); out (b,n,heads*d).  head_dim must be 32; K^T, V and the score tile live in shared memory:
- * n up to ~460, larger n returns SDETR_ERR_UNSUPPORTED. */
-int sdetr_attention_small(const float *qk, const float *v, float *out, int batch, int n, int heads, int head_dim,
-                          sdetr_stream_t stream);
-/* Same core on a packed projection buffer qkv (b,n,3,heads,d) (what sdetr_mha_in_proj writes). */
+ * nn.MultiheadAttention): out = softmax(Q K^T / sqrt(d)) V per (image, head).  qkv (b,n,3,heads,d): the packed
+ * projected queries, keys and values (what sdetr_mha_in_proj writes); out (b,n,heads*d).  head_dim must be 32; K^T, V
+ * and the score tile live in shared memory: n up to ~460, larger n returns SDETR_ERR_UNSUPPORTED. */
 int sdetr_attention_qkv(const float *qkv, float *out, int batch, int n, int heads, int head_dim, sdetr_stream_t stream);
 
 /* Pre-attention front (salience_transformer.py:368-372 + the packed in-projection of nn.MultiheadAttention):
@@ -335,14 +332,12 @@ int sdetr_mha_out_proj_ln_scatter(const float *attn, const float *t, const float
                                   const float *pos, float *dst_sum, int batch, int num_rows, int k, int channels,
                                   sdetr_stream_t stream);
 
-/* Row gather / scatter by per-image index (the top-k tokens of the pre-attention, salience_transformer.py:368-379):
- * out[b,j,:] = src[b,index[b,j],:]   /   dst[b,index[b,j],:] = src[b,j,:]  (indices unique per image).
- * src/dst (b,num_rows,C), index (b,k) int64. */
-int sdetr_rows_gather(const float *src, const int64_t *index, int batch, int num_rows, int k, int channels, float *out,
-                      sdetr_stream_t stream);
-/* t[b,j,:] = src[b,index[b,j],:],  x[b,j,:] = t[b,j,:] + pos[b,index[b,j],:]  (:368-371 in one pass) */
+/* Row gather / scatter by per-image index (the top-k tokens of the pre-attention, salience_transformer.py:368-379),
+ * indices unique per image; src/dst (b,num_rows,C), index (b,k) int64.
+ * t[b,j,:] = src[b,index[b,j],:],  x[b,j,:] = t[b,j,:] + pos[b,index[b,j],:]  (:368-371 in one pass) */
 int sdetr_rows_gather_add(const float *src, const float *pos, const int64_t *index, int batch, int num_rows, int k,
                           int channels, float *t, float *x, sdetr_stream_t stream);
+/* dst[b,index[b,j],:] = src[b,j,:] */
 int sdetr_rows_scatter(float *dst, const int64_t *index, int batch, int num_rows, int k, int channels, const float *src,
                        sdetr_stream_t stream);
 

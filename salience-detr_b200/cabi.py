@@ -75,11 +75,9 @@ SIGNATURES = {
     "sdetr_ffn_fused_layernorm": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _i, _i, _vp, _i64, _vp, _vp]),
     "sdetr_flatten_set_vectorized": (_i, [_i]),
     "sdetr_flatten_tokens": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "sdetr_attention_small": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "sdetr_attention_qkv": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "sdetr_mha_in_proj": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "sdetr_mha_out_proj_ln_scatter": (_i, [_vp] * 6 + [_f, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "sdetr_rows_gather": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "sdetr_rows_gather_add": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sdetr_rows_scatter": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "sdetr_conv2d_f16x3": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
@@ -506,17 +504,6 @@ def split_tf32(x, layout_b: bool = False, relu=0, chunk: int = 0):
     return out
 
 
-def rows_gather(src, index):
-    """src (b,n,C), index (b,k) int64 -> (b,k,C)."""
-    b, n, c = src.shape
-    k = index.shape[1]
-    out = torch.empty(b, k, c, device=src.device, dtype=torch.float32)
-    rc = lib().sdetr_rows_gather(_req(src, "src", torch.float32), _req(index, "index", torch.int64), b, n, k, c,
-                                 out.data_ptr(), _stream())
-    _check(rc, "sdetr_rows_gather")
-    return out
-
-
 def rows_scatter_(dst, index, src):
     """dst (b,n,C) <- src (b,k,C) at index (b,k) int64, in place."""
     b, n, c = dst.shape
@@ -816,16 +803,6 @@ def rows_gather_add(src, pos, index):
                                      _req(index, "index", torch.int64), b, n, k, c, t.data_ptr(), x.data_ptr(), _stream())
     _check(rc, "sdetr_rows_gather_add")
     return t, x
-
-
-def attention_small(qk, v):
-    """qk (b,n,2,h,d) [queries | keys], v (b,n,h,d) -> (b,n,h*d) = softmax(QK^T/sqrt(d)) V per head."""
-    b, n, _, h, d = qk.shape
-    out = torch.empty(b, n, h * d, device=qk.device, dtype=torch.float32)
-    rc = lib().sdetr_attention_small(_req(qk, "qk", torch.float32), _req(v, "v", torch.float32), out.data_ptr(), b, n, h, d,
-                                     _stream())
-    _check(rc, "sdetr_attention_small")
-    return out
 
 
 def attention_qkv(qkv, heads: int):

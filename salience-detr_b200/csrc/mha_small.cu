@@ -424,13 +424,6 @@ static int launch_attention(const float *q, const float *kmat, const float *v, i
     return check_launch(what);
 }
 
-extern "C" int sdetr_attention_small(const float *qk, const float *v, float *out, int batch, int n, int heads, int head_dim,
-                                     sdetr_stream_t stream) {
-    const int64_t c = (int64_t)heads * head_dim;
-    return launch_attention(qk, qk ? qk + c : nullptr, v, 2 * c, c, out, batch, n, heads, head_dim, (cudaStream_t)stream,
-                            "attention_small");
-}
-
 extern "C" int sdetr_attention_qkv(const float *qkv, float *out, int batch, int n, int heads, int head_dim,
                                    sdetr_stream_t stream) {
     const int64_t c = (int64_t)heads * head_dim;

@@ -553,17 +553,8 @@ extern "C" int sdetr_gelu_colmean(float *z, int batch, int num_rows, int channel
     return check_launch("gelu_colmean/broadcast");
 }
 
-// ---- generic row gather / scatter by index (the 300-token pre-attention, salience_transformer.py:368-379) ----
+// ---- generic row scatter by index (the 300-token pre-attention, salience_transformer.py:368-379) ----
 namespace sdetr {
-__global__ void __launch_bounds__(kRowThreads) rows_gather_kernel(const float *__restrict__ src, const int64_t *__restrict__ idx,
-                                                                  int batch, int n, int k, int C, float *__restrict__ out) {
-    const int lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
-    if (row >= (int64_t)batch * k) return;
-    const int b = (int)(row / k);
-    const float *s = src + ((int64_t)b * n + __ldg(idx + row)) * C;
-    for (int c = lane * 4; c < C; c += 128) st_stream_f4(out + row * C + c, ld_stream_f4(s + c));
-}
 __global__ void __launch_bounds__(kRowThreads) rows_scatter_kernel(float *__restrict__ dst, const int64_t *__restrict__ idx,
                                                                    int batch, int n, int k, int C, const float *__restrict__ src) {
     const int lane = threadIdx.x & 31;
@@ -574,17 +565,6 @@ __global__ void __launch_bounds__(kRowThreads) rows_scatter_kernel(float *__rest
     for (int c = lane * 4; c < C; c += 128) st_stream_f4(d + c, ld_stream_f4(src + row * C + c));
 }
 }  // namespace sdetr
-
-extern "C" int sdetr_rows_gather(const float *src, const int64_t *index, int batch, int num_rows, int k, int channels,
-                                 float *out, sdetr_stream_t stream) {
-    SDETR_REQUIRE(src && index && out, SDETR_ERR_INVALID_ARG, "rows_gather: null pointer");
-    SDETR_REQUIRE(batch > 0 && num_rows > 0 && k >= 0 && channels % 4 == 0 && aligned16(src) && aligned16(out),
-                  SDETR_ERR_INVALID_ARG, "rows_gather: bad sizes / alignment");
-    if (k == 0) return SDETR_OK;
-    rows_gather_kernel<<<row_blocks((int64_t)batch * k), kRowThreads, 0, (cudaStream_t)stream>>>(src, index, batch, num_rows, k,
-                                                                                                channels, out);
-    return check_launch("rows_gather");
-}
 
 extern "C" int sdetr_rows_scatter(float *dst, const int64_t *index, int batch, int num_rows, int k, int channels,
                                   const float *src, sdetr_stream_t stream) {

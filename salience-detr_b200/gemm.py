@@ -108,19 +108,8 @@ def _act_torch(x: Tensor, act) -> Tensor:
 
 
 def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input: bool = False,
-           input_act: Optional[str] = None, out: Optional[Tensor] = None) -> Tensor:
-    """y = act(x) @ weight.T + bias (act: None | "relu" | "gelu", fused into the operand load / split), inference only.
-    ``out``: optional 2-d (rows, N) destination (a row slice of a larger buffer); written in place by the 3xFP16 kernel, copied
-    into otherwise."""
-    if out is not None:
-        n0, k0 = weight.shape
-        if MODE == "auto" and OWN_KERNEL == "f16x3" and k0 % 64 == 0 and x.stride(-1) == 1 and x.numel() // k0 > SMALL_M:
-            x2 = x if x.dim() == 2 else x.reshape(-1, k0)
-            if x2.stride(0) % 4 == 0:
-                w_hi, w_lo, w_scale = split_weight_f16(weight)
-                return cabi.gemm_f16x3_pre(x2, w_hi, w_lo, w_scale, bias, 1 if relu_input else _ACT[input_act], out=out)
-        out.copy_(linear(x, weight, bias, relu_input, input_act).reshape(out.shape))
-        return out
+           input_act: Optional[str] = None) -> Tensor:
+    """y = act(x) @ weight.T + bias (act: None | "relu" | "gelu", fused into the operand load / split), inference only."""
     relu_input = 1 if relu_input else _ACT[input_act]
     n, k = weight.shape
     if MODE == "auto" and x.numel() // max(k, 1) <= SMALL_M:

@@ -147,15 +147,10 @@ class MultiScaleDeformableAttention(nn.Module):
 
     def forward_projected(self, query: Tensor, reference_points: Tensor, value_buf: Tensor, value_batch_stride: int,
                           value_token_stride: int, value_offset: int, num_value: int, spatial_shapes: Tensor,
-                          level_start_index: Tensor, query_order: Optional[Tensor] = None, schedule: int = 0,
-                          value_ready=None, proj: Optional[Tensor] = None) -> Tensor:
-        """Inference path with an already projected (and masked) value buffer; 2-d reference points.  ``value_ready``:
-        optional callable run right before the sampling launch (joins the stream that produces ``value_buf``)."""
-        if proj is None:  # else: the caller computed the offsets|logits projection already (overlapped with other work)
-            w, b = self.fused_projection()
-            proj = gemm.linear(query, w, b)
-        if value_ready is not None:
-            value_buf = value_ready()
+                          level_start_index: Tensor, query_order: Optional[Tensor] = None, schedule: int = 0) -> Tensor:
+        """Inference path with an already projected (and masked) value buffer; 2-d reference points."""
+        w, b = self.fused_projection()
+        proj = gemm.linear(query, w, b)
         out = cabi.msda_fused_forward(value_buf, value_batch_stride, value_token_stride, value_offset, spatial_shapes,
                                       level_start_index, reference_points, proj, self.num_heads,
                                       self.embed_dim // self.num_heads, self.num_levels, self.num_points, num_value,

@@ -17,7 +17,8 @@ How the path is laid out for an H100 (none of this is a translation of the refer
   the concatenated weights, the padded rows are zeroed once, and every layer samples its column slice;
 * per layer: one fused four-way gather, one GEMM for offsets|logits, one fused
   softmax+locations+sampling kernel (spatially tiled processing order), fused residual+LayerNorm,
-  in-place prefix-limited scatter.  Dense GEMMs / the 300-token MHA stay on cuBLAS / SDPA.
+  in-place prefix-limited scatter.  At C = 256 (head_dim 32) the 300-token pre-attention is three fused kernels and the
+  FFN is one; other widths run the pre-attention's projections / attention on cuBLAS / SDPA and the FFN as two GEMMs.
 """
 from __future__ import annotations
 
@@ -32,31 +33,8 @@ from torch.nn import functional as F
 from . import cabi, gemm
 from .ms_deform_attn import MultiScaleDeformableAttention
 
-OVERLAP_VALUE_PROJ = True  # all-layer value projection as a parallel branch (graph capture) / on a side stream (eager) beside the salience filter
-OVERLAP_VALUE_PROJ_EAGER = __import__("os").environ.get("SDETR_OVERLAP_EAGER", "0") != "0"  # eager too: off by default,
-# because the extra stream operations cost the (host-bound) eager path of the fresh-mask pipeline more than the overlap returns
-VALUE_PROJ_PER_LAYER = False  # (off: one N=1536 GEMM is cheaper than six N=256 ones)
-# each layer's value_proj as its own GEMM on a side stream beside that layer's (latency-bound)
-# pre-attention, joined right before the sampling kernel: the 45.7 MB it writes may still be in L2 when the
-# sampling kernel gathers from them (one 6-layer GEMM up front writes 274 MB, which L2 cannot hold), and the value rows
-# are 1 KB apart instead of 6 KB
-FUSED_GELU_MEAN = True     # MaskPredictor: GELU + token-mean of the global half as two fused launches (else torch ops)
-FUSED_QUERY_SUM = True     # `query + query_pos` written by the gather and kept current by the fused pre-attention (no add kernel)
-FUSED_PRE_ATTENTION = True  # C = 256 / head_dim 32: gather+in-proj, attention, out-proj+LN+scatter as three kernels
-# only for geometries the fused pre-attention does not cover (C != 256 or head_dim != 32):
-SMALL_ATTENTION = False   # sdetr_attention_small instead of SDPA between the library projections
-MHA_GEMM_TENSOR_CORE = False  # projections of the 600 rows on the tensor-core GEMM instead of cuBLAS SGEMM (latency-bound: slower)
-OVERLAP_PROJ = False  # (measured: 763 vs 773 images/s, e2e 918 vs 942 -- the extra launches and stream joins cost more than the overlap buys)
-# the offsets|logits GEMM of ALL rows runs on a side stream beside the (latency-bound, few-CTA) class-max /
-# top-300 / pre-attention chain, from the gather's q + pos; the 300 rows the pre-attention rewrites are recomputed afterwards
-FUSED_SMALL_PREDICTOR = __import__("os").environ.get("SDETR_FUSED_SMALL_PREDICTOR", "1") != "0"  # score modulation + MaskPredictor of a
-# level with at most PREDICTOR_SMALL_ROWS token rows as two fp32 kernels (csrc/predictor_small.cu) instead of ~15 latency-bound launches
-PREDICTOR_SMALL_ROWS = 4096
-FUSED_FFN = __import__("os").environ.get("SDETR_FUSED_FFN", "1") != "0"  # C = 256: linear1 -> ReLU -> linear2 -> +residual -> norm2
-# through sdetr_ffn_fused_layernorm (csrc/ffn_fused.cu: one persistent 3xFP16 kernel that keeps the hidden activations on chip)
-# instead of two gemm.linear calls and an add+LayerNorm launch
-FFN_CHUNK_ROWS = int(__import__("os").environ.get("SDETR_FFN_CHUNK", "0"))  # FFN in row chunks of this many rows, one FFN call
-# each.  0 (default) = one call over all rows.
+PREDICTOR_SMALL_ROWS = 4096  # score modulation + MaskPredictor of a level with at most this many token rows as two fp32
+# kernels (csrc/predictor_small.cu) instead of ~15 latency-bound launches; 0 = never
 TILE_CELL_PX = 64   # edge (image pixels) of the spatial cells that define the MSDA processing order
 MSDA_SCHEDULE = 1   # 0 = query-major, 1 = head-major chunks (see include/sdetr_b200.h)
 
@@ -101,7 +79,7 @@ class MaskPredictor(nn.Module):
         x = x if x.is_contiguous() else x.contiguous()
         z = gemm.linear(cabi.add_layernorm(x, None, ln.weight, ln.bias, ln.eps), fc.weight, fc.bias)
         half = self.h_dim // 2
-        if FUSED_GELU_MEAN and z.dim() == 3 and z.is_contiguous() and self.h_dim % 8 == 0 and self.h_dim <= 1024:
+        if z.dim() == 3 and z.is_contiguous() and self.h_dim % 8 == 0 and self.h_dim <= 1024:
             cabi.gelu_colmean_(z, half)  # GELU + global half = token mean, broadcast in place (:40-45), two launches
         else:
             z = F.gelu(z)
@@ -246,7 +224,7 @@ class SalienceTransformerEncoderLayer(nn.Module):
         b, nq, c = q.shape
         k = min(self.topk_sa, nq)
         top = cabi.topk_desc(mc, k)
-        if FUSED_PRE_ATTENTION and c == 256 and c // self.n_heads == 32 and k <= 448:  # attention kernel: K/V/P in smem
+        if c == 256 and c // self.n_heads == 32 and k <= 448:  # attention kernel: K/V/P in smem
             w_in_t, w_out_t = self._mha_transposed()
             t, qkv = cabi.mha_in_proj(q, qp, top, w_in_t, self.pre_attention.in_proj_bias)
             o = cabi.attention_qkv(qkv, self.n_heads)
@@ -256,66 +234,34 @@ class SalienceTransformerEncoderLayer(nn.Module):
         t, x = cabi.rows_gather_add(q, qp, top)           # t = q[top], x = t + qp[top]
         wqk, bqk, wv, bv = self._mha_views()
         h, d = self.n_heads, c // self.n_heads
-        lin = gemm.linear if MHA_GEMM_TENSOR_CORE else F.linear
-        qk = lin(x, wqk, bqk).view(b, k, 2, h, d)
-        v = lin(t, wv, bv).view(b, k, h, d)
-        if SMALL_ATTENTION and d == 32 and k <= 700 and qk.is_contiguous() and v.is_contiguous():
-            o = cabi.attention_small(qk, v)
-        else:
-            o = F.scaled_dot_product_attention(qk[:, :, 0].transpose(1, 2), qk[:, :, 1].transpose(1, 2), v.transpose(1, 2))
-            o = o.transpose(1, 2).reshape(b, k, c)
-        o = lin(o, self.pre_attention.out_proj.weight, self.pre_attention.out_proj.bias)
+        qk = F.linear(x, wqk, bqk).view(b, k, 2, h, d)
+        v = F.linear(t, wv, bv).view(b, k, h, d)
+        o = F.scaled_dot_product_attention(qk[:, :, 0].transpose(1, 2), qk[:, :, 1].transpose(1, 2), v.transpose(1, 2))
+        o = o.transpose(1, 2).reshape(b, k, c)
+        o = F.linear(o, self.pre_attention.out_proj.weight, self.pre_attention.out_proj.bias)
         t = cabi.add_layernorm(t, o, self.pre_norm.weight, self.pre_norm.bias, self.pre_norm.eps)
         cabi.rows_scatter_(q, top, t)  # q is this layer's private gather buffer
         return q, None, top
 
-    def overlaps_projection(self, nq: int) -> bool:
-        """True when the fused pre-attention runs (it keeps `q + pos` current), i.e. when the stale-row patch is exact."""
-        return (OVERLAP_PROJ and FUSED_PRE_ATTENTION and FUSED_QUERY_SUM and self.embed_dim == 256 and
-                self.embed_dim // self.n_heads == 32 and min(self.topk_sa, nq) <= 448)
-
     def forward_fast(self, q, qp, mc, ref_q, vbuf, v_bstride, v_tstride, v_off, num_value, spatial_shapes,
-                     level_start_index, order=None, schedule=MSDA_SCHEDULE, qs=None, value_ready=None, proj_future=None):
-        """``qs``: optional q + qp buffer (from the gather); the fused pre-attention keeps its rewritten rows current.
-        ``value_ready``: optional callable returning the value buffer, run right before the sampling launch.
-        ``proj_future``: optional (proj, side_stream): the offsets|logits projection of the PRE-attention ``qs``, in flight on
-        a side stream; joined here and the top-k rows the pre-attention rewrote are recomputed."""
+                     level_start_index, order=None, qs=None):
+        """``qs``: optional q + qp buffer (from the gather); the fused pre-attention keeps its rewritten rows current."""
         q, qs, top = self._pre_attention_fast(q, qp, mc, qs)
-        proj = None
-        if proj_future is not None:
-            proj, side = proj_future
-            cur = torch.cuda.current_stream(q.device)
-            cur.wait_stream(side)
-            proj.record_stream(cur)
-            # the side-stream GEMM may have read the rewritten rows mid-update: exactly those rows are replaced here
-            w, bias = self.self_attn.fused_projection()
-            cabi.rows_scatter_(proj, top, F.linear(cabi.rows_gather(qs, top), w, bias).contiguous())
         a = self.self_attn.forward_projected(qs if qs is not None else q + qp, ref_q, vbuf, v_bstride, v_tstride, v_off, num_value, spatial_shapes,
-                                             level_start_index, order, schedule, value_ready=value_ready, proj=proj)
+                                             level_start_index, order, MSDA_SCHEDULE)
         q = cabi.add_layernorm(q, a, self.norm1.weight, self.norm1.bias, self.norm1.eps, out=q)
         rows = q.shape[0] * q.shape[1]
         relu = isinstance(self.activation, nn.ReLU)
-        if (FUSED_FFN and relu and self.embed_dim == 256 and self.linear1.out_features % 128 == 0 and gemm.MODE == "auto" and
+        if (relu and self.embed_dim == 256 and self.linear1.out_features % 128 == 0 and gemm.MODE == "auto" and
                 gemm.OWN_KERNEL == "f16x3" and rows > gemm.SMALL_M and q.is_contiguous()):
             return cabi.ffn_fused_layernorm(q, gemm.split_weight_f16(self.linear1.weight), self.linear1.bias,
                                             gemm.split_weight_f16(self.linear2.weight), self.linear2.bias, self.norm2.weight,
                                             self.norm2.bias, self.norm2.eps, out=q)
-        if FFN_CHUNK_ROWS and relu and rows > FFN_CHUNK_ROWS + FFN_CHUNK_ROWS // 2:
-            q2 = q.view(rows, q.shape[-1])
-            f = torch.empty_like(q2)
-            n_chunks = -(-rows // FFN_CHUNK_ROWS)
-            step = -(-rows // n_chunks // 128) * 128  # equal chunks, whole 128-row panels
-            for r0 in range(0, rows, step):
-                h = gemm.linear(q2[r0:r0 + step], self.linear1.weight, self.linear1.bias)
-                gemm.linear(h, self.linear2.weight, self.linear2.bias, relu_input=True, out=f[r0:r0 + step])
-                del h  # the caching allocator hands the same block to the next chunk: the hidden buffer stays in L2
-            f = f.view_as(q)
-        else:
-            h = gemm.linear(q, self.linear1.weight, self.linear1.bias)
-            if relu:
-                f = gemm.linear(h, self.linear2.weight, self.linear2.bias, relu_input=True)  # ReLU fused into the operand split
-            else:  # any other activation module of the reference's constructor argument
-                f = gemm.linear(self.activation(h), self.linear2.weight, self.linear2.bias)
+        h = gemm.linear(q, self.linear1.weight, self.linear1.bias)
+        if relu:
+            f = gemm.linear(h, self.linear2.weight, self.linear2.bias, relu_input=True)  # ReLU fused into the operand split
+        else:  # any other activation module of the reference's constructor argument
+            f = gemm.linear(self.activation(h), self.linear2.weight, self.linear2.bias)
         return cabi.add_layernorm(q, f, self.norm2.weight, self.norm2.bias, self.norm2.eps, out=q)
 
 
@@ -344,13 +290,6 @@ class SalienceTransformerEncoder(nn.Module):
             rx = xs[None, None, :].expand(1, h, w).reshape(1, -1) / (valid_ratios[:, None, lvl, 0] * w)
             refs.append(torch.stack((rx, ry), -1))
         return torch.cat(refs, 1)[:, :, None] * valid_ratios[:, None]
-
-    def _side_stream(self, device):
-        streams = self.__dict__.setdefault("_side_streams", {})
-        key = str(device)
-        if key not in streams:
-            streams[key] = torch.cuda.Stream(device=device)
-        return streams[key]
 
     def _value_projection(self):
         """[6*C, C] weight / [6*C] bias of all layers' value_proj (rebuilt when any of them changes)."""
@@ -390,14 +329,9 @@ class SalienceTransformerEncoder(nn.Module):
         query = query.contiguous()  # the reference hands over a transposed view (base_transformer.py:21-26)
         mask_u8 = query_key_padding_mask.to(torch.uint8).contiguous()
         focus = focus_token_nums.to(torch.int32).contiguous()
-        per_layer = VALUE_PROJ_PER_LAYER and value_buffer is None
-        if per_layer:
-            cur = torch.cuda.current_stream(query.device)
-            side = self._side_stream(query.device)
-            vbuf, wide = None, c
-        else:  # one GEMM for the value projections of all layers; zero the padded rows once
-            vbuf = value_buffer if value_buffer is not None else self.project_values(query, mask_u8)
-            wide = vbuf.shape[-1]
+        # one GEMM for the value projections of all layers; zero the padded rows once
+        vbuf = value_buffer if value_buffer is not None else self.project_values(query, mask_u8)
+        wide = vbuf.shape[-1]
         out = query.clone()  # `value` stays the original tokens (:452); `out` is updated in place
         spatial_shapes = spatial_shapes.to(torch.int64).contiguous()
         level_start_index = level_start_index.to(torch.int64).contiguous()
@@ -408,35 +342,10 @@ class SalienceTransformerEncoder(nn.Module):
         for j, layer in enumerate(self.layers):
             inds = foreground_inds[j]
             nq = inds.shape[1]
-            qs = None
-            if FUSED_QUERY_SUM:
-                q, qp, fq, rq, qs = cabi.token_gather(out, pos, fg, vr, inds, spatial_shapes, level_start_index, nq, want_sum=True)
-            else:
-                q, qp, fq, rq = cabi.token_gather(out, pos, fg, vr, inds, spatial_shapes, level_start_index, nq)
-            ready = None
-            if per_layer:
-                # fork: this layer's value_proj (all Nv tokens, ms_deform_attn.py:316-319) runs beside the gather / class
-                # head / 300-token pre-attention; `ready` joins it right before the sampling kernel
-                side.wait_stream(cur)
-                with torch.cuda.stream(side):
-                    vj = layer.self_attn.project_value(query, None)
-                    cabi.zero_masked_rows_(vj, c, c, mask_u8, b * nv)
-
-                def ready(vj=vj):
-                    cur.wait_stream(side)
-                    vj.record_stream(cur)
-                    return vj
-            fut = None
-            if qs is not None and layer.overlaps_projection(nq):
-                cur_s, side_s = torch.cuda.current_stream(query.device), self._side_stream(query.device)
-                side_s.wait_stream(cur_s)
-                with torch.cuda.stream(side_s):
-                    wf, bf = layer.self_attn.fused_projection()
-                    fut = (gemm.linear(qs, wf, bf), side_s)
+            q, qp, fq, rq, qs = cabi.token_gather(out, pos, fg, vr, inds, spatial_shapes, level_start_index, nq, want_sum=True)
             mc = cabi.class_max_times_fg(gemm.linear(q, self.enhance_mcsp.weight, self.enhance_mcsp.bias), fq)
-            q = layer.forward_fast(q, qp, mc, rq, vbuf, nv * wide, wide, 0 if per_layer else j * c, nv, spatial_shapes,
-                                   level_start_index, None if query_orders is None else query_orders[j], qs=qs,
-                                   value_ready=ready, proj_future=fut)
+            q = layer.forward_fast(q, qp, mc, rq, vbuf, nv * wide, wide, j * c, nv, spatial_shapes,
+                                   level_start_index, None if query_orders is None else query_orders[j], qs=qs)
             cabi.token_scatter_(out, q, inds, focus)
         if multi_level_masks is not None:
             cabi.background_embed_(out, mask_u8, inds, self.background_embedding.row_embed.weight,
@@ -528,8 +437,8 @@ class SalienceTransformer(nn.Module):
         self.alpha.data.uniform_(-0.3, 0.3)
 
     def _side_stream(self, device):
-        """One side stream per (device, CURRENT stream): lanes that run the model eagerly on their own streams (FreshMaskPipeline)
-        must not meet on a shared side stream, which would order their value projections one after the other."""
+        """One side stream per (device, CURRENT stream): forwards captured from different streams must not meet on a shared
+        side stream, which would order their value projections one after the other."""
         streams = self.__dict__.setdefault("_side_streams", {})
         key = (str(device), torch.cuda.current_stream(device).cuda_stream)
         if key not in streams:
@@ -638,7 +547,7 @@ class SalienceTransformer(nn.Module):
         raw = torch.empty(b, nv, device=feat.device, dtype=torch.float32)
         prev = None
         mp = self.enc_mask_predictor
-        small_ok = (not grad and FUSED_SMALL_PREDICTOR and c == 256 and mp.h_dim == 256 and mp.layer1[1].in_features == 256 and
+        small_ok = (not grad and c == 256 and mp.h_dim == 256 and mp.layer1[1].in_features == 256 and
                     mem.is_contiguous())
         for lvl in range(L - 1, -1, -1):
             h, w = plan.shapes_list[lvl]
@@ -703,10 +612,10 @@ class SalienceTransformer(nn.Module):
                                                 [p.contiguous() for p in multi_level_pos_embeds],
                                                 self.level_embeds.detach().contiguous(), plan.keep.view(plan.keep.shape[0], -1))
         vbuf = None
-        if (OVERLAP_VALUE_PROJ and not VALUE_PROJ_PER_LAYER and not grad and feat.is_cuda and
-                (OVERLAP_VALUE_PROJ_EAGER or torch.cuda.is_current_stream_capturing())):
+        if not grad and feat.is_cuda and torch.cuda.is_current_stream_capturing():
             # fork: the (large) value projection only needs the tokens, so it becomes a parallel branch of the captured
-            # CUDA graph -- or, eagerly, runs on a side stream -- beside the salience filter's many small kernels
+            # CUDA graph beside the salience filter's many small kernels.  Not eagerly: there the extra stream operations
+            # cost the host-bound path (e.g. the fresh-mask pipeline) more than the overlap returns
             cur = torch.cuda.current_stream(feat.device)
             side = self._side_stream(feat.device)
             side.wait_stream(cur)

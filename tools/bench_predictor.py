@@ -27,7 +27,7 @@ with torch.no_grad():
         for lvl in range(L - 1, -1, -1):
             h, w = plan.shapes_list[lvl]
             s0 = plan.level_start[lvl]
-            if st.FUSED_SMALL_PREDICTOR and b * h * w <= st.PREDICTOR_SMALL_ROWS:
+            if b * h * w <= st.PREDICTOR_SMALL_ROWS:
                 hc, wc = plan.shapes_list[lvl + 1] if lvl != L - 1 else (0, 0)
                 coarse = raw[:, plan.level_start[lvl + 1]:plan.level_start[lvl + 1] + hc * wc] if lvl != L - 1 else None
                 ln = mp.layer1[0]
@@ -54,7 +54,6 @@ with torch.no_grad():
 
     outs = {}
     for rows in [0] + rows_arg:
-        st.FUSED_SMALL_PREDICTOR = rows > 0
         st.PREDICTOR_SMALL_ROWS = rows
         for _ in range(2):
             scores()

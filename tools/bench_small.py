@@ -1,11 +1,10 @@
 """Latency of the small (launch-bound) pieces with a warm L2, as they run inside a step: small-M dense projections
-(hand-written wgmma kernel vs cuBLAS fp32) and the 300-token pre-attention (fused kernels vs library path)."""
+(hand-written wgmma kernel vs cuBLAS fp32) and the 300-token pre-attention (fused kernels, whole and per part)."""
 import os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.nn.functional as F
 import salience_detr_b200 as pkg
-import salience_detr_b200.salience_transformer as st
 from salience_detr_b200.synthetic import build_model
 
 dev = "cuda:0"
@@ -59,10 +58,7 @@ torch.manual_seed(0)
 for b, nq in [(2, 11363), (2, 2272)]:
     q = torch.randn(b, nq, 256, device=dev); qp = torch.randn(b, nq, 256, device=dev); mc = torch.randn(b, nq, device=dev)
     with torch.no_grad():
-        res = {}
-        for fused in (False, True):
-            st.FUSED_PRE_ATTENTION = fused
-            res[fused] = graph_time(lambda: layer._pre_attention_fast(q, qp, mc), inner=10)
+        whole = graph_time(lambda: layer._pre_attention_fast(q, qp, mc), inner=10)
         top = pkg.cabi.topk_desc(mc, 300)
         w_in_t, w_out_t = layer._mha_transposed()
         t, qkv = pkg.cabi.mha_in_proj(q, qp, top, w_in_t, layer.pre_attention.in_proj_bias)
@@ -74,5 +70,5 @@ for b, nq in [(2, 11363), (2, 2272)]:
             "out_proj_ln_scatter": graph_time(lambda: pkg.cabi.mha_out_proj_ln_scatter_(q, o, t, w_out_t, layer.pre_attention.out_proj.bias,
                                                                                        layer.pre_norm.weight, layer.pre_norm.bias, 1e-5, top)),
         }
-    print(f"pre-attention b={b} nq={nq}: library path {res[False]:.1f} us, fused path {res[True]:.1f} us; parts:",
+    print(f"pre-attention b={b} nq={nq}: {whole:.1f} us; parts:",
           {k: round(v, 1) for k, v in parts.items()})

@@ -45,7 +45,7 @@ def wrap(mod, name):
 
 for name in ("token_gather", "class_max_times_fg", "topk_desc", "rows_gather_add", "add_layernorm", "rows_scatter_",
              "token_scatter_", "background_embed_", "msda_fused_forward", "salience_select", "order_prefixes",
-             "flatten_tokens", "zero_masked_rows_", "score_modulate_", "attention_small"):
+             "flatten_tokens", "zero_masked_rows_", "score_modulate_"):
     if hasattr(cabi, name):
         wrap(cabi, name)
 wrap(gemm, "linear")

@@ -44,7 +44,7 @@ def install():
     from salience_detr_b200 import cabi, gemm
     for name in ("token_gather", "class_max_times_fg", "topk_desc", "rows_gather_add", "add_layernorm", "rows_scatter_",
                  "token_scatter_", "background_embed_", "msda_fused_forward", "salience_select", "order_prefixes",
-                 "flatten_tokens", "zero_masked_rows_", "score_modulate_", "attention_small", "rows_gather", "split_tf32",
+                 "flatten_tokens", "zero_masked_rows_", "score_modulate_", "split_tf32",
                  "gemm_3xtf32_raw", "gemm_3xtf32"):
         if hasattr(cabi, name):
             _wrap(cabi, name)

@@ -24,7 +24,6 @@ args = ap.parse_args()
 if args.schedule is not None:
     import salience_detr_b200.salience_transformer as st
     st.MSDA_SCHEDULE = args.schedule
-    st.SalienceTransformerEncoderLayer.forward_fast.__defaults__ = (None, args.schedule)
 
 pkg.gemm.MODE = args.gemm
 dev = torch.device("cuda:0")

@@ -459,6 +459,27 @@ int sdetr_context_gate(const float *y, int64_t y_pitch, int64_t ldy, const float
 int sdetr_upsample_nearest_concat(const float *hi, int64_t hi_pitch, int64_t ldh, int Hi, int Wi, const float *lo, int64_t lo_pitch,
                                   int64_t ldl, int Ho, int Wo, int batch, int C, float *dst, int64_t dst_pitch, int64_t ldd,
                                   sdetr_stream_t stream);
+
+/* ---- ChannelMapper in token layout (models/necks/channel_mapper.py:8-80; ChannelMapper.forward_tokens) ----------------------
+ * GroupNorm of every level of a token buffer (nn.GroupNorm per level, models/bricks/misc.py:97-98): image n, token t, channel c
+ * at x + n * pitch + t * C + c (floats); level l = the level_size_host[l] tokens after the previous levels'.  Statistics per
+ * (image, level, group of C / num_groups consecutive channels) over all H*W*C/G elements of the level (padding pixels included,
+ * as nn.GroupNorm): per-tile Welford (count, mean, M2) partials merged with Chan's formula in a fixed order (no atomics; the
+ * result is bit-identical from run to run and does not depend on the grid); biased variance, rstd = rsqrt(var + eps);
+ * y = (x - mean) * rstd * gamma[l] + beta[l].  gamma / beta: (num_levels, C) row-major.  y may alias x (same pitch and rows).
+ * C % 4 == 0, C <= 4096, C % num_groups == 0 (else SDETR_ERR_UNSUPPORTED); x, y, gamma, beta, pitch 16-byte aligned.
+ * Three launches for all levels.  workspace: sdetr_group_norm_tokens_workspace_floats(...) floats, 8-byte aligned. */
+int64_t sdetr_group_norm_tokens_workspace_floats(int batch, int channels, int num_groups, int num_levels, const int32_t *level_size_host);
+int sdetr_group_norm_tokens(const float *x, float *y, int64_t pitch, int batch, int channels, int num_levels,
+                            const int32_t *level_size_host, const float *gamma, const float *beta, int num_groups, float eps,
+                            float *workspace, int64_t workspace_floats, sdetr_stream_t stream);
+/* The transformer's front end for features that are already tokens (salience_transformer.py:107-113 without the flatten):
+ * lpos = pos + level_embeds[l];  x = (feat + lpos) * keep[b,t]  -- the operations of sdetr_flatten_tokens[_pos] in the same
+ * order, so lpos and x are bit-identical to theirs for the same values.  feat, pos, lpos, x (b,Nv,C) contiguous, 16-byte
+ * aligned; keep (b,Nv); level_embeds (L,C); lpos may alias pos.  C % 4 == 0.  One launch. */
+int sdetr_token_lpos_keep(const float *feat, const float *pos, const float *level_embeds, const float *keep,
+                          const int32_t *level_size_host, int batch, int channels, int num_levels, float *lpos, float *x,
+                          sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

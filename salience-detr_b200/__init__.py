@@ -34,6 +34,7 @@ from .neck import (  # noqa: F401
     RepVggPluXBlock,
     SqueezeAndExcitation,
 )
+from .channel_mapper import ChannelMapper, level_views, tokens_of  # noqa: F401
 from .salience_transformer import (  # noqa: F401
     EncoderPlan,
     MaskPredictor,

@@ -85,6 +85,9 @@ SIGNATURES = {
     "sdetr_context_gate": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp,
                                 _i64, _i64, _vp]),
     "sdetr_upsample_nearest_concat": (_i, [_vp, _i64, _i64, _i, _i, _vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
+    "sdetr_group_norm_tokens_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
+    "sdetr_group_norm_tokens": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _i, _f, _vp, _i64, _vp]),
+    "sdetr_token_lpos_keep": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 
@@ -924,3 +927,40 @@ def upsample_nearest_concat(hi, hi_hw, lo, lo_hw, out=None):
                                              int(wo), b, c, *_token_rows(out, "out"), _stream())
     _check(rc, "sdetr_upsample_nearest_concat")
     return out
+
+
+# ---- ChannelMapper in token layout (channel_mapper.ChannelMapper.forward_tokens) ----------------------------------------------
+def group_norm_tokens_(tokens, level_sizes: Sequence[int], gamma, beta, num_groups: int, eps: float):
+    """nn.GroupNorm of every level of ``tokens`` (b, Nv, C) in place (three launches for all levels).  ``tokens`` may be a
+    token-range view of a larger buffer (unit channel stride, rows C apart); gamma / beta: (L, C) contiguous."""
+    b, nv, c = tokens.shape
+    L = len(level_sizes)
+    if not (tokens.is_cuda and tokens.dtype == torch.float32 and tokens.stride(2) == 1 and tokens.stride(1) == c):
+        raise RuntimeError("group_norm_tokens_: tokens must be CUDA float32 (b, Nv, C) with contiguous rows")
+    if sum(level_sizes) != nv or tuple(gamma.shape) != (L, c) or tuple(beta.shape) != (L, c):
+        raise RuntimeError(f"group_norm_tokens_: {nv} tokens, levels {list(level_sizes)}, gamma / beta must be ({L}, {c})")
+    sizes = _host_i32(level_sizes)
+    ws = torch.empty(max(int(lib().sdetr_group_norm_tokens_workspace_floats(b, c, int(num_groups), L, sizes)), 4),
+                     device=tokens.device, dtype=torch.float32)
+    pitch = tokens.stride(0) if b > 1 else nv * c
+    rc = lib().sdetr_group_norm_tokens(tokens.data_ptr(), tokens.data_ptr(), pitch, b, c, L, sizes, _req(gamma, "gamma", torch.float32),
+                                       _req(beta, "beta", torch.float32), int(num_groups), float(eps), ws.data_ptr(), ws.numel(),
+                                       _stream())
+    _check(rc, "sdetr_group_norm_tokens")
+    return tokens
+
+
+def token_lpos_keep(feat, pos, level_embeds, keep, level_sizes: Sequence[int], lpos=None):
+    """feat / pos (b, Nv, C) tokens -> (lpos, x): lpos = pos + level_embeds[l], x = (feat + lpos) * keep, bit-identical to
+    flatten_tokens[_pos] on the same values.  ``lpos``: optional destination, may be ``pos`` itself (in place)."""
+    b, nv, c = feat.shape
+    if tuple(pos.shape) != (b, nv, c) or sum(level_sizes) != nv or tuple(level_embeds.shape[1:]) != (c,):
+        raise RuntimeError(f"token_lpos_keep: pos must be {(b, nv, c)}, the levels must sum to {nv}, level_embeds (L, {c})")
+    lpos = lpos if lpos is not None else torch.empty_like(feat)
+    x = torch.empty_like(feat)
+    rc = lib().sdetr_token_lpos_keep(_req(feat, "feat", torch.float32), _req(pos, "pos", torch.float32),
+                                     _req(level_embeds, "level_embeds", torch.float32), _req(keep, "keep", torch.float32),
+                                     _host_i32(level_sizes), b, c, len(level_sizes), _req(lpos, "lpos", torch.float32), x.data_ptr(),
+                                     _stream())
+    _check(rc, "sdetr_token_lpos_keep")
+    return lpos, x

@@ -154,12 +154,12 @@ def nearest_index(n_in: int, n_out: int) -> Tensor:
 
 
 class _KConv:
-    """one folded convolution in kernel form: (Cout, k, k, Cin / groups) fp16 pair with its device scale, fp32 bias"""
+    """one folded convolution in kernel form: (Cout, k, k, Cin / groups) fp16 pair with its device scale, fp32 bias (or None)"""
 
-    def __init__(self, w: Tensor, b: Tensor, groups: int, stride: int, act: int):
+    def __init__(self, w: Tensor, b: Optional[Tensor], groups: int, stride: int, act: int):
         self.ksize, self.groups, self.stride, self.act = w.shape[-1], groups, stride, act
         self.w_hi, self.w_lo, self.w_scale = cabi.split_f16_pair_dev(w.float().permute(0, 2, 3, 1).contiguous())
-        self.bias = b.float().contiguous()
+        self.bias = b.float().contiguous() if b is not None else None
 
     def __call__(self, x: Tensor, base: Tensor, hw, out=None) -> Tensor:
         """x: (b, H*W, Cin) token view inside the contiguous tensor ``base`` (its activation scale is taken over base)"""

@@ -31,6 +31,7 @@ from torch import Tensor, nn
 from torch.nn import functional as F
 
 from . import cabi, gemm
+from .channel_mapper import tokens_of
 from .ms_deform_attn import MultiScaleDeformableAttention
 
 PREDICTOR_SMALL_ROWS = 4096  # score modulation + MaskPredictor of a level with at most this many token rows as two fp32
@@ -599,7 +600,18 @@ class SalienceTransformer(nn.Module):
             plan = self.make_plan(multi_level_masks)
         grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         x = None
-        if multi_level_pos_embeds is None:  # position embedding computed on the device from the masks, in token layout
+        tokens = None if grad else tokens_of(multi_level_feats)
+        if tokens is not None and tokens.is_cuda and tokens.dtype == torch.float32:
+            # the features are level views of one token buffer (ChannelMapper): it is the token layout already.  lpos and x are
+            # bit-identical to what the flatten kernels make from .contiguous() copies of the same maps
+            feat = tokens
+            keep, embeds = plan.keep.view(plan.keep.shape[0], -1), self.level_embeds.detach().contiguous()
+            if multi_level_pos_embeds is None:
+                lpos, x = cabi.token_lpos_keep(feat, self.position_tokens(plan), embeds, keep, plan.level_size)
+            else:
+                pos = cabi.maps_to_tokens([p.contiguous() for p in multi_level_pos_embeds])
+                lpos, x = cabi.token_lpos_keep(feat, pos, embeds, keep, plan.level_size, lpos=pos)
+        elif multi_level_pos_embeds is None:  # position embedding computed on the device from the masks, in token layout
             if grad:
                 raise RuntimeError("training path: pass the per-level position embeddings explicitly")
             feat, lpos, x = cabi.flatten_tokens_pos([f.contiguous() for f in multi_level_feats], self.position_tokens(plan),

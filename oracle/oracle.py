@@ -204,7 +204,8 @@ def _ln(sd, name, x):
 
 
 def msda_module(sd, pre, query, ref, value, shapes, lsi, mask, heads, levels, points, core="torch"):
-    """Restates MultiScaleDeformableAttention.forward (ms_deform_attn.py:311-377), 2-d ref points."""
+    """Restates MultiScaleDeformableAttention.forward (ms_deform_attn.py:311-377): 2-d reference points (encoder) or 4-d
+    reference boxes (decoder, :345-349).  Differentiable, in the dtype / on the device of ``query`` with ``core="torch"``."""
     b, nq, c = query.shape
     nv = value.shape[1]
     v = _lin(sd, pre + "value_proj", value)
@@ -214,8 +215,11 @@ def msda_module(sd, pre, query, ref, value, shapes, lsi, mask, heads, levels, po
     off = _lin(sd, pre + "sampling_offsets", query).view(b, nq, heads, levels, points, 2)
     w = _lin(sd, pre + "attention_weights", query).view(b, nq, heads, levels * points).softmax(-1)
     w = w.view(b, nq, heads, levels, points)
-    norm = torch.stack([shapes[:, 1], shapes[:, 0]], -1)
-    loc = ref[:, :, None, :, None, :] + off / norm[None, None, None, :, None, :]
+    if ref.shape[-1] == 4:
+        loc = ref[:, :, None, :, None, :2] + off / points * ref[:, :, None, :, None, 2:] * 0.5
+    else:
+        norm = torch.stack([shapes[:, 1], shapes[:, 0]], -1).to(off)  # integers: exact in any float dtype
+        loc = ref[:, :, None, :, None, :] + off / norm[None, None, None, :, None, :]
     if core == "torch":
         out = msda_core_torch(v, shapes.tolist(), loc, w)
     else:
@@ -257,12 +261,13 @@ def proposal_keep_mask(mask_flat, shapes_list):
     b = mask_flat.shape[0]
     keep = []
     cur = 0
+    dev = mask_flat.device  # float32 whatever the model's dtype: the mask is a selection, made as the fp32 model makes it
     for lvl, (h, w) in enumerate(shapes_list):
         m = mask_flat[:, cur:cur + h * w].view(b, h, w)
         vh = (~m[:, :, 0]).sum(1)
         vw = (~m[:, 0, :]).sum(1)
-        gy = (torch.arange(h, dtype=torch.float32) + 0.5)[None, :, None] / vh[:, None, None]
-        gx = (torch.arange(w, dtype=torch.float32) + 0.5)[None, None, :] / vw[:, None, None]
+        gy = (torch.arange(h, dtype=torch.float32, device=dev) + 0.5)[None, :, None] / vh[:, None, None]
+        gx = (torch.arange(w, dtype=torch.float32, device=dev) + 0.5)[None, None, :] / vw[:, None, None]
         wh = 0.05 * 2.0 ** lvl
         ok = (gy > 0.01) & (gy < 0.99) & (gx > 0.01) & (gx < 0.99) & (0.01 < wh < 0.99)
         keep.append((ok & ~m).flatten(1))
@@ -270,18 +275,23 @@ def proposal_keep_mask(mask_flat, shapes_list):
     return torch.cat(keep, 1)
 
 
-def salience_filter(sd, feat, lpos, mask_flat, masks, shapes, lsi, level_ratio, layer_ratio):
-    """Restates salience_transformer.py:112-168.  Returns a dict of everything the encoder consumes."""
+def salience_filter(sd, feat, lpos, mask_flat, masks, shapes, lsi, level_ratio, layer_ratio, selection=None):
+    """Restates salience_transformer.py:112-168.  Returns a dict of everything the encoder consumes.
+
+    Runs in the dtype / on the device of ``feat``; the scores stay differentiable.  ``selection``: optional dict with any of
+    ``selected_inds``, ``foreground_score``, ``focus_token_nums``, ``layer_num_query`` that replace what this function would
+    compute (no gradient flows through them), so that a float64 twin of a float32 run processes exactly the tokens that run
+    chose instead of re-deciding near-ties at the top-k boundary."""
     shapes_list = shapes.tolist()
     L = len(shapes_list)
     b = feat.shape[0]
     keep = proposal_keep_mask(mask_flat, shapes_list)
     mem = _ln(sd, "enc_output_norm", _lin(sd, "enc_output", (feat + lpos) * keep[..., None]))
     valid = torch.stack([(~m).sum((1, 2)) for m in masks], -1)
-    focus = (valid * torch.tensor(level_ratio, dtype=torch.float32)).int()
-    level_token_nums = focus.max(0)[0]
+    focus = (valid * torch.tensor(level_ratio, dtype=torch.float32, device=valid.device)).int()
+    level_token_nums = focus.max(0)[0].cpu()
     focus_token_nums = focus.sum(-1)
-    raw = torch.empty(b, feat.shape[1])
+    raw = torch.empty(b, feat.shape[1], dtype=feat.dtype, device=feat.device)
     score = None
     for lvl in range(L - 1, -1, -1):
         h, w = shapes_list[lvl]
@@ -293,33 +303,43 @@ def salience_filter(sd, feat, lpos, mask_flat, masks, shapes, lsi, level_ratio, 
         s = mask_predictor(sd, "enc_mask_predictor.", m_l)
         raw[:, s0:s0 + h * w] = s.squeeze(-1)
         score = s.transpose(1, 2).reshape(b, 1, h, w)
-    hw = shapes.prod(1)
-    inds, sel_score, fg = c_salience_select(raw, mask_flat, lsi, hw, level_token_nums.tolist())
+    sel = dict(selection or {})
+    if "selected_inds" in sel and "foreground_score" in sel:
+        inds, sel_score, fg = sel["selected_inds"], None, sel["foreground_score"]
+    else:
+        hw = shapes.prod(1).cpu()
+        inds, sel_score, fg = c_salience_select(raw.detach().float().cpu(), mask_flat.cpu(), lsi.cpu(), hw,
+                                                level_token_nums.tolist())
+        inds, sel_score, fg = inds.to(feat.device), sel_score.to(feat.device), fg.to(feat.device)
     K = inds.shape[1]
     nq = (K * torch.tensor(layer_ratio, dtype=torch.float32)).to(torch.int64).tolist()
     return dict(memory0=mem, raw_score=raw, selected_inds=inds, selected_score=sel_score,
-                foreground_score=fg, level_token_nums=level_token_nums, focus_token_nums=focus_token_nums,
-                layer_num_query=nq)
+                foreground_score=fg, level_token_nums=level_token_nums,
+                focus_token_nums=sel.get("focus_token_nums", focus_token_nums),
+                layer_num_query=list(sel.get("layer_num_query", nq)))
 
 
 def reference_points(shapes_list, valid_ratios):
     """Restates SalienceTransformerEncoder.get_reference_points (salience_transformer.py:417-432)."""
     refs = []
+    kw = dict(dtype=valid_ratios.dtype, device=valid_ratios.device)
     for lvl, (h, w) in enumerate(shapes_list):
-        ys = (torch.arange(h, dtype=torch.float32) + 0.5)
-        xs = (torch.arange(w, dtype=torch.float32) + 0.5)
+        ys = (torch.arange(h, **kw) + 0.5)
+        xs = (torch.arange(w, **kw) + 0.5)
         ry = ys[None, :, None].expand(1, h, w).reshape(1, -1) / (valid_ratios[:, None, lvl, 1] * h)
         rx = xs[None, None, :].expand(1, h, w).reshape(1, -1) / (valid_ratios[:, None, lvl, 0] * w)
         refs.append(torch.stack((rx, ry), -1))
     return torch.cat(refs, 1)[:, :, None] * valid_ratios[:, None]
 
 
-def pre_attention(sd, pre, q, qp, cls, fg_q, heads, topk_sa):
-    """Restates salience_transformer.py:366-379 (top-k salient tokens -> MHA -> LN -> scatter)."""
+def pre_attention(sd, pre, q, qp, cls, fg_q, heads, topk_sa, order=None):
+    """Restates salience_transformer.py:366-379 (top-k salient tokens -> MHA -> LN -> scatter).  ``order``: optional (b,k)
+    positions of the top-k tokens to use instead of ranking ``cls * fg_q`` here."""
     b, nq, c = q.shape
-    mc = cls.max(-1)[0] * fg_q
-    # canonical tie order (score desc, position asc); the set is what matters (MHA is permutation-equivariant)
-    order = torch.sort(mc, dim=1, descending=True, stable=True)[1][:, :topk_sa]
+    if order is None:
+        mc = cls.max(-1)[0] * fg_q
+        # canonical tie order (score desc, position asc); the set is what matters (MHA is permutation-equivariant)
+        order = torch.sort(mc, dim=1, descending=True, stable=True)[1][:, :topk_sa]
     ix = order[..., None].expand(-1, -1, c)
     t, tp = q.gather(1, ix), qp.gather(1, ix)
     x = t + tp
@@ -334,9 +354,9 @@ def pre_attention(sd, pre, q, qp, cls, fg_q, heads, topk_sa):
 
 
 def encoder_layer(sd, pre, q, qp, value, ref_q, shapes, lsi, mask, cls, fg_q, heads, levels, points,
-                  topk_sa, core="torch"):
+                  topk_sa, core="torch", pre_order=None):
     """Restates SalienceTransformerEncoderLayer.forward (salience_transformer.py:353-396)."""
-    q, _ = pre_attention(sd, pre, q, qp, cls, fg_q, heads, topk_sa)
+    q, _ = pre_attention(sd, pre, q, qp, cls, fg_q, heads, topk_sa, pre_order)
     a = msda_module(sd, pre + "self_attn.", q + qp, ref_q, value, shapes, lsi, mask, heads, levels, points, core)
     q = _ln(sd, pre + "norm1", q + a)
     f = _lin(sd, pre + "linear2", F.relu(_lin(sd, pre + "linear1", q)))
@@ -344,8 +364,11 @@ def encoder_layer(sd, pre, q, qp, value, ref_q, shapes, lsi, mask, cls, fg_q, he
 
 
 def encoder_forward(sd, feat, lpos, mask_flat, shapes, lsi, valid_ratios, filt, heads, points, topk_sa,
-                    num_layers, core="torch", use_c_helpers=False, trace=None):
-    """Restates SalienceTransformerEncoder.forward (salience_transformer.py:434-497)."""
+                    num_layers, core="torch", use_c_helpers=False, trace=None, pre_orders=None):
+    """Restates SalienceTransformerEncoder.forward (salience_transformer.py:434-497).
+
+    With ``core="torch"`` and ``use_c_helpers=False`` it is differentiable and runs in the dtype / on the device of ``feat``.
+    ``pre_orders``: optional list of per-layer (b,k) pre-attention top-k positions (see ``pre_attention``)."""
     shapes_list = shapes.tolist()
     L = len(shapes_list)
     b, nv, c = feat.shape
@@ -366,15 +389,17 @@ def encoder_forward(sd, feat, lpos, mask_flat, shapes, lsi, valid_ratios, filt, 
             rq = ref.view(b, nv, -1).gather(1, inds[..., None].expand(-1, -1, L * 2)).view(b, nq, L, 2)
         cls = _lin(sd, "encoder_class_head", q)
         q = encoder_layer(sd, f"encoder.layers.{j}.", q, qp, feat, rq, shapes, lsi, mask_flat, cls, fq, heads,
-                          L, points, topk_sa, core)
+                          L, points, topk_sa, core, None if pre_orders is None else pre_orders[j])
         if trace is not None:
             trace.append(q)
         if use_c_helpers:
             c_token_scatter(out, q, inds, focus)
-        else:
+        else:  # out of place: autograd keeps the gathers' inputs
+            rows = []
             for i in range(b):
                 n = min(int(focus[i]), nq)
-                out[i, inds[i, :n]] = q[i, :n]
+                rows.append(out[i].index_put((inds[i, :n],), q[i, :n]))
+            out = torch.stack(rows)
     row, col = sd["encoder.background_embedding.row_embed.weight"], sd["encoder.background_embedding.col_embed.weight"]
     if use_c_helpers:
         c_background_embed(out, mask_flat, inds, row, col, shapes, lsi)
@@ -390,19 +415,22 @@ def encoder_forward(sd, feat, lpos, mask_flat, shapes, lsi, valid_ratios, filt, 
     return out
 
 
-def encoder_half_forward(sd, feats, masks, pos_embeds, cfg: Dict, core="torch", use_c_helpers=False, trace=None):
+def encoder_half_forward(sd, feats, masks, pos_embeds, cfg: Dict, core="torch", use_c_helpers=False, trace=None,
+                         selection=None, pre_orders=None):
     """salience_transformer.py:106-183: (multi-level feats, masks, pos) -> encoder memory (b,Nv,C).
 
-    cfg: heads, points, topk_sa, num_layers, level_filter_ratio, layer_filter_ratio.
+    cfg: heads, points, topk_sa, num_layers, level_filter_ratio, layer_filter_ratio.  ``selection`` / ``pre_orders``: see
+    ``salience_filter`` / ``encoder_forward``.
     """
     feat = flatten_levels(feats)
     mask_flat = flatten_levels(masks)
     lpos = flatten_levels([p + l.view(1, -1, 1, 1) for p, l in zip(pos_embeds, sd["level_embeds"])])
     shapes, lsi, vr = level_misc(masks)
+    vr = vr.to(feat)
     filt = salience_filter(sd, feat, lpos, mask_flat, masks, shapes, lsi, cfg["level_filter_ratio"],
-                           cfg["layer_filter_ratio"])
+                           cfg["layer_filter_ratio"], selection)
     mem = encoder_forward(sd, feat, lpos, mask_flat, shapes, lsi, vr, filt, cfg["heads"], cfg["points"],
-                          cfg["topk_sa"], cfg["num_layers"], core, use_c_helpers, trace)
+                          cfg["topk_sa"], cfg["num_layers"], core, use_c_helpers, trace, pre_orders)
     return mem, filt
 
 

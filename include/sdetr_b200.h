@@ -480,6 +480,62 @@ int sdetr_group_norm_tokens(const float *x, float *y, int64_t pitch, int batch, 
 int sdetr_token_lpos_keep(const float *feat, const float *pos, const float *level_embeds, const float *keep,
                           const int32_t *level_size_host, int batch, int channels, int num_levels, float *lpos, float *x,
                           sdetr_stream_t stream);
+
+/* ---- Detection loss: HungarianMatcher + HybridSetCriterion.calculate_loss (models/matcher/hungarian_matcher.py:7-91,
+ * models/bricks/set_criterion.py:14-212, models/bricks/losses.py:15-21) ---------------------------------------------------
+ * One problem is one (output, image) pair.  Its descriptor names the output's rows in place: query q's K class logits at
+ * logits + q * logit_stride (classes contiguous) and its cxcywh box at boxes + q * box_stride (4 contiguous floats), so slices
+ * of a stacked (layers, b, Q, K) tensor need no copy.  gt_boxes (num_gt, 4) cxcywh and gt_labels (num_gt) int64 are
+ * contiguous; gt_labels NULL means every label is 0 (two_stage_binary_cls).  src / tgt (query, gt) index pairs are int64.
+ * The table (at most SDETR_SET_MAX_PROBLEMS problems) travels to the device as a kernel parameter: no copy, no sync. */
+#define SDETR_SET_MAX_PROBLEMS 128
+#define SDETR_SET_MAX_QUERIES 4096
+typedef struct sdetr_set_problem {
+    const float *logits;
+    const float *boxes;
+    const float *gt_boxes;
+    const int64_t *gt_labels;
+    int64_t *src;       /* sdetr_set_match: written, num_gt entries, ascending queries; loss: read, num_pairs entries */
+    int64_t *tgt;
+    float *grad_logits; /* sdetr_set_loss_backward: (Q, K) contiguous, fully written */
+    float *grad_boxes;  /* sdetr_set_loss_backward: (Q, 4) contiguous, fully written (0 on unmatched rows) */
+    int64_t logit_stride;
+    int64_t box_stride;
+    int32_t num_queries; /* Q >= 1 */
+    int32_t num_gt;
+    int32_t num_pairs;   /* loss only */
+    int32_t output;      /* loss only: row of the (num_outputs, 3) loss tensor this problem adds to */
+} sdetr_set_problem;
+/* Exact minimum-cost assignment of every problem's gts (rows) to its queries (columns), one CTA per problem, one launch:
+ * cost = cost_bbox * L1(pred, gt) + cost_class * focal(pos - neg at the gt label, +1e-6 inside the logs) - cost_giou * GIoU in
+ * fp32; shortest augmenting path with fp64 duals, ties to the lowest column.  Writes src (ascending query indices) / tgt of each
+ * problem (num_gt pairs; nothing when num_gt == 0) and status[i] = 0.  A non-finite cost, or a gt label outside
+ * [0, num_classes), sets status[i] = 1 and writes the pairs (k, k) instead (scipy / the reference's indexing raise there).  Q <= SDETR_SET_MAX_QUERIES and num_gt <= Q (else
+ * SDETR_ERR_UNSUPPORTED).  workspace: sdetr_set_match_workspace_floats(...) floats (the cost matrices). */
+int64_t sdetr_set_match_workspace_floats(const sdetr_set_problem *problems_host, int num_problems);
+int sdetr_set_match(const sdetr_set_problem *problems_host, int num_problems, int num_classes, float cost_class, float cost_bbox,
+                    float cost_giou, float alpha, float gamma, int32_t *status, float *workspace, int64_t workspace_floats,
+                    sdetr_stream_t stream);
+/* The solver of sdetr_set_match on given costs: problem i's (num_gt, num_queries) row-major fp32 matrix (rows gts, columns
+ * queries) starts at cost + sum over the earlier problems of num_gt * num_queries.  Only num_queries, num_gt, src and tgt of
+ * the descriptors are read.  Same outputs, status and limits as sdetr_set_match.  One launch. */
+int sdetr_set_assign(const sdetr_set_problem *problems_host, int num_problems, const float *cost, int64_t cost_floats,
+                     int32_t *status, sdetr_stream_t stream);
+/* loss[o] = (varifocal class loss, L1, sum of 1 - GIoU) of the matched pairs of every problem with output == o, divided by
+ * num_boxes (*num_boxes_dev when not NULL, else num_boxes_host).  Class target t = onehot * IoU(pair) and weight
+ * w = (1 - alpha) sigmoid(x)^gamma (1 - onehot) + t, both detached; the loss sums w * BCEwithlogits(x, t) over all Q x K logits.
+ * Sums run in a fixed order without float atomics (bit-reproducible).  A problem with status[i] != 0 (status may be NULL), a
+ * pair index out of range or a gt label outside [0, num_classes) makes its output's losses NaN.  Two launches; workspace: sdetr_set_loss_workspace_floats(...). */
+int64_t sdetr_set_loss_workspace_floats(const sdetr_set_problem *problems_host, int num_problems);
+int sdetr_set_loss_forward(const sdetr_set_problem *problems_host, int num_problems, int num_outputs, int num_classes, float alpha,
+                           float gamma, const int32_t *status, float num_boxes_host, const float *num_boxes_dev, float *workspace,
+                           int64_t workspace_floats, float *loss, sdetr_stream_t stream);
+/* Gradients of sum(grad_loss * loss) w.r.t. every problem's logits and boxes, into grad_logits / grad_boxes: w (sigmoid(x) - t)
+ * per logit; sign(pred - gt) (0 at 0) and the GIoU gradient with torch autograd's conventions (max / min ties split half and
+ * half, clamp(min=0) passes where its input is >= 0) per matched box.  grad_loss (num_outputs, 3) contiguous.  One launch. */
+int sdetr_set_loss_backward(const sdetr_set_problem *problems_host, int num_problems, int num_outputs, int num_classes, float alpha,
+                            float gamma, const int32_t *status, float num_boxes_host, const float *num_boxes_dev,
+                            const float *grad_loss, sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -20,6 +20,7 @@ from .ms_deform_attn import (  # noqa: F401
 from . import gemm  # noqa: F401
 from .position_encoding import PositionEmbeddingSine  # noqa: F401
 from .criterion import SalienceCriterion, load_reference_checkpoint, sigmoid_focal_loss  # noqa: F401
+from .set_criterion import HungarianMatcher, HybridSetCriterion  # noqa: F401
 from .decoder import (  # noqa: F401
     MLP,
     SalienceTransformerDecoder,

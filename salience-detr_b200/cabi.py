@@ -88,6 +88,12 @@ SIGNATURES = {
     "sdetr_group_norm_tokens_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
     "sdetr_group_norm_tokens": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _i, _f, _vp, _i64, _vp]),
     "sdetr_token_lpos_keep": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "sdetr_set_match_workspace_floats": (_i64, [_vp, _i]),
+    "sdetr_set_match": (_i, [_vp, _i, _i, _f, _f, _f, _f, _f, _vp, _vp, _i64, _vp]),
+    "sdetr_set_assign": (_i, [_vp, _i, _vp, _i64, _vp, _vp]),
+    "sdetr_set_loss_workspace_floats": (_i64, [_vp, _i]),
+    "sdetr_set_loss_forward": (_i, [_vp, _i, _i, _i, _f, _f, _vp, _f, _vp, _vp, _i64, _vp, _vp]),
+    "sdetr_set_loss_backward": (_i, [_vp, _i, _i, _i, _f, _f, _vp, _f, _vp, _vp, _vp]),
 }
 
 
@@ -964,3 +970,73 @@ def token_lpos_keep(feat, pos, level_embeds, keep, level_sizes: Sequence[int], l
                                      _stream())
     _check(rc, "sdetr_token_lpos_keep")
     return lpos, x
+
+
+# ---- detection loss (set_criterion.cu) ------------------------------------------------------------------------------------
+SET_MAX_PROBLEMS = 128  # include/sdetr_b200.h SDETR_SET_MAX_PROBLEMS
+SET_MAX_QUERIES = 4096  # SDETR_SET_MAX_QUERIES: the solver's shared-memory limit
+
+
+class SetProblem(ctypes.Structure):
+    """``sdetr_set_problem``: one (output, image) problem of the matcher / loss entry points."""
+    _fields_ = [("logits", _vp), ("boxes", _vp), ("gt_boxes", _vp), ("gt_labels", _vp), ("src", _vp), ("tgt", _vp),
+                ("grad_logits", _vp), ("grad_boxes", _vp), ("logit_stride", _i64), ("box_stride", _i64),
+                ("num_queries", ctypes.c_int32), ("num_gt", ctypes.c_int32), ("num_pairs", ctypes.c_int32),
+                ("output", ctypes.c_int32)]
+
+
+def _problem_table(problems):
+    if len(problems) > SET_MAX_PROBLEMS:
+        raise RuntimeError(f"{len(problems)} (output, image) problems in one call; at most {SET_MAX_PROBLEMS}")
+    return (SetProblem * max(len(problems), 1))(*problems)
+
+
+def _num_boxes_args(num_boxes):
+    """num_boxes: a Python number (host value) or a one-element float32 CUDA tensor (read by the kernels)."""
+    if torch.is_tensor(num_boxes):
+        if not (num_boxes.is_cuda and num_boxes.dtype == torch.float32 and num_boxes.numel() == 1):
+            raise RuntimeError("num_boxes must be a number or a one-element CUDA float32 tensor")
+        return 1.0, num_boxes.data_ptr()
+    return float(num_boxes), None
+
+
+def set_match(problems, num_classes: int, cost_class: float, cost_bbox: float, cost_giou: float, alpha: float, gamma: float,
+              status):
+    """Cost matrices + exact assignments of all ``problems`` (their src / tgt buffers are written) in one launch;
+    status (len(problems),) int32 receives 1 for a problem with a non-finite cost.  -> the workspace holding every problem's
+    (num_gt, num_queries) cost matrix, one after the other."""
+    tab = _problem_table(problems)
+    need = int(lib().sdetr_set_match_workspace_floats(tab, len(problems)))
+    ws = torch.empty(max(need, 1), device=status.device, dtype=torch.float32)
+    _check(lib().sdetr_set_match(tab, len(problems), int(num_classes), float(cost_class), float(cost_bbox), float(cost_giou),
+                                 float(alpha), float(gamma), _req(status, "status", torch.int32), ws.data_ptr(), ws.numel(),
+                                 _stream()), "sdetr_set_match")
+    return ws
+
+
+def set_assign(problems, cost, status):
+    """Exact assignments of given costs: ``cost`` holds every problem's (num_gt, num_queries) fp32 matrix, one after the other."""
+    tab = _problem_table(problems)
+    _check(lib().sdetr_set_assign(tab, len(problems), _req(cost, "cost", torch.float32), cost.numel(),
+                                  _req(status, "status", torch.int32), _stream()), "sdetr_set_assign")
+
+
+def set_loss_forward(problems, num_outputs: int, num_classes: int, alpha: float, gamma: float, status, num_boxes, loss):
+    """Writes loss (num_outputs, 3) float32, contiguous: (loss_class, loss_bbox, loss_giou) per output."""
+    tab = _problem_table(problems)
+    need = int(lib().sdetr_set_loss_workspace_floats(tab, len(problems)))
+    ws = torch.empty(max(need, 1), device=loss.device, dtype=torch.float32)
+    nb_host, nb_dev = _num_boxes_args(num_boxes)
+    _check(lib().sdetr_set_loss_forward(tab, len(problems), int(num_outputs), int(num_classes), float(alpha), float(gamma),
+                                        status.data_ptr() if status is not None else None, nb_host, nb_dev, ws.data_ptr(),
+                                        ws.numel(), _req(loss, "loss", torch.float32), _stream()), "sdetr_set_loss_forward")
+    return loss
+
+
+def set_loss_backward(problems, num_outputs: int, num_classes: int, alpha: float, gamma: float, status, num_boxes, grad_loss):
+    """Writes every problem's grad_logits / grad_boxes for the (num_outputs, 3) upstream gradient ``grad_loss``."""
+    tab = _problem_table(problems)
+    nb_host, nb_dev = _num_boxes_args(num_boxes)
+    _check(lib().sdetr_set_loss_backward(tab, len(problems), int(num_outputs), int(num_classes), float(alpha), float(gamma),
+                                         status.data_ptr() if status is not None else None, nb_host, nb_dev,
+                                         _req(grad_loss, "grad_loss", torch.float32), _stream()), "sdetr_set_loss_backward")

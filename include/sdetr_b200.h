@@ -536,6 +536,47 @@ int sdetr_set_loss_forward(const sdetr_set_problem *problems_host, int num_probl
 int sdetr_set_loss_backward(const sdetr_set_problem *problems_host, int num_problems, int num_outputs, int num_classes, float alpha,
                             float gamma, const int32_t *status, float num_boxes_host, const float *num_boxes_dev,
                             const float *grad_loss, sdetr_stream_t stream);
+
+/* ---- Contrastive denoising queries: GenerateCDNQueries.forward after its random draws (models/bricks/denoising.py:178-329,
+ * generate_query_masks :64-76) and the denoising-loss indices of DNDETRDetector.compute_dn_loss
+ * (models/detectors/base_detector.py:205-218) ---------------------------------------------------------------------------------
+ * Image i has num_gt gts: gt_labels (num_gt) int64 and gt_boxes (num_gt, 4) cxcywh fp32, both contiguous.  The table (at most
+ * SDETR_CDN_MAX_IMAGES images) travels to the device as a kernel parameter: no copy, no sync. */
+#define SDETR_CDN_MAX_IMAGES 128
+typedef struct sdetr_cdn_image {
+    const int64_t *gt_labels;
+    const float *gt_boxes;
+    int32_t num_gt;
+    int32_t reserved;
+} sdetr_cdn_image;
+/* With m = max_gt (the largest num_gt), G = groups, S = the sum of the num_gt and D = 2 G m, the reference's draws over its
+ * repeated gt list of n = 2 G S entries (entry r S + (gts of the images before i) + t is copy r < 2G of image i's gt t):
+ *   label_rand (n) fp32 and label_randint (n) int64: the label draws, both NULL when label_noise_prob * 0.5 == 0;
+ *   box_randint (n, 4) fp32 in {0, 1} and box_rand (n, 4) fp32: the box draws, both NULL when box_noise_scale == 0.
+ * Copy r of gt t lands in slot r m + t of its image; copy 2g is the positive and 2g + 1 the negative of group g.  Writes
+ *   label_queries (b, D, C) = label_encoder.weight row of the noised label where(label_rand < label_threshold, label_randint,
+ *     label), NaN where that label is outside [0, num_classes) (an IndexError in the reference), zeros in padding slots;
+ *   box_queries (b, D, 4) = inverse_sigmoid of the noised box (diff = wh / 2 for both corners, sign = randint * 2 - 1, +1 on
+ *     the negative copies, xyxy + (part * diff) * box_noise_scale, clamp(0, 1), back to cxcywh), zeros in padding slots;
+ *     every operation rounded separately, as the reference's chain of torch kernels;
+ *   noised_labels (b, D) int32: the label of each slot, -1 in padding slots and where the label is out of range;
+ *   attn_mask (T, T) bytes (torch.bool), T = D + num_queries: generate_query_masks(2m);
+ *   status (b) int32: 1 where one of the image's noised labels is outside [0, num_classes), else 0.
+ * weight_rows / weight_cols: the shape of `weight` (label_encoder.weight), must be (num_classes, embed_dim).  One launch. */
+int sdetr_cdn_queries(const sdetr_cdn_image *images_host, int num_images, const float *label_rand, const int64_t *label_randint,
+                      const float *box_randint, const float *box_rand, float label_threshold, float box_noise_scale,
+                      const float *weight, int num_classes, int embed_dim, int weight_rows, int weight_cols, int num_queries,
+                      int groups, int max_gt, float *label_queries, float *box_queries, int32_t *noised_labels, uint8_t *attn_mask,
+                      int32_t *status, sdetr_stream_t stream);
+/* grad_weight (num_classes, embed_dim), fully written: row k = the sum over the slots s < num_slots with noised_labels[s] == k,
+ * in ascending s, of grad_label_queries[s, :] ((num_slots, embed_dim) contiguous).  No atomics: bit-reproducible.  One launch. */
+int sdetr_cdn_queries_backward(const float *grad_label_queries, const int32_t *noised_labels, int64_t num_slots, int num_classes,
+                               int embed_dim, float *grad_weight, sdetr_stream_t stream);
+/* indices (2, P) int64, P = groups * sum of num_gt_host: image after image, the pairs (g * max_gt + t, t) for g < groups,
+ * t < num_gt_host[i] (g outer): row 0 the query, row 1 the gt.  max_gt: the reference's max_gt_num_per_image (2 m for CDN).
+ * One launch (none when P == 0). */
+int sdetr_cdn_loss_indices(const int32_t *num_gt_host, int num_images, int groups, int max_gt, int64_t *indices,
+                           sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -94,6 +94,9 @@ SIGNATURES = {
     "sdetr_set_loss_workspace_floats": (_i64, [_vp, _i]),
     "sdetr_set_loss_forward": (_i, [_vp, _i, _i, _i, _f, _f, _vp, _f, _vp, _vp, _i64, _vp, _vp]),
     "sdetr_set_loss_backward": (_i, [_vp, _i, _i, _i, _f, _f, _vp, _f, _vp, _vp, _vp]),
+    "sdetr_cdn_queries": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp] + [_i] * 7 + [_vp] * 6),
+    "sdetr_cdn_queries_backward": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
+    "sdetr_cdn_loss_indices": (_i, [_vp, _i, _i, _i, _vp, _vp]),
 }
 
 
@@ -1040,3 +1043,65 @@ def set_loss_backward(problems, num_outputs: int, num_classes: int, alpha: float
     _check(lib().sdetr_set_loss_backward(tab, len(problems), int(num_outputs), int(num_classes), float(alpha), float(gamma),
                                          status.data_ptr() if status is not None else None, nb_host, nb_dev,
                                          _req(grad_loss, "grad_loss", torch.float32), _stream()), "sdetr_set_loss_backward")
+
+
+# ---- contrastive denoising queries (denoising.cu) -----------------------------------------------------------------------------
+CDN_MAX_IMAGES = 128  # include/sdetr_b200.h SDETR_CDN_MAX_IMAGES
+
+
+class CDNImage(ctypes.Structure):
+    """``sdetr_cdn_image``: one image's gts for the denoising-query entry points."""
+    _fields_ = [("gt_labels", _vp), ("gt_boxes", _vp), ("num_gt", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
+def _opt(t, name, dtype):
+    return _req(t, name, dtype) if t is not None else None
+
+
+def cdn_queries(labels, boxes, draws, weight, num_classes: int, embed_dim: int, label_threshold: float, box_noise_scale: float,
+                num_queries: int, groups: int, max_gt: int):
+    """labels / boxes: per-image int64 (n_i,) / float32 (n_i, 4) contiguous CUDA tensors; draws: (label_rand, label_randint,
+    box_randint, box_rand), None where that noise is off.  -> (label_queries (b, D, C), box_queries (b, D, 4), noised_labels
+    (b, D) int32, attn_mask (T, T) bool, status (b,) int32) with D = 2 * groups * max_gt, T = D + num_queries."""
+    b = len(labels)
+    if b > CDN_MAX_IMAGES:
+        raise RuntimeError(f"{b} images in one call; at most {CDN_MAX_IMAGES}")
+    K, C = int(num_classes), int(embed_dim)
+    dev = weight.device
+    D = 2 * groups * max_gt
+    ims = (CDNImage * max(b, 1))(*[CDNImage(gt_labels=_req(lb, "gt_labels", torch.int64) if lb.numel() else None,
+                                            gt_boxes=_req(bx, "gt_boxes", torch.float32) if lb.numel() else None,
+                                            num_gt=lb.numel()) for lb, bx in zip(labels, boxes)])
+    label_q = torch.empty(b, D, C, device=dev, dtype=torch.float32)
+    box_q = torch.empty(b, D, 4, device=dev, dtype=torch.float32)
+    noised = torch.empty(b, D, device=dev, dtype=torch.int32)
+    mask = torch.empty(D + num_queries, D + num_queries, device=dev, dtype=torch.bool)
+    status = torch.empty(b, device=dev, dtype=torch.int32)
+    lr, li, bs, br = draws
+    _check(lib().sdetr_cdn_queries(ims, b, _opt(lr, "label_rand", torch.float32), _opt(li, "label_randint", torch.int64),
+                                   _opt(bs, "box_randint", torch.float32), _opt(br, "box_rand", torch.float32),
+                                   float(label_threshold), float(box_noise_scale), _req(weight, "weight", torch.float32), K, C,
+                                   *[int(x) for x in weight.shape],
+                                   int(num_queries), int(groups), int(max_gt), label_q.data_ptr(), box_q.data_ptr(),
+                                   noised.data_ptr(), mask.data_ptr(), status.data_ptr(), _stream()), "sdetr_cdn_queries")
+    return label_q, box_q, noised, mask, status
+
+
+def cdn_queries_backward(grad_label_queries, noised_labels, num_classes: int):
+    """(b, D, C) gradient of the label queries + the forward's noised labels -> grad of label_encoder.weight (K, C)."""
+    C = grad_label_queries.shape[-1]
+    gw = torch.empty(num_classes, C, device=grad_label_queries.device, dtype=torch.float32)
+    _check(lib().sdetr_cdn_queries_backward(_req(grad_label_queries, "grad_label_queries", torch.float32),
+                                            _req(noised_labels, "noised_labels", torch.int32), noised_labels.numel(),
+                                            int(num_classes), C, gw.data_ptr(), _stream()), "sdetr_cdn_queries_backward")
+    return gw
+
+
+def cdn_loss_indices(counts: Sequence[int], groups: int, max_gt: int, device):
+    """-> (2, groups * sum(counts)) int64: per image the (g * max_gt + t, t) pairs of compute_dn_loss, image after image."""
+    if len(counts) > CDN_MAX_IMAGES:
+        raise RuntimeError(f"{len(counts)} images in one call; at most {CDN_MAX_IMAGES}")
+    out = torch.empty(2, groups * sum(counts), device=device, dtype=torch.int64)
+    _check(lib().sdetr_cdn_loss_indices(_host_i32(counts) if counts else None, len(counts), int(groups), int(max_gt),
+                                        out.data_ptr() if out.numel() else None, _stream()), "sdetr_cdn_loss_indices")
+    return out

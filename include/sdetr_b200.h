@@ -459,6 +459,40 @@ int sdetr_context_gate(const float *y, int64_t y_pitch, int64_t ldy, const float
 int sdetr_upsample_nearest_concat(const float *hi, int64_t hi_pitch, int64_t ldh, int Hi, int Wi, const float *lo, int64_t lo_pitch,
                                   int64_t ldl, int Ho, int Wo, int batch, int C, float *dst, int64_t dst_pitch, int64_t ldd,
                                   sdetr_stream_t stream);
+/* Training (RepVGGPluXNetwork.forward_tokens under autograd).  The input gradient of a stride-1 convolution is
+ * sdetr_conv2d_f16x3 on dY with the weights flipped in both spatial axes and transposed per group: (Cin, k, k, Cout / groups),
+ * W'[g Cin_g + ci, ky, kx, co] = W[g Cout_g + co, ci, k - 1 - ky, k - 1 - kx].  The stride-2 one is this transposed
+ * convolution with the same W': dY (Hy x Wy, Cin channels = the forward's Cout) -> dX (H x W, Cout channels = the forward's
+ * Cin); output pixel (iy, ix) with tap (ky, kx) reads dY[(iy - pad + ky) / 2, (ix - pad + kx) / 2] when both are even and in
+ * range, zero otherwise.  Hy, Wy must be the forward's output size of H, W.  Same operand rules as sdetr_conv2d_f16x3; no bias,
+ * no activation. */
+/* One pass over a convolution weight w (Cout, Cin / groups, k, k) in PyTorch's layout with the device scale *scale_dev
+ * (sdetr_pow2_scale, target 14): the fp16 pair (fwd_hi, fwd_lo) in sdetr_conv2d_f16x3's (Cout, k, k, Cin / groups) layout and,
+ * unless dgrad_hi == dgrad_lo == NULL, the pair of the input-gradient weights W' (Cin, k, k, Cout / groups) described below.
+ * The arithmetic of sdetr_split_f16_pair_dev. */
+int sdetr_conv2d_f16x3_split_weight(const float *w, int Cout, int Cin, int groups, int ksize, const float *scale_dev, void *fwd_hi,
+                                    void *fwd_lo, void *dgrad_hi, void *dgrad_lo, sdetr_stream_t stream);
+int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
+                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev, int Cout,
+                                  int groups, int ksize, int H, int W, float *dx, int64_t dx_pitch, int64_t lddx,
+                                  sdetr_stream_t stream);
+/* Weight gradient of y = conv(x, W) (the family of sdetr_conv2d_f16x3; x: H x W, Cin channels; dy: Ho x Wo, Cout channels):
+ * dw[co, ci, ky, kx] = sum over output pixels of dy[pixel, co] x[shifted pixel, g Cin_g + ci], written fp32 in PyTorch's
+ * (Cout, Cin / groups, k, k) layout.  3xFP16 on wgmma: dy and x are multiplied by their power-of-two device scalars
+ * (sdetr_pow2_scale, target 12) before the hi / lo split.  The pixel range is split over CTAs by a rule of the shape alone and
+ * the partial sums are added in split order: bit-reproducible.  Two launches.  dy, x, their pitches and row strides 16-byte
+ * aligned; workspace: sdetr_conv2d_f16x3_wgrad_workspace_floats(batch, Ho, Wo, Cin, Cout, groups, ksize) floats, 16-byte
+ * aligned (0 for an unsupported shape). */
+int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, int Wo, int Cin, int Cout, int groups, int ksize);
+int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
+                             int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin, int Cout,
+                             int groups, int ksize, int stride, float *workspace, int64_t workspace_floats, float *dw,
+                             sdetr_stream_t stream);
+/* Gradient of the hi half of sdetr_upsample_nearest_concat: d_hi (Hi x Wi) = for each source pixel, the sum of g[:, :, 0:C] over
+ * the destination pixels (Ho x Wo) that read it, rows then columns in order (no atomics: deterministic).  The lo half's gradient
+ * is g[:, :, C:2C] itself.  C % 4 == 0; all row operands 16-byte aligned. */
+int sdetr_upsample_nearest_concat_backward(const float *g, int64_t g_pitch, int64_t ldg, int Ho, int Wo, int Hi, int Wi, int batch,
+                                           int C, float *d_hi, int64_t d_pitch, int64_t ldd, sdetr_stream_t stream);
 
 /* ---- ChannelMapper in token layout (models/necks/channel_mapper.py:8-80; ChannelMapper.forward_tokens) ----------------------
  * GroupNorm of every level of a token buffer (nn.GroupNorm per level, models/bricks/misc.py:97-98): image n, token t, channel c

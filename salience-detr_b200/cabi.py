@@ -85,6 +85,12 @@ SIGNATURES = {
     "sdetr_context_gate": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp,
                                 _i64, _i64, _vp]),
     "sdetr_upsample_nearest_concat": (_i, [_vp, _i64, _i64, _i, _i, _vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
+    "sdetr_conv2d_f16x3_split_weight": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sdetr_conv2d_f16x3_transposed": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i64, _i64,
+                                           _vp]),
+    "sdetr_conv2d_f16x3_wgrad_workspace_floats": (_i64, [_i] * 7),
+    "sdetr_conv2d_f16x3_wgrad": (_i, [_vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp] + [_i] * 8 + [_vp, _i64, _vp, _vp]),
+    "sdetr_upsample_nearest_concat_backward": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
     "sdetr_group_norm_tokens_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
     "sdetr_group_norm_tokens": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _i, _f, _vp, _i64, _vp]),
     "sdetr_token_lpos_keep": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -935,6 +941,72 @@ def upsample_nearest_concat(hi, hi_hw, lo, lo_hw, out=None):
     rc = lib().sdetr_upsample_nearest_concat(*_token_rows(hi, "hi"), int(hi_hw[0]), int(hi_hw[1]), *_token_rows(lo, "lo"), int(ho),
                                              int(wo), b, c, *_token_rows(out, "out"), _stream())
     _check(rc, "sdetr_upsample_nearest_concat")
+    return out
+
+
+def conv2d_f16x3_split_weight(w, groups: int, dgrad: bool = True):
+    """(fwd_hi, fwd_lo, dgrad_hi, dgrad_lo, scale) of a (Cout, Cin / groups, k, k) fp32 weight in one pass: the pair for
+    conv2d_f16x3 (Cout, k, k, Cin / groups) and, with ``dgrad``, the pair of the flipped, per-group transposed input-gradient
+    weights (Cin, k, k, Cout / groups) (else None, None); scale: the power-of-two device scale of both (target 14)."""
+    cout, cin_g, k, _ = w.shape
+    scale = pow2_scale(w, 14)
+    f_hi = torch.empty(cout, k, k, cin_g, device=w.device, dtype=torch.float16)
+    f_lo = torch.empty_like(f_hi)
+    d_hi = torch.empty(cin_g * groups, k, k, cout // groups, device=w.device, dtype=torch.float16) if dgrad else None
+    d_lo = torch.empty_like(d_hi) if dgrad else None
+    rc = lib().sdetr_conv2d_f16x3_split_weight(_req(w, "w", torch.float32), cout, cin_g * groups, int(groups), k, scale.data_ptr(),
+                                               f_hi.data_ptr(), f_lo.data_ptr(), d_hi.data_ptr() if dgrad else None,
+                                               d_lo.data_ptr() if dgrad else None, _stream())
+    _check(rc, "sdetr_conv2d_f16x3_split_weight")
+    return f_hi, f_lo, d_hi, d_lo, scale
+
+
+def conv2d_f16x3_transposed(dy, dy_hw, a_scale, w_hi, w_lo, w_scale, groups: int, ksize: int, hw):
+    """Input gradient of a stride-2 convolution of an (H, W) = hw map: dy (b, Hy*Wy, Cout) view, W' = the (Cin, k, k, Cout / groups)
+    flipped, per-group transposed weights as a split_f16_pair_dev pair; a_scale: pow2_scale of dy (target 12).  -> (b, H*W, Cin)."""
+    b, n, cin = dy.shape
+    if n != dy_hw[0] * dy_hw[1]:
+        raise RuntimeError(f"conv2d_f16x3_transposed: dy has {n} rows per image, the map is {dy_hw[0]}x{dy_hw[1]}")
+    cout = w_hi.shape[0]
+    dx = torch.empty(b, hw[0] * hw[1], cout, device=dy.device, dtype=torch.float32)
+    rc = lib().sdetr_conv2d_f16x3_transposed(*_token_rows(dy, "dy")[:3], b, int(dy_hw[0]), int(dy_hw[1]), cin,
+                                             _req(a_scale, "a_scale", torch.float32), _req(w_hi, "w_hi", torch.float16),
+                                             _req(w_lo, "w_lo", torch.float16), _req(w_scale, "w_scale", torch.float32), cout,
+                                             int(groups), int(ksize), int(hw[0]), int(hw[1]), *_token_rows(dx, "dx"), _stream())
+    _check(rc, "sdetr_conv2d_f16x3_transposed")
+    return dx
+
+
+def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int):
+    """Weight gradient (Cout, Cin / groups, k, k) of y = conv(x, W): dy (b, Ho*Wo, Cout), x (b, H*W, Cin) views with unit channel
+    stride, hw = (H, W); dy_scale / x_scale: their pow2_scale device scalars (target 12).  Bit-reproducible."""
+    b, _, cin = x.shape
+    cout, cin_g, k, _ = (int(v) for v in weight_shape)
+    groups = cin // cin_g
+    pad = k // 2
+    ho, wo = (hw[0] + 2 * pad - k) // stride + 1, (hw[1] + 2 * pad - k) // stride + 1
+    if tuple(dy.shape) != (b, ho * wo, cout) or x.shape[1] != hw[0] * hw[1]:
+        raise RuntimeError("conv2d_f16x3_wgrad: dy, x and the map size do not match")
+    dw = torch.empty(cout, cin_g, k, k, device=x.device, dtype=torch.float32)
+    ws = torch.empty(max(int(lib().sdetr_conv2d_f16x3_wgrad_workspace_floats(b, ho, wo, cin, cout, groups, k)), 4), device=x.device,
+                     dtype=torch.float32)
+    rc = lib().sdetr_conv2d_f16x3_wgrad(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
+                                        _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
+                                        int(stride), ws.data_ptr(), ws.numel(), dw.data_ptr(), _stream())
+    _check(rc, "sdetr_conv2d_f16x3_wgrad")
+    return dw
+
+
+def upsample_nearest_concat_backward(g_hi, lo_hw, hi_hw):
+    """Gradient of hi in upsample_nearest_concat: g_hi (b, Ho*Wo, C) view (the first C channels of the concatenation's
+    gradient) -> (b, Hi*Wi, C), each source pixel the fixed-order sum over the destination pixels that read it."""
+    b, n, c = g_hi.shape
+    if n != lo_hw[0] * lo_hw[1]:
+        raise RuntimeError("upsample_nearest_concat_backward: shapes do not match")
+    out = torch.empty(b, hi_hw[0] * hi_hw[1], c, device=g_hi.device, dtype=torch.float32)
+    rc = lib().sdetr_upsample_nearest_concat_backward(*_token_rows(g_hi, "g"), int(lo_hw[0]), int(lo_hw[1]), int(hi_hw[0]),
+                                                      int(hi_hw[1]), b, c, *_token_rows(out, "out"), _stream())
+    _check(rc, "sdetr_upsample_nearest_concat_backward")
     return out
 
 

@@ -49,6 +49,10 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 __device__ __forceinline__ float silu(float x) { return x / (1.f + expf(-x)); }
 
+// TRANSPOSED: the input gradient of a stride-2 convolution.  x is dY (H x W), y is dX (Ho x Wo), W the flipped, per-group
+// transposed weights (see sdetr_conv2d_f16x3_transposed); output pixel (oy, ox) with tap (ky, kx) reads x[(oy - pad + ky) / 2,
+// (ox - pad + kx) / 2] when both are even and in range, and zero otherwise.
+template <bool TRANSPOSED>
 __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -68,7 +72,7 @@ __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams
         if (m < p.M) {
             const int n = m / hwo, pix = m - n * hwo, oy = pix / p.Wo, ox = pix - oy * p.Wo;
             arow[j] = p.x + (int64_t)n * p.x_pitch + cin0 + ac * 4;
-            iy0[j] = oy * p.stride - pad, ix0[j] = ox * p.stride - pad;
+            iy0[j] = oy * (TRANSPOSED ? 1 : p.stride) - pad, ix0[j] = ox * (TRANSPOSED ? 1 : p.stride) - pad;
         }
     }
     auto load_stage = [&](int s, int kb) {
@@ -76,8 +80,15 @@ __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams
         const int t = kb / cblocks, cb = kb - t * cblocks, ky = t / p.ksize, kx = t - ky * p.ksize;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            const int r = (tid >> 4) + 8 * j, iy = iy0[j] + ky, ix = ix0[j] + kx;
-            const bool ok = (unsigned)iy < (unsigned)p.H && (unsigned)ix < (unsigned)p.W;
+            const int r = (tid >> 4) + 8 * j;
+            int iy = iy0[j] + ky, ix = ix0[j] + kx;
+            bool ok;
+            if (TRANSPOSED) {
+                ok = ((iy | ix) & 1) == 0 && (unsigned)iy < 2u * p.H && (unsigned)ix < 2u * p.W;
+                iy >>= 1, ix >>= 1;
+            } else {
+                ok = (unsigned)iy < (unsigned)p.H && (unsigned)ix < (unsigned)p.W;
+            }
             const float *src = ok ? arow[j] + ((int64_t)iy * p.W + ix) * p.ldx + cb * kCvK : p.x;
             cp_async16(st + r * 256 + ((ac ^ (r & 7)) << 4), src, ok);
         }
@@ -281,6 +292,211 @@ __global__ void upsample_concat_kernel(Rows hi, int Hi, int Wi, Rows lo, int Ho,
     }
 }
 
+// gradient of the hi half: each source pixel sums its destination range [first_dst(s), first_dst(s + 1)) per axis, rows then
+// columns in order (no atomics).  first_dst(s): the first destination whose nearest_src is >= s (nearest_src is monotonic).
+__device__ __forceinline__ int first_dst(int s, int in, int out) {
+    int lo = 0, hi = out;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (nearest_src(mid, in, out) >= s) hi = mid; else lo = mid + 1;
+    }
+    return lo;
+}
+
+__global__ void upsample_concat_backward_kernel(Rows g, int Ho, int Wo, int Hi, int Wi, int batch, int C, float *dst,
+                                                int64_t d_pitch, int64_t ldd) {
+    const int c4 = C >> 2, hwi = Hi * Wi;
+    const int64_t total = (int64_t)batch * hwi * c4;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % c4) * 4;
+        const int64_t r = i / c4;
+        const int n = (int)(r / hwi), pix = (int)(r - (int64_t)n * hwi), sy = pix / Wi, sx = pix - sy * Wi;
+        const int y0 = first_dst(sy, Hi, Ho), y1 = first_dst(sy + 1, Hi, Ho);
+        const int x0 = first_dst(sx, Wi, Wo), x1 = first_dst(sx + 1, Wi, Wo);
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int oy = y0; oy < y1; ++oy)
+            for (int ox = x0; ox < x1; ++ox) {
+                const float4 v = g.at(n, oy * Wo + ox, c);
+                s.x += v.x, s.y += v.y, s.z += v.z, s.w += v.w;
+            }
+        *reinterpret_cast<float4 *>(dst + (int64_t)n * d_pitch + (int64_t)pix * ldd + c) = s;
+    }
+}
+
+// ---- convolution weight gradient ---------------------------------------------------------------------------------------
+// dW[co, ci, ky, kx] = sum over output pixels m of dY[m, co] . X[shift(m, ky, kx), ci], per group.  One CTA (one warpgroup) per
+// 64 (co) x 64 (ci) tile of one tap and one split of the pixel range: a GEMM with M = co, N = ci, K = pixels.  Per 64-pixel
+// k-block the CTA copies the dY and X rows (fp32, cp.async, X zero-filled outside the map) into a 3-stage ring; dY^T is the
+// register A operand (split in registers, like the forward's activation); X is split into fp16 hi / lo and written TRANSPOSED
+// (pixel-contiguous, 128-byte swizzle) into one shared W_hi / W_lo-shaped pair, so wgmma reads it K-major.  Each split writes
+// its partial tile to the workspace; a second launch sums the splits in split order (bit-reproducible, no atomics) into the
+// (Cout, Cin / groups, k, k) layout.
+constexpr int kWgStageBytes = 2 * kCvABytes;
+constexpr int kWgSmem = kCvStages * kWgStageBytes + 2 * kCvBBytes + 1024 /* alignment */;
+constexpr int kWgTargetCtas = 512;  // splits = ceil(512 / tiles) at most: a function of the shape alone, so the bits are too
+
+struct WgradParams {
+    const float *dy;
+    int64_t dy_pitch, lddy;
+    const float *x;
+    int64_t x_pitch, ldx;
+    const float *dy_scale, *x_scale;
+    float *part;  // (splits, Cout, cin_g, k, k)
+    int H, W, Ho, Wo, M, Cout, cin_g, cout_g, ksize, stride, kb_per_split;
+};
+
+__global__ void __launch_bounds__(kCvThreads) conv_wgrad_f16x3_kernel(const WgradParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *bhi = smem + kCvStages * kWgStageBytes, *blo = bhi + kCvBBytes;
+    const int tid = threadIdx.x, taps = p.ksize * p.ksize, ci_tiles = p.cin_g / kCvN;
+    const int tap = blockIdx.x % taps, cit = (blockIdx.x / taps) % ci_tiles, cot = blockIdx.x / (taps * ci_tiles);
+    const int co0 = cot * kCvM, ci0 = cit * kCvN, xc0 = (co0 / p.cout_g) * p.cin_g + ci0;
+    const int ky = tap / p.ksize, kx = tap - ky * p.ksize, pad = p.ksize >> 1, hwo = p.Ho * p.Wo;
+    const int kb0 = blockIdx.y * p.kb_per_split, kb1 = min(kb0 + p.kb_per_split, (p.M + kCvK - 1) / kCvK), kblocks = kb1 - kb0;
+    const int ac = tid & 15;
+
+    auto load_stage = [&](int s, int kb) {
+        uint8_t *st = smem + s * kWgStageBytes;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int r = (tid >> 4) + 8 * j, m = kb * kCvK + r;
+            bool okd = false, okx = false;
+            const float *sd = p.dy, *sx = p.x;
+            if (m < p.M) {
+                const int n = m / hwo, pix = m - n * hwo, oy = pix / p.Wo, ox = pix - oy * p.Wo;
+                const int iy = oy * p.stride - pad + ky, ix = ox * p.stride - pad + kx;
+                okd = true, sd = p.dy + (int64_t)n * p.dy_pitch + (int64_t)pix * p.lddy + co0 + ac * 4;
+                okx = (unsigned)iy < (unsigned)p.H && (unsigned)ix < (unsigned)p.W;
+                if (okx) sx = p.x + (int64_t)n * p.x_pitch + ((int64_t)iy * p.W + ix) * p.ldx + xc0 + ac * 4;
+            }
+            const int off = r * 256 + ((ac ^ (r & 7)) << 4);
+            cp_async16(st + off, sd, okd);
+            cp_async16(st + kCvABytes + off, sx, okx);
+        }
+    };
+
+    const float ds = __ldg(p.dy_scale), xs = __ldg(p.x_scale), out_scale = 1.f / (ds * xs);
+    const int warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3, r0 = warp * 16 + g;
+    float d[32], acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int s = 0; s < kCvStages - 1; ++s) {
+        if (s < kblocks) load_stage(s, kb0 + s);
+        cp_async_commit();
+    }
+    for (int kb = 0; kb < kblocks; ++kb) {
+        cp_async_wait_1();
+        __syncthreads();  // the stage has landed; every warp is done with W_hi / W_lo and the stage the next copy overwrites
+        if (kb + kCvStages - 1 < kblocks) load_stage((kb + kCvStages - 1) % kCvStages, kb0 + kb + kCvStages - 1);
+        cp_async_commit();
+        const uint8_t *st = smem + (kb % kCvStages) * kWgStageBytes, *sx = st + kCvABytes;
+        // X (pixel, ci) -> hi / lo (ci, pixel): thread = channel tid & 63, 8-pixel chunks (tid >> 6) + 2 jj
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int ci = tid & 63, ch = (tid >> 6) + 2 * jj;
+            uint32_t h[4], l[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int p0 = ch * 8 + 2 * e, p1 = p0 + 1;
+                const float v0 = *reinterpret_cast<const float *>(sx + p0 * 256 + ((((ci >> 2) ^ (p0 & 7)) << 4) | ((ci & 3) << 2)));
+                const float v1 = *reinterpret_cast<const float *>(sx + p1 * 256 + ((((ci >> 2) ^ (p1 & 7)) << 4) | ((ci & 3) << 2)));
+                split2(v0 * xs, v1 * xs, h[e], l[e]);
+            }
+            const int off = ci * 128 + ((ch ^ (ci & 7)) << 4);
+            *reinterpret_cast<uint4 *>(bhi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+            *reinterpret_cast<uint4 *>(blo + off) = make_uint4(l[0], l[1], l[2], l[3]);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> wgmma operand reads
+        __syncthreads();
+        uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {  // A = dY^T: row = output channel, column = pixel
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int co = r0 + (j & 1) * 8, px = kk * 16 + 2 * q + (j >> 1) * 8;
+                const float v0 = *reinterpret_cast<const float *>(st + px * 256 + ((((co >> 2) ^ (px & 7)) << 4) | ((co & 3) << 2)));
+                const float v1 =
+                    *reinterpret_cast<const float *>(st + (px + 1) * 256 + ((((co >> 2) ^ ((px + 1) & 7)) << 4) | ((co & 3) << 2)));
+                split2(v0 * ds, v1 * ds, ahi[kk][j], alo[kk][j]);
+            }
+        }
+        wgmma_fence();
+        const uint32_t bh = smem_u32(bhi), bl = smem_u32(blo);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            wgmma_f16_rs_n64(d, alo[kk], wgmma_desc(bh + kk * 32), kk);
+            wgmma_f16_rs_n64(d, ahi[kk], wgmma_desc(bl + kk * 32), 1);
+            wgmma_f16_rs_n64(d, ahi[kk], wgmma_desc(bh + kk * 32), 1);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[i] += d[i];
+    }
+    // acc[4j + 2h + e] = (output channel co0 + r0 + 8h, input channel ci0 + 8j + 2q + e)
+    float *part = p.part + (int64_t)blockIdx.y * p.Cout * p.cin_g * taps;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int64_t row = (int64_t)(co0 + r0 + 8 * h) * p.cin_g;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) part[(row + ci0 + 8 * j + 2 * q + e) * taps + tap] = acc[4 * j + 2 * h + e] * out_scale;
+    }
+}
+
+__global__ void wgrad_reduce_kernel(const float *__restrict__ part, int splits, int64_t n, float *__restrict__ dw) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float s = 0.f;
+        for (int k = 0; k < splits; ++k) s += part[(int64_t)k * n + i];
+        dw[i] = s;
+    }
+}
+
+// split of the pixel range: (splits, k-blocks per split), from the shape alone
+inline void wgrad_splits(int64_t M, int tiles, int &splits, int &per) {
+    const int kblocks = (int)((M + kCvK - 1) / kCvK);
+    if (kblocks == 0) {
+        splits = 0, per = 1;
+        return;
+    }
+    int want = (kWgTargetCtas + tiles - 1) / tiles;
+    want = want < 1 ? 1 : (want > kblocks ? kblocks : want);
+    per = (kblocks + want - 1) / want;
+    splits = (kblocks + per - 1) / per;
+}
+
+// the channel / kernel shapes sdetr_conv2d_f16x3_wgrad takes (its workspace size function answers 0 for the others)
+inline bool wgrad_shape_ok(int Cin, int Cout, int groups, int ksize) {
+    return Cin > 0 && Cout > 0 && groups > 0 && Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kCvK == 0 &&
+           (Cout / groups) % kCvN == 0 && (ksize == 1 || ksize == 3);
+}
+
+// one pass over a (Cout, Cin / groups, k, k) weight: the fp16 pair of the forward layout (Cout, k, k, Cin / groups) and, when
+// asked, of the input-gradient layout (Cin, k, k, Cout / groups) flipped in both spatial axes -- the arithmetic of
+// sdetr_split_f16_pair_dev with one device scale for both
+__global__ void split_conv_weight_kernel(const float *__restrict__ w, int cout, int cin_g, int groups, int ksize,
+                                         const float *__restrict__ scale_dev, __half *__restrict__ f_hi, __half *__restrict__ f_lo,
+                                         __half *__restrict__ d_hi, __half *__restrict__ d_lo) {
+    const int taps = ksize * ksize, cout_g = cout / groups;
+    const int64_t n = (int64_t)cout * cin_g * taps;
+    const float scale = __ldg(scale_dev);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int tap = (int)(i % taps), ci = (int)((i / taps) % cin_g), co = (int)(i / ((int64_t)taps * cin_g));
+        const float x = w[i] * scale;
+        const __half h = __float2half_rn(x), l = __float2half_rn(x - __half2float(h));
+        const int64_t fi = ((int64_t)co * taps + tap) * cin_g + ci;
+        f_hi[fi] = h, f_lo[fi] = l;
+        if (d_hi) {
+            const int g = co / cout_g;
+            const int64_t di = ((int64_t)(g * cin_g + ci) * taps + (taps - 1 - tap)) * cout_g + (co - g * cout_g);
+            d_hi[di] = h, d_lo[di] = l;
+        }
+    }
+}
+
 inline bool rows_ok(const float *p, int64_t pitch, int64_t ld) { return aligned16(p) && pitch % 4 == 0 && ld % 4 == 0; }
 inline int elementwise_blocks(int64_t total) {
     const int64_t want = (total + 255) / 256, cap = 8LL * sm_count();
@@ -312,12 +528,85 @@ extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, 
     SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3: too many output pixels");
     if (M == 0) return SDETR_OK;
     static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel, kCvSmem, "conv2d_f16x3");
+    SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<false>, kCvSmem, "conv2d_f16x3");
     const ConvParams p{x, x_pitch, ldx, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
                        w_scale_dev, bias, y, y_pitch, ldy, H, W, Ho, Wo, (int)M, Cin / groups, Cout / groups, ksize, stride, act};
     const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
-    conv_f16x3_kernel<<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
+    conv_f16x3_kernel<false><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
     return check_launch("conv2d_f16x3");
+}
+
+extern "C" int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
+                                             const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
+                                             int Cout, int groups, int ksize, int H, int W, float *dx, int64_t dx_pitch,
+                                             int64_t lddx, sdetr_stream_t stream) {
+    SDETR_REQUIRE(dy && a_scale_dev && W_hi && W_lo && w_scale_dev && dx, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_transposed: null pointer");
+    SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_transposed: bad sizes");
+    SDETR_REQUIRE(ksize == 1 || ksize == 3, SDETR_ERR_UNSUPPORTED, "conv2d_f16x3_transposed: takes kernel 1 or 3");
+    SDETR_REQUIRE(Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kCvK == 0 && (Cout / groups) % kCvN == 0,
+                  SDETR_ERR_UNSUPPORTED, "conv2d_f16x3_transposed: Cin/groups=%d and Cout/groups=%d must be multiples of 64",
+                  Cin / groups, Cout / groups);
+    const int pad = ksize / 2, hy = H > 0 ? (H + 2 * pad - ksize) / 2 + 1 : 0, wy = W > 0 ? (W + 2 * pad - ksize) / 2 + 1 : 0;
+    SDETR_REQUIRE(Hy == hy && Wy == wy, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_transposed: dY is %dx%d, a stride-2 convolution of %dx%d gives %dx%d", Hy, Wy, H, W, hy, wy);
+    SDETR_REQUIRE(rows_ok(dy, dy_pitch, lddy) && lddy >= Cin && aligned16(W_hi) && aligned16(W_lo), SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_transposed: dy, its pitch and row stride and the weights must be 16-byte aligned");
+    SDETR_REQUIRE((reinterpret_cast<uintptr_t>(dx) & 7) == 0 && dx_pitch % 2 == 0 && lddx % 2 == 0 && lddx >= Cout,
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_transposed: dx, its pitch and row stride must be 8-byte aligned");
+    const int64_t M = (int64_t)batch * H * W;
+    SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_transposed: too many output pixels");
+    if (M == 0) return SDETR_OK;
+    static PerDeviceOnce once;
+    SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<true>, kCvSmem, "conv2d_f16x3_transposed");
+    const ConvParams p{dy, dy_pitch, lddy, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
+                       w_scale_dev, nullptr, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups, Cout / groups, ksize, 2, 0};
+    const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
+    conv_f16x3_kernel<true><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
+    return check_launch("conv2d_f16x3_transposed");
+}
+
+extern "C" int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, int Wo, int Cin, int Cout, int groups, int ksize) {
+    if (batch <= 0 || Ho <= 0 || Wo <= 0 || !wgrad_shape_ok(Cin, Cout, groups, ksize)) return 0;
+    const int tiles = (Cout / kCvM) * ((Cin / groups) / kCvN) * ksize * ksize;
+    int splits, per;
+    wgrad_splits((int64_t)batch * Ho * Wo, tiles, splits, per);
+    return (int64_t)splits * Cout * (Cin / groups) * ksize * ksize;
+}
+
+extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
+                                        int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin,
+                                        int Cout, int groups, int ksize, int stride, float *workspace, int64_t workspace_floats,
+                                        float *dw, sdetr_stream_t stream) {
+    SDETR_REQUIRE(dy && dy_scale_dev && x && x_scale_dev && dw && workspace, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_wgrad: null pointer");
+    SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_wgrad: bad sizes");
+    SDETR_REQUIRE((ksize == 1 || ksize == 3) && (stride == 1 || stride == 2), SDETR_ERR_UNSUPPORTED,
+                  "conv2d_f16x3_wgrad: takes kernel 1 or 3, stride 1 or 2");
+    SDETR_REQUIRE(wgrad_shape_ok(Cin, Cout, groups, 1), SDETR_ERR_UNSUPPORTED,
+                  "conv2d_f16x3_wgrad: Cin/groups=%d and Cout/groups=%d must be multiples of 64", Cin / groups, Cout / groups);
+    SDETR_REQUIRE(rows_ok(dy, dy_pitch, lddy) && lddy >= Cout && rows_ok(x, x_pitch, ldx) && ldx >= Cin, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_wgrad: dy, x, their pitches and row strides must be 16-byte aligned");
+    const int pad = ksize / 2, Ho = H > 0 ? (H + 2 * pad - ksize) / stride + 1 : 0, Wo = W > 0 ? (W + 2 * pad - ksize) / stride + 1 : 0;
+    const int64_t M = (int64_t)batch * Ho * Wo, n = (int64_t)Cout * (Cin / groups) * ksize * ksize;
+    SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_wgrad: too many output pixels");
+    const int tiles = (Cout / kCvM) * ((Cin / groups) / kCvN) * ksize * ksize;
+    int splits, per;
+    wgrad_splits(M, tiles, splits, per);
+    SDETR_REQUIRE(aligned16(workspace) && workspace_floats >= (int64_t)splits * n, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_wgrad: workspace too small or not 16-byte aligned");
+    if (splits > 0) {
+        static PerDeviceOnce once;
+        SDETR_OPT_IN_SMEM(once, conv_wgrad_f16x3_kernel, kWgSmem, "conv2d_f16x3_wgrad");
+        const WgradParams p{dy, dy_pitch, lddy, x, x_pitch, ldx, dy_scale_dev, x_scale_dev, workspace, H, W, Ho, Wo, (int)M, Cout,
+                            Cin / groups, Cout / groups, ksize, stride, per};
+        conv_wgrad_f16x3_kernel<<<dim3((unsigned)tiles, (unsigned)splits), kCvThreads, kWgSmem, (cudaStream_t)stream>>>(p);
+        const int rc = check_launch("conv2d_f16x3_wgrad");
+        if (rc) return rc;
+    }
+    wgrad_reduce_kernel<<<elementwise_blocks(n), 256, 0, (cudaStream_t)stream>>>(workspace, splits, n, dw);
+    return check_launch("conv2d_f16x3_wgrad (split sum)");
 }
 
 extern "C" int64_t sdetr_context_gate_workspace_floats(int batch, int HW, int C) {
@@ -366,4 +655,32 @@ extern "C" int sdetr_upsample_nearest_concat(const float *hi, int64_t hi_pitch, 
                                                                                          Rows{lo, lo_pitch, ldl}, Ho, Wo, batch, C,
                                                                                          dst, dst_pitch, ldd);
     return check_launch("upsample_nearest_concat");
+}
+
+extern "C" int sdetr_upsample_nearest_concat_backward(const float *g, int64_t g_pitch, int64_t ldg, int Ho, int Wo, int Hi, int Wi,
+                                                      int batch, int C, float *d_hi, int64_t d_pitch, int64_t ldd,
+                                                      sdetr_stream_t stream) {
+    SDETR_REQUIRE(g && d_hi, SDETR_ERR_INVALID_ARG, "upsample_nearest_concat_backward: null pointer");
+    SDETR_REQUIRE(batch >= 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && C > 0 && C % 4 == 0, SDETR_ERR_INVALID_ARG,
+                  "upsample_nearest_concat_backward: bad sizes (C a multiple of 4)");
+    SDETR_REQUIRE(rows_ok(g, g_pitch, ldg) && ldg >= C && rows_ok(d_hi, d_pitch, ldd) && ldd >= C, SDETR_ERR_INVALID_ARG,
+                  "upsample_nearest_concat_backward: operands, pitches and row strides must be 16-byte aligned");
+    const int64_t total = (int64_t)batch * Hi * Wi * (C / 4);
+    if (total == 0) return SDETR_OK;
+    upsample_concat_backward_kernel<<<elementwise_blocks(total), 256, 0, (cudaStream_t)stream>>>(Rows{g, g_pitch, ldg}, Ho, Wo, Hi,
+                                                                                                  Wi, batch, C, d_hi, d_pitch, ldd);
+    return check_launch("upsample_nearest_concat_backward");
+}
+
+extern "C" int sdetr_conv2d_f16x3_split_weight(const float *w, int Cout, int Cin, int groups, int ksize, const float *scale_dev,
+                                               void *fwd_hi, void *fwd_lo, void *dgrad_hi, void *dgrad_lo, sdetr_stream_t stream) {
+    SDETR_REQUIRE(w && scale_dev && fwd_hi && fwd_lo && (dgrad_hi == nullptr) == (dgrad_lo == nullptr), SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_split_weight: null pointer (dgrad_hi and dgrad_lo go together)");
+    SDETR_REQUIRE(Cout > 0 && Cin > 0 && groups > 0 && Cin % groups == 0 && Cout % groups == 0 && (ksize == 1 || ksize == 3),
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_split_weight: bad sizes");
+    const int64_t n = (int64_t)Cout * (Cin / groups) * ksize * ksize;
+    split_conv_weight_kernel<<<elementwise_blocks(n), 256, 0, (cudaStream_t)stream>>>(
+        w, Cout, Cin / groups, groups, ksize, scale_dev, reinterpret_cast<__half *>(fwd_hi), reinterpret_cast<__half *>(fwd_lo),
+        reinterpret_cast<__half *>(dgrad_hi), reinterpret_cast<__half *>(dgrad_lo));
+    return check_launch("conv2d_f16x3_split_weight");
 }

@@ -12,6 +12,17 @@ each RepVGG block's ``conv1 (3x3) + alpha * conv2 (1x1)`` into one grouped 3x3 c
 CSP layer's ``conv1 || conv2`` (two 1x1 over the same input) into one projection.  The kernels (``include/sdetr_b200.h``):
 ``sdetr_conv2d_f16x3`` (implicit-GEMM convolution, 3xFP16 on wgmma, bias + SiLU epilogue), ``sdetr_context_gate``
 (SqueezeAndExcitation + the block's residual) and ``sdetr_upsample_nearest_concat`` (the top-down path's operand).
+
+In training, or whenever autograd records (``training_tokens_supported``), ``forward_tokens`` follows the reference's op
+structure instead of the folded one: every convolution (a RepVGG block's 3x3 and 1x1, a CSP layer's conv1 and conv2 apart) runs
+on the same kernel through an autograd Function.  Its forward splits the weight once (``sdetr_conv2d_f16x3_split_weight``) into
+both fp16 layouts; its backward is the input gradient (``sdetr_conv2d_f16x3`` on dY with the flipped, per-group transposed
+weights; ``sdetr_conv2d_f16x3_transposed`` for stride 2) and ``sdetr_conv2d_f16x3_wgrad``.  Each
+BatchNorm is the module itself on the channels-last ``(b, C, H, W)`` view of the token rows (no copy), so batch statistics, running statistics,
+``momentum``, eval mode with gradients and ``nn.SyncBatchNorm`` behave as the modules define.  SiLU, the context gate, the
+residuals and the concatenations are torch ops on token rows; the top-down operand's backward is
+``sdetr_upsample_nearest_concat_backward``.  No host synchronisation and a fixed launch count, so a forward + backward can be
+captured in a CUDA graph.
 """
 from __future__ import annotations
 
@@ -153,6 +164,77 @@ def nearest_index(n_in: int, n_out: int) -> Tensor:
     return src.clamp(max=n_in - 1)
 
 
+def nearest_ranges(n_in: int, n_out: int) -> Tuple[Tensor, Tensor]:
+    """[begin, end) of the output positions that read each input position under nearest_index: the ranges the upsample
+    backward (sdetr_upsample_nearest_concat_backward) sums over"""
+    src = nearest_index(n_in, n_out)
+    s = torch.arange(n_in, dtype=torch.int64)
+    return torch.searchsorted(src, s, right=False), torch.searchsorted(src, s, right=True)
+
+
+class _TokenConv2d(torch.autograd.Function):
+    """y = conv2d(x, weight) on token rows, no bias (every convolution of the training path is followed by a BatchNorm).
+    x: (b, H*W, Cin) view; a_scale: pow2_scale (target 12) of a contiguous tensor that holds x, shared by the convolutions that
+    read the same input.  The weight is split once per call into both fp16 layouts the forward and the input gradient read."""
+
+    @staticmethod
+    def forward(ctx, x, weight, a_scale, hw, stride):
+        groups, k = x.shape[2] // weight.shape[1], weight.shape[-1]
+        w_hi, w_lo, ctx.d_hi, ctx.d_lo, ctx.w_scale = cabi.conv2d_f16x3_split_weight(weight.detach(), groups, ctx.needs_input_grad[0])
+        y = cabi.conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, ctx.w_scale, None, groups, k, stride, 0)
+        ctx.save_for_backward(x, a_scale)
+        ctx.hw, ctx.stride, ctx.groups, ctx.w_shape = hw, stride, groups, weight.shape
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, a_scale = ctx.saved_tensors
+        gy = gy.contiguous()  # the BatchNorm gradients this path produces already are: no copy
+        g_scale = cabi.pow2_scale(gy, 12)
+        k, pad = ctx.w_shape[-1], ctx.w_shape[-1] // 2
+        ho, wo = ((v + 2 * pad - k) // ctx.stride + 1 for v in ctx.hw)
+        dx = dw = None
+        if ctx.needs_input_grad[0]:
+            if ctx.stride == 1:
+                dx = cabi.conv2d_f16x3(gy, (ho, wo), g_scale, ctx.d_hi, ctx.d_lo, ctx.w_scale, None, ctx.groups, k, 1, 0)
+            else:
+                dx = cabi.conv2d_f16x3_transposed(gy, (ho, wo), g_scale, ctx.d_hi, ctx.d_lo, ctx.w_scale, ctx.groups, k, ctx.hw)
+        if ctx.needs_input_grad[1]:
+            dw = cabi.conv2d_f16x3_wgrad(gy, g_scale, x, a_scale, ctx.hw, ctx.w_shape, ctx.stride)
+        return dx, dw, None, None, None
+
+
+class _UpsampleConcat(torch.autograd.Function):
+    """[nearest(hi) | lo] on token rows (sdetr_upsample_nearest_concat) with its backward"""
+
+    @staticmethod
+    def forward(ctx, hi, hi_hw, lo, lo_hw):
+        ctx.hi_hw, ctx.lo_hw, ctx.c = hi_hw, lo_hw, hi.shape[2]
+        return cabi.upsample_nearest_concat(hi, hi_hw, lo, lo_hw)
+
+    @staticmethod
+    def backward(ctx, g):
+        c = ctx.c
+        d_hi = cabi.upsample_nearest_concat_backward(g[:, :, :c], ctx.lo_hw, ctx.hi_hw) if ctx.needs_input_grad[0] else None
+        return d_hi, None, g[:, :, c:], None
+
+
+def _norm_rows(bn: nn.Module, y: Tensor, hw) -> Tensor:
+    """the BatchNorm module on (b, H*W, C) token rows, which are the channels-last layout of (b, C, H, W): torch's
+    channels-last BatchNorm reads them in place (an (N, C, 1, 1) view would take the NCHW kernels with one pixel per image)"""
+    b, n, c = y.shape
+    return bn(y.view(b, hw[0], hw[1], c).permute(0, 3, 1, 2)).permute(0, 2, 3, 1).reshape(b, n, c)
+
+
+def _gate_rows(se: SqueezeAndExcitation, y: Tensor) -> Tensor:
+    """SqueezeAndExcitation on (b, HW, C) token rows"""
+    c = y.shape[2]
+    p = torch.softmax(F.linear(y, se.conv_mask.weight.view(1, c), se.conv_mask.bias).squeeze(2), 1)
+    ctx = torch.bmm(p.unsqueeze(1), y).squeeze(1)
+    gate = torch.sigmoid(F.linear(F.relu(F.linear(ctx, se.se_module[0].weight.view(-1, c))), se.se_module[2].weight.view(c, -1)))
+    return gate.unsqueeze(1) * y
+
+
 class _KConv:
     """one folded convolution in kernel form: (Cout, k, k, Cin / groups) fp16 pair with its device scale, fp32 bias (or None)"""
 
@@ -243,26 +325,24 @@ class RepVGGPluXNetwork(nn.Module):
             output["pool"] = F.max_pool2d(list(output.values())[-1], 1, 2, 0)
         return output
 
-    # ---- token-layout inference --------------------------------------------------------------------------------------
-    def tokens_supported(self, memory: Tensor, shapes_list: Sequence[Tuple[int, int]]) -> bool:
-        """True when forward_tokens can run this call: eval mode, CUDA fp32 memory, no autograd, no extra block, one channel
-        width C at every level with C / groups a multiple of 64, the reference's BatchNorm / SiLU layers, CSP layers without conv3
-        and with at least one block, and stride-2 downsampling that lands on the next level's shape (as the reference's
-        concatenation needs)."""
-        if self.training or self.extra_block or not memory.is_cuda or memory.dtype != torch.float32 or memory.dim() != 3:
-            return False
-        if torch.is_grad_enabled() and (memory.requires_grad or any(p.requires_grad for p in self.parameters())):
+    # ---- token-layout inference and training ---------------------------------------------------------------------------
+    def _autograd_records(self, memory: Tensor) -> bool:
+        return torch.is_grad_enabled() and (memory.requires_grad or any(p.requires_grad for p in self.parameters()))
+
+    def _tokens_structure_ok(self, memory: Tensor, shapes_list, norms) -> bool:
+        """the structural conditions of both token paths; ``norms``: the BatchNorm types accepted"""
+        if self.extra_block or not memory.is_cuda or memory.dtype != torch.float32 or memory.dim() != 3:
             return False
         c = memory.shape[2]
         if len(shapes_list) != len(self.layer_blocks) + 1 or len(shapes_list) < 2 or c % self.groups or (c // self.groups) % 64:
             return False
         for m in self.modules():
-            if isinstance(m, nn.modules.batchnorm._BatchNorm) and type(m) is not nn.BatchNorm2d:
+            if isinstance(m, nn.modules.batchnorm._BatchNorm) and type(m) not in norms:
                 return False
             if isinstance(m, Conv2dNormActivation):
                 if m[0].in_channels not in (c, 2 * c) or m[0].out_channels != c or m[0].dilation != (1, 1):
                     return False
-                if len(m) < 2 or type(m[1]) is not nn.BatchNorm2d or (len(m) == 3 and type(m[2]) is not nn.SiLU):
+                if len(m) < 2 or type(m[1]) not in norms or (len(m) == 3 and type(m[2]) is not nn.SiLU):
                     return False
         for layer in list(self.layer_blocks) + list(self.pan_blocks):
             if not isinstance(layer.conv3, nn.Identity) or len(layer.bottlenecks) == 0:
@@ -274,6 +354,27 @@ class RepVGGPluXNetwork(nn.Module):
             if ((h - 1) // 2 + 1, (w - 1) // 2 + 1) != (h2, w2):
                 return False
         return True
+
+    def tokens_supported(self, memory: Tensor, shapes_list: Sequence[Tuple[int, int]]) -> bool:
+        """True when forward_tokens can run this call on the folded eval weights: eval mode, CUDA fp32 memory, no autograd, no
+        extra block, one channel width C at every level with C / groups a multiple of 64, the reference's BatchNorm / SiLU
+        layers, CSP layers without conv3 and with at least one block, and stride-2 downsampling that lands on the next level's
+        shape (as the reference's concatenation needs)."""
+        if self.training or self._autograd_records(memory):
+            return False
+        return self._tokens_structure_ok(memory, shapes_list, (nn.BatchNorm2d,))
+
+    def training_tokens_supported(self, memory: Tensor, shapes_list: Sequence[Tuple[int, int]]) -> bool:
+        """True when forward_tokens runs this call with the reference's op structure under autograd: training mode or autograd
+        recording, the structure tokens_supported asks for (BatchNorm2d or SyncBatchNorm layers), fp32 CUDA parameters and
+        convolutions without bias."""
+        if not (self.training or self._autograd_records(memory)):
+            return False
+        if any(not p.is_cuda or p.dtype != torch.float32 for p in self.parameters()):
+            return False
+        if any(isinstance(m, Conv2dNormActivation) and m[0].bias is not None for m in self.modules()):
+            return False
+        return self._tokens_structure_ok(memory, shapes_list, (nn.BatchNorm2d, nn.SyncBatchNorm))
 
     def _kernel_weights(self):
         """folded eval weights in kernel form, rebuilt when any parameter or buffer changes (in place or replaced)"""
@@ -311,13 +412,46 @@ class RepVGGPluXNetwork(nn.Module):
             base = cur
         return dst
 
+    def _conv_norm_act_rows(self, m: Conv2dNormActivation, x: Tensor, a_scale: Tensor, hw, stride: int = 1) -> Tensor:
+        pad, k = m[0].kernel_size[0] // 2, m[0].kernel_size[0]
+        y = _norm_rows(m[1], _TokenConv2d.apply(x, m[0].weight, a_scale, hw, stride),
+                       [(v + 2 * pad - k) // stride + 1 for v in hw])
+        return m[2](y) if len(m) > 2 else y
+
+    def _csp_rows(self, layer: CSPRepPluXLayer, x: Tensor, hw) -> Tensor:
+        x_scale = cabi.pow2_scale(x, 12)
+        h = self._conv_norm_act_rows(layer.conv1, x, x_scale, hw)
+        for blk in layer.bottlenecks:
+            h_scale = cabi.pow2_scale(h, 12)
+            y = _norm_rows(blk.conv1[1], _TokenConv2d.apply(h, blk.conv1[0].weight, h_scale, hw, 1), hw)
+            y = y + blk.alpha * _norm_rows(blk.conv2[1], _TokenConv2d.apply(h, blk.conv2[0].weight, h_scale, hw, 1), hw)
+            h = _gate_rows(blk.se_module, blk.activation(y)) + h
+        return h + self._conv_norm_act_rows(layer.conv2, x, x_scale, hw)
+
+    def _forward_tokens_autograd(self, memory: Tensor, shapes_list, lv) -> Tensor:
+        """forward()'s op structure on token rows (training_tokens_supported)"""
+        levels = len(shapes_list)
+        lat = [None] * levels
+        feat_high, src = lv[-1], memory
+        for idx in range(levels - 1, 0, -1):
+            lat[idx] = self._conv_norm_act_rows(self.lateral_convs[idx - 1], feat_high, cabi.pow2_scale(src, 12), shapes_list[idx])
+            cat = _UpsampleConcat.apply(lat[idx], shapes_list[idx], lv[idx - 1], shapes_list[idx - 1])
+            feat_high = src = self._csp_rows(self.layer_blocks[idx - 1], cat, shapes_list[idx - 1])
+        outs = [feat_high]
+        for idx in range(levels - 1):
+            down = self._conv_norm_act_rows(self.downsample_blocks[idx], outs[-1], cabi.pow2_scale(outs[-1], 12), shapes_list[idx],
+                                            stride=2)
+            outs.append(self._csp_rows(self.pan_blocks[idx], torch.cat([down, lat[idx + 1]], 2), shapes_list[idx + 1]))
+        return torch.cat(outs, 1)
+
     def forward_tokens(self, memory: Tensor, shapes_list: Sequence[Tuple[int, int]]) -> Tensor:
-        """The neck on the encoder memory (b, Nv, C) with levels of shapes_list in token order -> (b, Nv, C), same values as
-        forward() on the NCHW maps in eval mode.  No host synchronisation: capturable in a CUDA graph."""
-        if not self.tokens_supported(memory, shapes_list):
-            raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported)")
+        """The neck on the encoder memory (b, Nv, C) with levels of shapes_list in token order -> (b, Nv, C), the values of
+        forward() on the NCHW maps.  Eval without autograd runs the folded weights (tokens_supported); training or autograd the
+        reference's op structure (training_tokens_supported).  No host synchronisation: capturable in a CUDA graph."""
+        folded = self.tokens_supported(memory, shapes_list)
+        if not folded and not self.training_tokens_supported(memory, shapes_list):
+            raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported / training_tokens_supported)")
         memory = memory.contiguous()
-        f = self._kernel_weights()
         b, nv, c = memory.shape
         shapes_list = [tuple(int(v) for v in s) for s in shapes_list]
         sizes = [h * w for h, w in shapes_list]
@@ -326,6 +460,9 @@ class RepVGGPluXNetwork(nn.Module):
             raise RuntimeError(f"forward_tokens: memory has {nv} tokens, the levels {sum(sizes)}")
         levels = len(sizes)
         lv = [memory[:, s:s + n] for s, n in zip(starts, sizes)]
+        if not folded:
+            return self._forward_tokens_autograd(memory, shapes_list, lv)
+        f = self._kernel_weights()
         out = torch.zeros_like(memory)  # zero: the activation scale of a level slice is taken over the whole tensor
         outs = [out[:, s:s + n] for s, n in zip(starts, sizes)]
         # bottom-up operands [downsample(previous output) | lateral output] of levels 1..L-1: the lateral convolutions of the

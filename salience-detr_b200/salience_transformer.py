@@ -701,7 +701,14 @@ class SalienceTransformer(nn.Module):
             return memory, salience
         if self.neck is not None:  # :185-192 (any nn.Module taking {i: NCHW}; neck.RepVGGPluXNetwork also runs in token layout)
             tokens_ok = getattr(self.neck, "tokens_supported", None)
-            if tokens_ok is not None and hasattr(self.neck, "forward_tokens") and tokens_ok(memory, plan.shapes_list):
+            training_ok = getattr(self.neck, "training_tokens_supported", None)
+            # a training neck takes the token path while a CUDA graph is being captured: replayed it is bound by the device and
+            # faster than cuDNN fp32 (tools/bench_neck_train.py); run eagerly its ~1600 launches bind it to the host, where it is
+            # no faster than the NCHW route below
+            if hasattr(self.neck, "forward_tokens") and (
+                    (tokens_ok is not None and tokens_ok(memory, plan.shapes_list)) or
+                    (training_ok is not None and torch.cuda.is_current_stream_capturing() and
+                     training_ok(memory, plan.shapes_list))):
                 memory = self.neck.forward_tokens(memory, plan.shapes_list)
             elif memory.is_cuda and not (torch.is_grad_enabled() and memory.requires_grad):
                 feats = dict(enumerate(cabi.tokens_to_maps(memory.contiguous(), plan.shapes_list)))   # one launch each way

@@ -165,9 +165,12 @@ int sdetr_upsample_bilinear_ac_backward(const float *grad_fine, int planes, int 
  *   concatenate levels, sort by score descending, reorder indices                       (:156-158)
  *   foreground_score = where(mask, min over the whole (b,Nv) tensor, score)             (:166-168)
  * Order of equal scores (unspecified in torch.topk/sort): larger score first, then smaller token index.
+ * As in torch.sort, -0 == +0 and every NaN (either sign) ranks above +inf.  A minimum over scores that hold a
+ * NaN is the NaN 0x7fffffff; of +0 and -0 it is -0.  selected_score keeps the bits of the score ranked.
  * raw_score (b,Nv); mask (b,Nv) uint8, 1 = padding; level_start_host / level_size_host / level_k_host:
  * HOST int32 arrays of length num_levels (k_l = level_token_nums, :120; k_l <= size_l).
- * -> selected_inds (b,K) int64, selected_score (b,K), foreground_score (b,Nv), K = sum k_l.
+ * -> selected_inds (b,K) int64, selected_score (b,K) (both may be NULL when K = 0), foreground_score (b,Nv),
+ * K = sum k_l.
  * tile_order (b,K) int32, nullable: positions 0..K-1 of each image's selected list ordered by the
  * spatial cell of their token (cell_px x cell_px image pixels; level-l token = level_stride_host[l] px):
  * the processing order handed to sdetr_msda_forward_ex after sdetr_order_prefixes().
@@ -188,7 +191,7 @@ int sdetr_order_prefixes(const int32_t *tile_order, int batch, int K, int num_la
                          const int32_t *nq_host, const int64_t *order_offset_host, int32_t *out_orders,
                          sdetr_stream_t stream);
 
-/* Generic segmented top-k by score (descending; ties: smaller position first).  Used for the
+/* Generic segmented top-k by score (descending, NaNs first; ties: smaller position first).  Used for the
  * "top-300 most salient tokens" pre-attention selection (salience_transformer.py:366-367).
  * score (segments, n) -> topk_index (segments, k) int64 positions within the segment.
  * workspace: sdetr_topk_workspace() bytes. */

@@ -113,13 +113,16 @@ __device__ __forceinline__ float block_max(float m) {
     return m;
 }
 
-// fp32 -> uint32 whose ascending order is the DESCENDING order of the floats (-0 == +0, NaN first).
+// fp32 -> uint32 whose ascending order is the DESCENDING order of the floats, as torch.sort(descending=True) orders
+// them: -0 == +0, and every NaN (either sign, any payload) is one key that comes first.
 __device__ __forceinline__ uint32_t desc_key(float f) {
+    if (f != f) return 0u;
     if (f == 0.f) f = 0.f;  // canonicalise -0
     uint32_t u = __float_as_uint(f);
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);  // ascending-orderable
-    return ~u;
+    return ~u;  // +inf -> 0x007fffff; no number maps to 0, the key of the NaNs
 }
+// the inverse for every key but those of a zero (gives +0) and of the NaNs (gives the NaN 0x7fffffff)
 __device__ __forceinline__ float desc_key_inv(uint32_t k) {
     uint32_t u = ~k;
     u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;

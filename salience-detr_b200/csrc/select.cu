@@ -265,34 +265,64 @@ constexpr int kBitonicMax = 16384;  // 128 KB of shared memory
 
 // ---- kernels ---------------------------------------------------------------------------------------------
 
+// `score.min()` (salience_transformer.py:146,168) as a minimum of keys in which every NaN is the smallest and -0 < +0,
+// so that the result does not depend on the reduction order: a NaN propagates, as in torch, and comes out as the NaN
+// 0x7fffffff (torch leaves which NaN to the backend); of +0 and -0 the minimum is -0.
+__device__ __forceinline__ uint32_t min_key(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return f != f ? 0u : (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float min_key_inv(uint32_t k) {
+    return __uint_as_float(k == 0u ? 0x7fffffffu : (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+__device__ __forceinline__ int level_of(const LevelTable &tb, int t) {
+    int l = 0;
+#pragma unroll
+    for (int u = 1; u < kMaxLevels; ++u)
+        if (u < tb.L && t >= tb.start[u]) l = u;
+    return l;
+}
+
+// The score token t of image row `row` was ranked by, with its own bits.  The key gives it back except for a zero (the
+// key dropped its sign) and a NaN (sign and payload): those few are read again, so a selected -0 stays -0.
+template <class LevelOf>
+__device__ __forceinline__ float selected_score(uint32_t key, const float *raw, const uint8_t *mask, const float *lmin,
+                                                int64_t row, int t, LevelOf level) {
+    const float s = desc_key_inv(key);
+    if (s != 0.f && s == s) return s;
+    return __ldg(mask + row + t) ? __ldg(lmin + level()) : __ldg(raw + row + t);
+}
+
 // per-level minimum over the whole (batch, HW_l) score tensor (salience_transformer.py:146 `score.min()`)
 __global__ void __launch_bounds__(1024) level_min_kernel(const float *__restrict__ raw, LevelTable tb, int batch,
                                                          int nv, float *__restrict__ lmin) {
-    __shared__ float red[32];
+    __shared__ uint32_t red[32];
     const int l = blockIdx.x;
-    float m = INFINITY;
+    uint32_t m = min_key(INFINITY);
     const int total = batch * tb.size[l];
     for (int i = threadIdx.x; i < total; i += blockDim.x) {
         const int b = i / tb.size[l], t = i - b * tb.size[l];
-        m = fminf(m, __ldg(raw + (int64_t)b * nv + tb.start[l] + t));
+        m = min(m, min_key(__ldg(raw + (int64_t)b * nv + tb.start[l] + t)));
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    for (int o = 16; o > 0; o >>= 1) m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
     __syncthreads();
     if (threadIdx.x < 32) {
         m = red[threadIdx.x];
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
-        if (threadIdx.x == 0) lmin[l] = m;
+        for (int o = 16; o > 0; o >>= 1) m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if (threadIdx.x == 0) lmin[l] = min_key_inv(m);
     }
 }
 
 // foreground_score = where(mask, global min, raw)  (salience_transformer.py:166-168)
 __global__ void foreground_kernel(const float *__restrict__ raw, const uint8_t *__restrict__ mask,
                                   const float *__restrict__ lmin, int L, int64_t total, float *__restrict__ fg) {
-    float g = INFINITY;
-    for (int l = 0; l < L; ++l) g = fminf(g, __ldg(lmin + l));
+    uint32_t gk = min_key(INFINITY);
+    for (int l = 0; l < L; ++l) gk = min(gk, min_key(__ldg(lmin + l)));
+    const float g = min_key_inv(gk);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
         fg[i] = mask[i] ? g : raw[i];
 }
@@ -320,6 +350,9 @@ __global__ void __launch_bounds__(kSortThreads) level_sort_kernel(const float *_
 __global__ void __launch_bounds__(kSortThreads) merge_sort_kernel(const uint32_t *lk, const uint32_t *lv, LevelTable tb,
                                                                   int nv, int K, uint32_t *ka, uint32_t *va,
                                                                   uint32_t *kb, uint32_t *vb,
+                                                                  const float *__restrict__ raw,
+                                                                  const uint8_t *__restrict__ mask,
+                                                                  const float *__restrict__ lmin,
                                                                   int64_t *__restrict__ sel_inds,
                                                                   float *__restrict__ sel_score) {
     __shared__ SortSmem sm;
@@ -335,8 +368,10 @@ __global__ void __launch_bounds__(kSortThreads) merge_sort_kernel(const uint32_t
     };
     block_radix_sort(load0, K, ka + dst, va + dst, kb + dst, vb + dst, sm);
     for (int j = threadIdx.x; j < K; j += blockDim.x) {
-        sel_inds[dst + j] = (int64_t)((volatile uint32_t *)vb)[dst + j];
-        sel_score[dst + j] = desc_key_inv(((volatile uint32_t *)kb)[dst + j]);
+        const int t = (int)((volatile uint32_t *)vb)[dst + j];
+        sel_inds[dst + j] = t;
+        sel_score[dst + j] = selected_score(((volatile uint32_t *)kb)[dst + j], raw, mask, lmin, src, t,
+                                            [&] { return level_of(tb, t); });
     }
 }
 
@@ -441,32 +476,35 @@ __global__ void __launch_bounds__(kSortThreads) level_select_kernel(const float 
 // requested, the spatial-cell processing order of the sorted list.  K <= kBitonicMax.
 __global__ void __launch_bounds__(kSortThreads) merge_bitonic_kernel(const uint32_t *__restrict__ ck,
                                                                      const uint32_t *__restrict__ cv, LevelTable tb,
-                                                                     int K, int N, int cell_px, int cells_x,
+                                                                     int K, int N, int nv, int cell_px, int cells_x,
+                                                                     const float *__restrict__ raw,
+                                                                     const uint8_t *__restrict__ mask,
+                                                                     const float *__restrict__ lmin,
                                                                      int64_t *__restrict__ sel_inds,
                                                                      float *__restrict__ sel_score,
                                                                      int32_t *__restrict__ tile_order) {
     extern __shared__ unsigned long long keys[];
     const int b = blockIdx.x;
-    const int64_t base = (int64_t)b * K;
+    const int64_t base = (int64_t)b * K, row = (int64_t)b * nv;
     for (int j = threadIdx.x; j < N; j += kSortThreads)
         keys[j] = j < K ? ((unsigned long long)ck[base + j] << 32) | cv[base + j] : ~0ull;
     __syncthreads();
     bitonic_sort_smem(keys, N);
     for (int j = threadIdx.x; j < K; j += kSortThreads) {
         const unsigned long long e = keys[j];
-        sel_inds[base + j] = (int64_t)(e & 0xffffffffull);
-        sel_score[base + j] = desc_key_inv((uint32_t)(e >> 32));
+        const int t = (int)(e & 0xffffffffull);
+        sel_inds[base + j] = t;
+        sel_score[base + j] = selected_score((uint32_t)(e >> 32), raw, mask, lmin, row, t, [&] { return level_of(tb, t); });
     }
     if (!tile_order) return;
     __syncthreads();
-    for (int j = threadIdx.x; j < N; j += kSortThreads) {
+    // a block-uniform trip count: every thread reaches the barrier, also when N < kSortThreads
+    for (int j0 = 0; j0 < N; j0 += kSortThreads) {
+        const int j = j0 + threadIdx.x;
         unsigned long long e = ~0ull;
         if (j < K) {
             const int t = (int)(keys[j] & 0xffffffffull);
-            int l = 0;
-#pragma unroll
-            for (int u = 1; u < kMaxLevels; ++u)
-                if (u < tb.L && t >= tb.start[u]) l = u;
+            const int l = level_of(tb, t);
             const int r = t - tb.start[l];
             const int y = r / tb.width[l], x = r - y * tb.width[l];
             const int cy = (y * tb.stride[l] + tb.stride[l] / 2) / cell_px;
@@ -474,7 +512,7 @@ __global__ void __launch_bounds__(kSortThreads) merge_bitonic_kernel(const uint3
             e = ((unsigned long long)(((uint32_t)(cy * cells_x + cx) << 3) | (uint32_t)l) << 32) | (uint32_t)j;
         }
         __syncthreads();  // every thread has read keys[j] of this round before anyone overwrites it
-        keys[j] = e;
+        if (j < N) keys[j] = e;
     }
     __syncthreads();
     bitonic_sort_smem(keys, N);
@@ -564,8 +602,9 @@ __device__ __forceinline__ int lower_bound_u64(const unsigned long long *a, int 
 }
 
 __global__ void __launch_bounds__(256) merge_rank_kernel(const unsigned long long *__restrict__ sorted, ListTable lt, int K,
-                                                         int batch, int64_t *__restrict__ sel_inds,
-                                                         float *__restrict__ sel_score) {
+                                                         int batch, int nv, const float *__restrict__ raw,
+                                                         const uint8_t *__restrict__ mask, const float *__restrict__ lmin,
+                                                         int64_t *__restrict__ sel_inds, float *__restrict__ sel_score) {
     const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= (int64_t)batch * K) return;
     const int b = (int)(g / K), j = (int)(g - (int64_t)b * K);
@@ -577,8 +616,10 @@ __global__ void __launch_bounds__(256) merge_rank_kernel(const unsigned long lon
     int pos = j - lt.off[li];
     for (int t = 0; t < lt.n; ++t)
         if (t != li) pos += lower_bound_u64(base + lt.off[t], lt.cnt[t], key);
-    sel_inds[(int64_t)b * K + pos] = (int64_t)(key & 0xffffffffull);
-    sel_score[(int64_t)b * K + pos] = desc_key_inv((uint32_t)(key >> 32));
+    const int t = (int)(key & 0xffffffffull);
+    sel_inds[(int64_t)b * K + pos] = t;
+    sel_score[(int64_t)b * K + pos] = selected_score((uint32_t)(key >> 32), raw, mask, lmin, (int64_t)b * nv, t,
+                                                     [&] { return lt.level[li]; });
 }
 
 // image: processing order = counting sort of the selected positions by (spatial cell, level).  The order inside
@@ -665,8 +706,7 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
                                      int batch, int num_value, int num_levels, int64_t *selected_inds,
                                      float *selected_score, float *foreground_score, int32_t *tile_order,
                                      void *workspace, size_t workspace_bytes, sdetr_stream_t stream) {
-    SDETR_REQUIRE(raw_score && mask && level_start_host && level_size_host && level_k_host && selected_inds &&
-                      selected_score && foreground_score && workspace,
+    SDETR_REQUIRE(raw_score && mask && level_start_host && level_size_host && level_k_host && foreground_score && workspace,
                   SDETR_ERR_INVALID_ARG, "salience_select: null pointer");
     SDETR_REQUIRE(batch > 0 && num_value > 0 && num_levels > 0 && num_levels <= kMaxLevels, SDETR_ERR_INVALID_ARG,
                   "salience_select: bad sizes (batch %d, num_value %d, levels %d)", batch, num_value, num_levels);
@@ -691,6 +731,8 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
         }
     }
     tb.koff[num_levels] = K;
+    // with K = 0 the selection outputs are empty (an empty tensor may have a null data pointer)
+    SDETR_REQUIRE(K == 0 || (selected_inds && selected_score), SDETR_ERR_INVALID_ARG, "salience_select: null pointer");
     SDETR_REQUIRE(cover == num_value, SDETR_ERR_INVALID_ARG, "salience_select: levels cover %d of %d tokens", cover,
                   num_value);
     cudaStream_t s = (cudaStream_t)stream;
@@ -736,7 +778,8 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
         level_select_sort_kernel<<<batch * lt.n, kSortThreads, 0, s>>>(raw_score, mask, lmin, tb, lt, num_value, K, sorted);
         if ((rc = check_launch("salience_select/level_select_sort"))) return rc;
         const int64_t cand = (int64_t)batch * K;
-        merge_rank_kernel<<<(unsigned)((cand + 255) / 256), 256, 0, s>>>(sorted, lt, K, batch, selected_inds, selected_score);
+        merge_rank_kernel<<<(unsigned)((cand + 255) / 256), 256, 0, s>>>(sorted, lt, K, batch, num_value, raw_score, mask,
+                                                                         lmin, selected_inds, selected_score);
         if ((rc = check_launch("salience_select/merge_rank"))) return rc;
         if (tile_order) {
             tile_count_kernel<<<batch, kSortThreads, (size_t)(bins + 1) * sizeof(uint32_t), s>>>(selected_inds, tb, K, cell_px,
@@ -754,8 +797,9 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
         const size_t smem = (size_t)N * sizeof(unsigned long long);
         static PerDeviceOnce once_b;
         SDETR_OPT_IN_SMEM(once_b, merge_bitonic_kernel, kBitonicMax * (int)sizeof(unsigned long long), "salience_select");
-        merge_bitonic_kernel<<<batch, kSortThreads, smem, s>>>(buf[0], buf[1], tb, K, N, tile_order ? cell_px : 1,
-                                                               cells_x, selected_inds, selected_score, tile_order);
+        merge_bitonic_kernel<<<batch, kSortThreads, smem, s>>>(buf[0], buf[1], tb, K, N, num_value,
+                                                               tile_order ? cell_px : 1, cells_x, raw_score, mask, lmin,
+                                                               selected_inds, selected_score, tile_order);
         return check_launch("salience_select/merge_bitonic");
     }
     // large-K fallback (e.g. the 5-scale geometry, K = 45 570): segmented LSD radix sorts through global memory
@@ -763,7 +807,7 @@ extern "C" int sdetr_salience_select(const float *raw_score, const uint8_t *mask
                                                                   buf[2], buf[3]);
     if ((rc = check_launch("salience_select/level_sort"))) return rc;
     merge_sort_kernel<<<batch, kSortThreads, 0, s>>>(buf[2], buf[3], tb, num_value, K, buf[4], buf[5], buf[6], buf[7],
-                                                     selected_inds, selected_score);
+                                                     raw_score, mask, lmin, selected_inds, selected_score);
     if ((rc = check_launch("salience_select/merge_sort"))) return rc;
     if (tile_order) {
         const int cells_x = (max_w_px + cell_px - 1) / cell_px + 1;

@@ -230,7 +230,8 @@ def _select_case(b, shapes, ratios, seed, pad=None, quantize=False):
     dict(b=2, shapes=[(12, 16), (6, 8), (3, 4), (2, 2)], ratios=(0.4, 0.8, 1.0, 1.0), seed=1, pad=[0.0, 0.3]),
     dict(b=3, shapes=[(40, 50), (20, 25), (10, 13)], ratios=(0.3, 0.6, 1.0), seed=2, pad=[0.0, 0.1, 0.5], quantize=True),
     dict(b=1, shapes=[(100, 168), (50, 84), (25, 42), (13, 21)], ratios=(0.4, 0.8, 1.0, 1.0), seed=3, pad=[0.008]),
-    # k_0 = 10 080 > 8192: single-CTA bitonic merge path;  K = 40 320 > 16 384: global-memory radix path (5-scale size)
+    # k_0 = 10 080 (5 slices of 2048) and K = 40 320 (21 slices): both fit the rank-merge path; the bitonic and radix
+    # paths are covered in test_select_paths.py
     dict(b=2, shapes=[(100, 168)], ratios=(0.6,), seed=4, pad=[0.0, 0.2]),
     dict(b=2, shapes=[(200, 336), (100, 168)], ratios=(0.4, 0.8), seed=5, pad=[0.0, 0.1]),
 ])
@@ -728,8 +729,8 @@ def test_msda_module_reference_boxes(pkg):
 
 def test_five_scale_stress_geometry(pkg):
     """salience_detr_resnet50_5scale geometry (strides 4/8/16/32, Nv = 89 250, K = 45 330 with the 800x1333-in-800x1344
-    padding mask; 45 570 for an all-valid mask): the large-K selection path
-    (global-memory radix sorts) stays bit-exact with the oracle and the encoder half runs end to end."""
+    padding mask; 45 570 for an all-valid mask): the selection (25 slices of 2048 and 2464 cell bins, so the rank-merge
+    path) stays bit-exact with the oracle and the encoder half runs end to end."""
     from salience_detr_b200.synthetic import build_model, make_inputs
     torch.cuda.synchronize()  # surface any earlier asynchronous error here, not inside this test
     model = build_model(strides=(4, 8, 16, 32)).to(DEV)

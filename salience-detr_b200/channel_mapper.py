@@ -23,7 +23,7 @@ from typing import List, Mapping, Optional, Sequence, Tuple
 import torch
 from torch import Tensor, nn
 
-from . import cabi
+from . import cabi, derived
 from .neck import Conv2dNormActivation, _KConv
 
 
@@ -77,8 +77,6 @@ class ChannelMapper(nn.Module):
                                                    padding=1, bias=bias, groups=groups, dilation=dilation, norm_layer=norm_layer,
                                                    activation_layer=activation_layer, inplace=inplace))
             in_channel = out_channels
-        self._kernel_key = None
-        self._kernel = None
         self.init_weights()
 
     def init_weights(self):
@@ -139,17 +137,15 @@ class ChannelMapper(nn.Module):
 
     def _kernel_weights(self):
         """convolutions in kernel form and the (L, C) GroupNorm affine tables, rebuilt when any parameter changes"""
-        key = tuple((p.data_ptr(), p._version) for p in self.parameters())
-        if self._kernel_key != key:
-            with torch.no_grad():
-                convs = [_KConv(m[0].weight.detach(), m[0].bias.detach() if m[0].bias is not None else None, m[0].groups,
-                                m[0].stride[0], 0) for m in self.convs]
-                gn = [m[1] for m in self.convs]
-                ones = torch.ones(gn[0].num_channels, device=self.convs[0][0].weight.device)
-                gamma = torch.stack([n.weight.detach() if n.affine else ones for n in gn]).float().contiguous()
-                beta = torch.stack([n.bias.detach() if n.affine else ones * 0 for n in gn]).float().contiguous()
-            self._kernel, self._kernel_key = (convs, gamma, beta, gn[0].num_groups, gn[0].eps), key
-        return self._kernel
+        def build():
+            convs = [_KConv(m[0].weight.detach(), m[0].bias.detach() if m[0].bias is not None else None, m[0].groups,
+                            m[0].stride[0], 0) for m in self.convs]
+            gn = [m[1] for m in self.convs]
+            ones = torch.ones(gn[0].num_channels, device=self.convs[0][0].weight.device)
+            gamma = torch.stack([n.weight.detach() if n.affine else ones for n in gn]).float().contiguous()
+            beta = torch.stack([n.bias.detach() if n.affine else ones * 0 for n in gn]).float().contiguous()
+            return convs, gamma, beta, gn[0].num_groups, gn[0].eps
+        return derived.cached(self, "kernel_weights", list(self.parameters()), build)
 
     def launches_per_forward(self, nchw_inputs: Optional[int] = None) -> int:
         """library launches of one forward_tokens: one transpose per NCHW input (default: all inputs), per convolution 2

@@ -28,7 +28,7 @@ import torch
 from torch import Tensor, nn
 from torch.nn import functional as F
 
-from . import cabi, gemm
+from . import cabi, derived, gemm
 from .ms_deform_attn import MultiScaleDeformableAttention
 
 
@@ -144,8 +144,6 @@ class SalienceTransformerDecoder(nn.Module):
         self.class_head = nn.ModuleList([nn.Linear(self.embed_dim, num_classes) for _ in range(num_layers)])
         self.bbox_head = nn.ModuleList([MLP(self.embed_dim, self.embed_dim, 4, 3) for _ in range(num_layers)])
         self.norm = nn.LayerNorm(self.embed_dim)
-        self._vproj_key = None
-        self._vproj = None
         self.init_weights()
 
     def init_weights(self):
@@ -160,13 +158,9 @@ class SalienceTransformerDecoder(nn.Module):
             nn.init.constant_(bbox_head.layers[-1].bias, 0.0)
 
     def _value_projection(self):
-        ps = [(l.cross_attn.value_proj.weight, l.cross_attn.value_proj.bias) for l in self.layers]
-        key = tuple((w.data_ptr(), w._version, b._version) for w, b in ps)
-        if self._vproj_key != key:
-            with torch.no_grad():
-                self._vproj = (torch.cat([w for w, _ in ps], 0).contiguous(), torch.cat([b for _, b in ps], 0).contiguous())
-            self._vproj_key = key
-        return self._vproj
+        ws = [l.cross_attn.value_proj.weight for l in self.layers]
+        bs = [l.cross_attn.value_proj.bias for l in self.layers]
+        return derived.cached(self, "value_projection", ws + bs, lambda: (torch.cat(ws, 0).contiguous(), torch.cat(bs, 0).contiguous()))
 
     def forward(self, query, reference_points, value, spatial_shapes, level_start_index, valid_ratios, key_padding_mask=None,
                 attn_mask=None):

@@ -18,14 +18,13 @@ These are true dense GEMMs, the only place of the path where tensor cores belong
 from __future__ import annotations
 
 import contextlib
-import weakref
 from typing import Dict, Optional, Tuple
 
 import torch
 from torch import Tensor
 from torch.nn import functional as F
 
-from . import cabi
+from . import cabi, derived
 
 MODE = "auto"
 OWN_KERNEL = __import__("os").environ.get("SDETR_GEMM_KERNEL", "f16x3")  # "auto" / "tcgen05" own-kernel flavour: "f16x3" (3xFP16, K % 64 == 0) or "tf32x3" (3xTF32)
@@ -33,14 +32,6 @@ PRESPLIT_PERSISTENT = True  # persistent kernel fed a pre-split weight (W_hi / W
 LONG_K_PRESPLIT = False  # K >= 1024: True = "SS" kernel with the pre-split weight, False = persistent raw-weight kernel "P" (measured equal or faster)
 SMALL_M = 2304  # "auto": at most this many rows -> cuBLAS fp32 (latency-bound; measured faster than either tensor-core path, tools/bench_small.py)
 K_CHUNK = 512  # longest reduction handed to one tensor-core GEMM (its accumulator truncates: error ~ length)
-_weight_cache: Dict[int, tuple] = {}
-
-
-def _prune(cache: Dict[int, tuple]):
-    """Drop entries whose parameter has been freed (the caches are keyed by id(), which outlives the object)."""
-    if len(cache) >= 64:
-        for k in [k for k, v in cache.items() if v[2]() is None]:
-            del cache[k]
 
 
 @contextlib.contextmanager
@@ -59,45 +50,17 @@ def _chunk_of(K: int) -> int:
 
 def split_weight(weight: Tensor) -> Tensor:
     """(N,K) -> cached (N,3K) per-chunk [hi|lo|hi]; rebuilt when the parameter is modified in place or replaced."""
-    key = (weight.data_ptr(), weight._version, tuple(weight.shape), _chunk_of(weight.shape[1]))
-    hit = _weight_cache.get(id(weight))
-    # the weak reference guards against id()/data_ptr reuse by a NEW tensor after the cached one was freed
-    if hit is None or hit[0] != key or hit[2]() is not weight:
-        with torch.no_grad():
-            hit = (key, cabi.split_tf32(weight.detach().contiguous(), layout_b=True, chunk=_chunk_of(weight.shape[1])),
-                   weakref.ref(weight))
-        _prune(_weight_cache)
-        _weight_cache[id(weight)] = hit
-    return hit[1]
-
-
-_pair_cache: Dict[int, tuple] = {}
+    return derived.cached(weight, "split_tf32", (weight,), lambda: cabi.split_tf32(
+        weight.detach().contiguous(), layout_b=True, chunk=_chunk_of(weight.shape[1])))
 
 
 def split_weight_pair(weight: Tensor) -> Tuple[Tensor, Tensor]:
-    key = (weight.data_ptr(), weight._version, tuple(weight.shape))
-    hit = _pair_cache.get(id(weight))
-    if hit is None or hit[0] != key or hit[2]() is not weight:
-        with torch.no_grad():
-            hit = (key, cabi.split_tf32_pair(weight.detach()), weakref.ref(weight))
-        _prune(_pair_cache)
-        _pair_cache[id(weight)] = hit
-    return hit[1]
-
-
-_f16_cache: Dict[int, tuple] = {}
+    return derived.cached(weight, "split_tf32_pair", (weight,), lambda: cabi.split_tf32_pair(weight.detach()))
 
 
 def split_weight_f16(weight: Tensor):
     """(N,K) -> cached (W_hi fp16, W_lo fp16, power-of-two scale); one host read of max|W| per parameter version."""
-    key = (weight.data_ptr(), weight._version, tuple(weight.shape))
-    hit = _f16_cache.get(id(weight))
-    if hit is None or hit[0] != key or hit[2]() is not weight:
-        with torch.no_grad():
-            hit = (key, cabi.split_f16_pair(weight.detach()), weakref.ref(weight))
-        _prune(_f16_cache)
-        _f16_cache[id(weight)] = hit
-    return hit[1]
+    return derived.cached(weight, "split_f16_pair", (weight,), lambda: cabi.split_f16_pair(weight.detach()))
 
 
 _ACT = {None: 0, "relu": 1, "gelu": 2}
@@ -150,30 +113,25 @@ def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input:
 
 # ---- training path: tensor-core Linear with autograd ---------------------------------------------------------------------------
 TRAIN_TENSOR_CORE = __import__("os").environ.get("SDETR_TRAIN_TENSOR_CORE", "1") != "0"
-_train_cache: Dict[int, tuple] = {}
 _const16: Dict[int, Tensor] = {}
+
+
+def _split_train(weight: Tensor):
+    w = weight.detach()
+    scale = cabi.pow2_scale(w if w.is_contiguous() else w.contiguous(), 14)
+    fwd = cabi.split_f16_pair_dev(w, scale)
+    bwd = cabi.split_f16_pair_dev(w.t().contiguous(), scale) if w.shape[0] % 64 == 0 else None
+    return fwd, bwd
 
 
 def _train_splits(weight: Tensor):
     """Per parameter VERSION (the optimizer bumps it every step): device-side power-of-two scale, the 3xFP16 split of W (for y)
     and of W^T (for dx).  Everything stays on the device -- no host read of max|W|, unlike ``split_weight_f16``."""
-    key = (weight.data_ptr(), weight._version, tuple(weight.shape))
-    hit = _train_cache.get(id(weight))
-    capturing = weight.is_cuda and torch.cuda.is_current_stream_capturing()
     # inside a CUDA-graph capture of a training step the split kernels must be PART of the graph (the optimizer rewrites the
     # weights on every replay, and no Python runs then): never serve a capture from the cache, never cache what it produced
-    if capturing or hit is None or hit[0] != key or hit[2]() is not weight:
-        with torch.no_grad():
-            w = weight.detach()
-            scale = cabi.pow2_scale(w if w.is_contiguous() else w.contiguous(), 14)
-            fwd = cabi.split_f16_pair_dev(w, scale)
-            bwd = cabi.split_f16_pair_dev(w.t().contiguous(), scale) if w.shape[0] % 64 == 0 else None
-        hit = (key, (fwd, bwd), weakref.ref(weight))
-        if capturing:
-            return hit[1]
-        _prune(_train_cache)
-        _train_cache[id(weight)] = hit
-    return hit[1]
+    if weight.is_cuda and torch.cuda.is_current_stream_capturing():
+        return _split_train(weight)
+    return derived.cached(weight, "train_splits", (weight,), lambda: _split_train(weight))
 
 
 class _LinearF16x3(torch.autograd.Function):

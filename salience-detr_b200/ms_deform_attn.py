@@ -25,7 +25,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 from torch.nn import functional as F
 
-from . import cabi, gemm
+from . import cabi, derived, gemm
 
 
 def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step=64):
@@ -96,9 +96,6 @@ class MultiScaleDeformableAttention(nn.Module):
         self.attention_weights = nn.Linear(embed_dim, n)
         self.value_proj = nn.Linear(embed_dim, embed_dim)
         self.output_proj = nn.Linear(embed_dim, embed_dim)
-        self._fused_w: Optional[Tensor] = None
-        self._fused_b: Optional[Tensor] = None
-        self._fused_key = None
         self.init_weights()
 
     def init_weights(self):
@@ -118,19 +115,13 @@ class MultiScaleDeformableAttention(nn.Module):
             self.value_proj.bias.zero_()
             nn.init.xavier_uniform_(self.output_proj.weight)
             self.output_proj.bias.zero_()
-        self._fused_w = None
 
     # -- inference fast path --------------------------------------------------------------------------------
     def fused_projection(self):
         """Concatenated [sampling_offsets | attention_weights] weight/bias (one GEMM, N = 3*M*L*P)."""
         so, aw = self.sampling_offsets, self.attention_weights
-        key = (so.weight.data_ptr(), so.weight._version, so.bias._version, aw.weight._version, aw.bias._version)
-        if self._fused_w is None or self._fused_key != key:  # rebuilt after load_state_dict / optimizer steps
-            self._fused_key = key
-            with torch.no_grad():
-                self._fused_w = torch.cat([self.sampling_offsets.weight, self.attention_weights.weight], 0).contiguous()
-                self._fused_b = torch.cat([self.sampling_offsets.bias, self.attention_weights.bias], 0).contiguous()
-        return self._fused_w, self._fused_b
+        return derived.cached(self, "fused_projection", (so.weight, so.bias, aw.weight, aw.bias), lambda: (
+            torch.cat([so.weight, aw.weight], 0).contiguous(), torch.cat([so.bias, aw.bias], 0).contiguous()))
 
     def project_value(self, value: Tensor, key_padding_mask: Optional[Tensor]) -> Tensor:
         """value_proj + zeroing of padded rows (ms_deform_attn.py:316-321) -> (b,Nv,M,D)."""

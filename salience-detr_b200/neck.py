@@ -33,7 +33,7 @@ import torch
 from torch import Tensor, nn
 from torch.nn import functional as F
 
-from . import cabi
+from . import cabi, derived
 
 
 class Conv2dNormActivation(nn.Sequential):
@@ -284,8 +284,6 @@ class RepVGGPluXNetwork(nn.Module):
         self.extra_block = extra_block
         self.groups = groups
         self._activation = activation
-        self._folded_key = None
-        self._folded = None
         self.init_weights()
 
     def init_weights(self):
@@ -378,19 +376,16 @@ class RepVGGPluXNetwork(nn.Module):
 
     def _kernel_weights(self):
         """folded eval weights in kernel form, rebuilt when any parameter or buffer changes (in place or replaced)"""
-        ts = list(self.parameters()) + list(self.buffers())
-        key = tuple((t.data_ptr(), t._version) for t in ts)
-        if self._folded_key != key:
+        def build():
             silu = cabi.ACT_SILU
-            with torch.no_grad():
-                f = dict(lateral=[_KConv(*fold_conv_norm(m, torch.float64), 1, 1, silu) for m in self.lateral_convs],
-                         down=[_KConv(*fold_conv_norm(m, torch.float64), 1, 2, silu) for m in self.downsample_blocks])
-                for name in ("layer_blocks", "pan_blocks"):
-                    f[name] = [(_KConv(*fold_csp_projection(layer, torch.float64), 1, 1, silu),
-                                [(_KConv(*fold_repvgg(blk, torch.float64), blk.conv1[0].groups, 1, silu), _KGate(blk.se_module))
-                                 for blk in layer.bottlenecks]) for layer in getattr(self, name)]
-            self._folded, self._folded_key = f, key
-        return self._folded
+            f = dict(lateral=[_KConv(*fold_conv_norm(m, torch.float64), 1, 1, silu) for m in self.lateral_convs],
+                     down=[_KConv(*fold_conv_norm(m, torch.float64), 1, 2, silu) for m in self.downsample_blocks])
+            for name in ("layer_blocks", "pan_blocks"):
+                f[name] = [(_KConv(*fold_csp_projection(layer, torch.float64), 1, 1, silu),
+                            [(_KConv(*fold_repvgg(blk, torch.float64), blk.conv1[0].groups, 1, silu), _KGate(blk.se_module))
+                             for blk in layer.bottlenecks]) for layer in getattr(self, name)]
+            return f
+        return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), build)
 
     @staticmethod
     def launches_per_forward(levels: int = 4, blocks: int = 3) -> int:

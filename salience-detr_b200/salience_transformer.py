@@ -30,7 +30,7 @@ import torch
 from torch import Tensor, nn
 from torch.nn import functional as F
 
-from . import cabi, gemm
+from . import cabi, derived, gemm
 from .channel_mapper import tokens_of
 from .ms_deform_attn import MultiScaleDeformableAttention
 
@@ -64,14 +64,10 @@ class MaskPredictor(nn.Module):
         """(W1^T, b1, W2a^T, b2a, W2b^T, b2b, w2c, b2c) with the weights in (in, out) layout, cached per parameter version
         (sdetr_mask_predictor_level streams weight rows)."""
         lins = [self.layer1[1], self.layer2[0], self.layer2[2], self.layer2[4]]
-        key = tuple((m.weight.data_ptr(), m.weight._version, m.bias.data_ptr(), m.bias._version) for m in lins)
-        if getattr(self, "_t_key", None) != key:
-            with torch.no_grad():
-                self._t = (lins[0].weight.detach().t().contiguous(), lins[0].bias.detach(), lins[1].weight.detach().t().contiguous(),
-                           lins[1].bias.detach(), lins[2].weight.detach().t().contiguous(), lins[2].bias.detach(),
-                           lins[3].weight.detach().reshape(-1).contiguous(), lins[3].bias.detach())
-            self._t_key = key
-        return self._t
+        return derived.cached(self, "transposed_weights", [t for m in lins for t in (m.weight, m.bias)], lambda: (
+            lins[0].weight.detach().t().contiguous(), lins[0].bias.detach(), lins[1].weight.detach().t().contiguous(),
+            lins[1].bias.detach(), lins[2].weight.detach().t().contiguous(), lins[2].bias.detach(),
+            lins[3].weight.detach().reshape(-1).contiguous(), lins[3].bias.detach()))
 
     def forward_fast(self, x):
         """Inference: same math; projections on the tensor cores, GELUs fused into the next GEMM's operand load,
@@ -198,25 +194,16 @@ class SalienceTransformerEncoderLayer(nn.Module):
 
     # -- inference fast path ------------------------------------------------------------------------------------
     def _mha_views(self):
-        """Stable views of in_proj_{weight,bias}: [q|k] rows and [v] rows (stable objects keep the weight-split caches warm)."""
-        w, bias = self.pre_attention.in_proj_weight, self.pre_attention.in_proj_bias
-        key = (w.data_ptr(), bias.data_ptr())
-        if getattr(self, "_mha_key", None) != key:
-            c = self.embed_dim
-            self._mha_key = key
-            self._mha = (w.detach()[:2 * c], bias.detach()[:2 * c], w.detach()[2 * c:], bias.detach()[2 * c:])
-        return self._mha
+        """Views of in_proj_{weight,bias}: [q|k] rows and [v] rows."""
+        w, bias, c = self.pre_attention.in_proj_weight, self.pre_attention.in_proj_bias, self.embed_dim
+        return derived.cached(self, "mha_views", (w, bias), lambda: (
+            w.detach()[:2 * c], bias.detach()[:2 * c], w.detach()[2 * c:], bias.detach()[2 * c:]))
 
     def _mha_transposed(self):
         """in_proj_weight^T (C,3C) and out_proj.weight^T (C,C), cached per parameter version (the fused pre-attention
         kernels stream weight rows of the (in, out) layout)."""
         w, wo = self.pre_attention.in_proj_weight, self.pre_attention.out_proj.weight
-        key = (w.data_ptr(), w._version, wo.data_ptr(), wo._version)
-        if getattr(self, "_mha_t_key", None) != key:
-            with torch.no_grad():
-                self._mha_t = (w.detach().t().contiguous(), wo.detach().t().contiguous())
-            self._mha_t_key = key
-        return self._mha_t
+        return derived.cached(self, "mha_transposed", (w, wo), lambda: (w.detach().t().contiguous(), wo.detach().t().contiguous()))
 
     def _pre_attention_fast(self, q, qp, mc, qs=None):
         """Top-k salient tokens -> MHA -> LN -> scatter (reference :366-379).  C = 256, head_dim = 32 (every reference
@@ -274,8 +261,6 @@ class SalienceTransformerEncoder(nn.Module):
         self.embed_dim = encoder_layer.embed_dim
         self.background_embedding = PositionEmbeddingLearned(max_num_embedding, num_pos_feats=self.embed_dim // 2)
         self.enhance_mcsp: Optional[nn.Module] = None  # injected by SalienceTransformer (reference :79)
-        self._vproj_key = None
-        self._vproj = None
         for layer in self.layers:
             layer.init_weights()
 
@@ -294,13 +279,9 @@ class SalienceTransformerEncoder(nn.Module):
 
     def _value_projection(self):
         """[6*C, C] weight / [6*C] bias of all layers' value_proj (rebuilt when any of them changes)."""
-        ps = [(l.self_attn.value_proj.weight, l.self_attn.value_proj.bias) for l in self.layers]
-        key = tuple((w.data_ptr(), w._version, b._version) for w, b in ps)
-        if self._vproj_key != key:
-            with torch.no_grad():
-                self._vproj = (torch.cat([w for w, _ in ps], 0).contiguous(), torch.cat([b for _, b in ps], 0).contiguous())
-            self._vproj_key = key
-        return self._vproj
+        ws = [l.self_attn.value_proj.weight for l in self.layers]
+        bs = [l.self_attn.value_proj.bias for l in self.layers]
+        return derived.cached(self, "value_projection", ws + bs, lambda: (torch.cat(ws, 0).contiguous(), torch.cat(bs, 0).contiguous()))
 
     def project_values(self, tokens: Tensor, mask_u8: Tensor) -> Tensor:
         """(b,Nv,C) value tokens -> (b,Nv,layers*C): every layer's value_proj in ONE GEMM (the value tokens never
@@ -449,13 +430,9 @@ class SalienceTransformer(nn.Module):
     # -- plan ------------------------------------------------------------------------------------------------
     def _ratios_host(self):
         """Host copies of the two ratio buffers (one device read per buffer version, not one per plan)."""
-        key = (self.level_filter_ratio.data_ptr(), self.level_filter_ratio._version, self.layer_filter_ratio.data_ptr(),
-               self.layer_filter_ratio._version)
-        if self.__dict__.get("_ratio_key") != key:
-            self.__dict__["_ratio_key"] = key
-            self.__dict__["_ratio_host"] = (self.level_filter_ratio.detach().float().cpu().numpy().copy(),
-                                            self.layer_filter_ratio.detach().float().cpu().numpy().copy())
-        return self.__dict__["_ratio_host"]
+        lv, ly = self.level_filter_ratio, self.layer_filter_ratio
+        return derived.cached(self, "ratios_host", (lv, ly), lambda: (lv.detach().float().cpu().numpy().copy(),
+                                                                       ly.detach().float().cpu().numpy().copy()))
 
     @torch.no_grad()
     def make_plan(self, multi_level_masks: Sequence[Tensor]) -> EncoderPlan:

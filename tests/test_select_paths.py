@@ -8,6 +8,8 @@ histogram (`select_path` restates the rule):
 2. bitonic merge: otherwise, when K <= 16384 (one CTA sorts all K winners in shared memory);
 3. LSD radix sorts through global memory: every other case.
 Every GPU case checks under torch.profiler that the kernels of its predicted path ran."""
+import time
+
 import numpy as np
 import pytest
 import torch
@@ -216,17 +218,27 @@ def pkg():
     return p
 
 
-def launched_kernels(fn):
-    """Names of the kernels `fn` launches.  The profiler can miss the first launch after it starts, so `fn` runs twice
-    inside the window and the union is taken."""
+def launched_kernels(fn, expect):
+    """Names of the kernels `fn` launches.  The profiler can drop launches near the edges of its window (a window of a
+    few short kernels can come back empty), but never records a launch that did not happen.  So each window is padded
+    by 20 ms at both ends, `fn` runs twice inside it, and the union over up to five windows is taken, stopping once it
+    holds every kernel of `expect`: a path that launches other kernels still shows them, one that misses a kernel of
+    `expect` still misses it."""
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        fn()
+    got = set()
+    for _ in range(5):
         torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return {k for k in KERNEL_NAMES if any(k in n for n in names)}  # no kernel name contains another
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            time.sleep(0.02)
+            fn()
+            fn()
+            torch.cuda.synchronize()
+            time.sleep(0.02)
+        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+        got |= {k for k in KERNEL_NAMES if any(k in n for n in names)}  # no kernel name contains another
+        if got >= expect:
+            break
+    return got
 
 
 def _run(pkg, case, raw, mask):
@@ -245,8 +257,9 @@ def confirm_path(pkg, case):
         starts, sizes = geometry(case)
         raw = make_scores("ties", case["b"], sizes, torch.Generator().manual_seed(0)).to(DEV)
         mask = make_mask(case).to(torch.uint8).to(DEV)
-        got = launched_kernels(lambda: _run(pkg, case, raw, mask))
-        assert got == expected_kernels(case["path"], case["order"]), (case["id"], got)
+        want = expected_kernels(case["path"], case["order"])
+        got = launched_kernels(lambda: _run(pkg, case, raw, mask), want)
+        assert got == want, (case["id"], got)
         _CONFIRMED[case["id"]] = case["path"]
     return _CONFIRMED[case["id"]]
 
@@ -306,7 +319,7 @@ def test_topk_desc_value_edges(pkg, seg, n, k):
     g = torch.Generator().manual_seed(n)
     want_kernel = {"topk_select_kernel"} if k <= 4096 else {"topk_kernel"}
     s = make_scores("ties", seg, [n], g).to(DEV)
-    assert launched_kernels(lambda: pkg.cabi.topk_desc(s, k)) == want_kernel
+    assert launched_kernels(lambda: pkg.cabi.topk_desc(s, k), want_kernel) == want_kernel
     for kind in KINDS:
         s = make_scores(kind, seg, [n], g)
         want = torch.sort(s, dim=1, descending=True, stable=True)[1][:, :k]

@@ -5,7 +5,9 @@ counts of the bench workload (salience_detr_resnet50_800_1333, bs=2), hidden 204
   python tools/bench_ffn.py [--reps 20] [--out FILE]
 
 Each call is timed alone with CUDA events after a 256 MiB L2 flush, after warm-up; medians.  TFLOP/s counts what the tensor
-cores execute: 3 fp16 products per logical product (3xFP16).  Also reports whether, on one CTA per panel (cap 1), the
+cores execute: 3 fp16 products per logical product (3xFP16).  The fused kernel keeps x and the hidden activations on chip and
+streams all of W1 and W2 (fp16 hi / lo pairs, 4 MiB at hidden 2048) from L2 once per 128-row panel; weight_bytes is that
+traffic and fused_l2_gbps its rate, to set against the L2 ceiling of tools/micro/l2_bw.cu.  Also reports whether, on one CTA per panel (cap 1), the
 fused linear2 output before LayerNorm equals the two-GEMM path's bit for bit.
 """
 import argparse
@@ -22,6 +24,7 @@ import salience_detr_b200 as pkg  # noqa: E402
 
 ROWS = (22726, 18180, 13634, 13634, 9090, 4544)
 HIDDEN = 2048
+PANEL_ROWS = 128  # rows per panel of the fused kernel (kFM in csrc/ffn_fused.cu)
 
 
 def card():
@@ -61,7 +64,7 @@ def main():
     s1, s2 = cabi.split_f16_pair(w1), cabi.split_f16_pair(w2)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     res = {"card": card(), "hidden": HIDDEN, "reps": args.reps, "shapes": []}
-    tot_f = tot_t = 0.0
+    tot_f = tot_t = tot_w = 0.0
     for rows in ROWS:
         x = torch.randn(rows, 256, generator=g).to(dev)
         y = torch.empty_like(x)
@@ -78,13 +81,16 @@ def main():
 
         t_f, t_t = timed(fused, args.reps, flush), timed(two, args.reps, flush)
         exe = 3 * 2 * 2 * rows * 256 * HIDDEN  # executed tensor-core flops: 3 products x 2 GEMMs
-        tot_f, tot_t = tot_f + t_f, tot_t + t_t
+        wbytes = -(-rows // PANEL_ROWS) * 2 * 2 * HIDDEN * 256 * 2  # per panel: W1 and W2, hi and lo, fp16
+        tot_f, tot_t, tot_w = tot_f + t_f, tot_t + t_t, tot_w + wbytes
         res["shapes"].append({"rows": rows, "fused_us": round(t_f, 1), "two_gemm_us": round(t_t, 1),
                               "fused_tflops_executed": round(exe / t_f / 1e6, 1),
-                              "two_gemm_tflops_executed": round(exe / t_t / 1e6, 1)})
+                              "two_gemm_tflops_executed": round(exe / t_t / 1e6, 1),
+                              "weight_bytes": wbytes, "fused_l2_gbps": round(wbytes / t_f / 1e3)})
         print(json.dumps(res["shapes"][-1]), flush=True)
     res["fused_us_total"], res["two_gemm_us_total"] = round(tot_f, 1), round(tot_t, 1)
     res["fused_vs_two_gemm"] = round(tot_f / tot_t, 4)
+    res["weight_bytes_total"], res["fused_l2_gbps"] = int(tot_w), round(tot_w / tot_f / 1e3)
     lib = cabi.lib()
     x = torch.randn(1000, 256, generator=g).to(dev)
     lib.sdetr_set_persistent_ctas(1)

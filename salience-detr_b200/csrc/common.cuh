@@ -61,6 +61,13 @@ int persistent_ctas();  // CTAs of a persistent one-per-SM kernel: sm_count(), o
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---- device helpers -------------------------------------------------------------------------------
+// torch.relu: a NaN propagates (as the canonical NaN; fmaxf would return the 0).  One max.NaN instruction, the cost of fmaxf.
+__device__ __forceinline__ float relu_nan(float x) {
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+    return r;
+}
+
 __device__ __forceinline__ float4 ldg_f4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
 
 // streaming (read-once) 128-bit load / store: keep L1 for the gathered value tiles
@@ -79,7 +86,14 @@ __device__ __forceinline__ void st_stream_f4(float *p, const float4 &v) {
 
 // ---- max|x| in one launch (sdetr_pow2_scale, the deterministic MSDA backward's scale) ----------------------------------
 // This thread's grid-stride share of max|x[0, n)|.  fmaxf skips NaN: `nonfinite` is set when a NaN or an infinity is seen.
-// 16-byte aligned x is read with 128-bit streaming loads, any other x element by element.
+// 16-byte aligned x is read with 128-bit streaming loads, any other x element by element.  FINITE_ONLY: infinities count
+// as 0 too (the maximum of the finite entries).
+template <bool FINITE_ONLY>
+__device__ __forceinline__ float abs_for_max(float v) {
+    const float a = fabsf(v);
+    return FINITE_ONLY && !(a <= FLT_MAX) ? 0.f : a;
+}
+template <bool FINITE_ONLY = false>
 __device__ __forceinline__ float thread_absmax(const float *__restrict__ x, int64_t n, bool &nonfinite) {
     float m = 0.f;
     bool bad = false;
@@ -88,14 +102,15 @@ __device__ __forceinline__ float thread_absmax(const float *__restrict__ x, int6
         for (int64_t i = t * 4; i < n; i += nt * 4) {
             if (i + 3 < n) {
                 const float4 v = ld_stream_f4(x + i);
-                m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+                m = fmaxf(m, fmaxf(fmaxf(abs_for_max<FINITE_ONLY>(v.x), abs_for_max<FINITE_ONLY>(v.y)),
+                                   fmaxf(abs_for_max<FINITE_ONLY>(v.z), abs_for_max<FINITE_ONLY>(v.w))));
                 bad |= !(fabsf(v.x) <= FLT_MAX) | !(fabsf(v.y) <= FLT_MAX) | !(fabsf(v.z) <= FLT_MAX) | !(fabsf(v.w) <= FLT_MAX);
             } else {
-                for (int64_t j = i; j < n; ++j) m = fmaxf(m, fabsf(x[j])), bad |= !(fabsf(x[j]) <= FLT_MAX);
+                for (int64_t j = i; j < n; ++j) m = fmaxf(m, abs_for_max<FINITE_ONLY>(x[j])), bad |= !(fabsf(x[j]) <= FLT_MAX);
             }
         }
     } else {
-        for (int64_t i = t; i < n; i += nt) m = fmaxf(m, fabsf(x[i])), bad |= !(fabsf(x[i]) <= FLT_MAX);
+        for (int64_t i = t; i < n; i += nt) m = fmaxf(m, abs_for_max<FINITE_ONLY>(x[i])), bad |= !(fabsf(x[i]) <= FLT_MAX);
     }
     nonfinite |= bad;
     return m;

@@ -161,8 +161,8 @@ __global__ void __launch_bounds__(kGThreads, 1)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int r = r0 + 8 * h;
-                    const float v0 = fmaxf(acc1[4 * j + 2 * h] * p.out1 + bb0, 0.f) * kActScale;
-                    const float v1 = fmaxf(acc1[4 * j + 2 * h + 1] * p.out1 + bb1, 0.f) * kActScale;
+                    const float v0 = relu_nan(acc1[4 * j + 2 * h] * p.out1 + bb0) * kActScale;
+                    const float v1 = relu_nan(acc1[4 * j + 2 * h + 1] * p.out1 + bb1) * kActScale;
                     uint32_t vh, vl;
                     split2(v0, v1, vh, vl);
                     const int off = r * 128 + ((j ^ (r & 7)) << 4) + 4 * q;

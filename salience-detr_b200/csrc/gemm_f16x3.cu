@@ -106,11 +106,12 @@ namespace sdetr {
 __global__ void __launch_bounds__(256) pow2_scale_kernel(const float *__restrict__ x, int64_t n, int target_log2,
                                                          unsigned int *__restrict__ state /* [0] max bits, [1] blocks done */,
                                                          float *__restrict__ scale) {
-    bool nonfinite = false;  // not needed here: NaN / inf propagate through the GEMM whatever the scale
-    float m = block_max(thread_absmax(x, n, nonfinite));
+    // the scale comes from the finite entries: a NaN or inf propagates through the GEMM whatever the scale, and an inf
+    // counted here would give a scale that flushes every finite entry to zero in fp16
+    bool nonfinite = false;
+    const float m = block_max(thread_absmax<true>(x, n, nonfinite));
     __shared__ bool last;
     if (threadIdx.x == 0) {
-        if (!(m <= 3.0e38f)) m = 3.0e38f;                 // NaN / inf: the GEMM propagates them whatever the scale
         atomicMax(state, __float_as_uint(m));             // non-negative floats order like their bit patterns
         __threadfence();
         last = atomicAdd(state + 1, 1u) == gridDim.x - 1;

@@ -400,7 +400,7 @@ __global__ void __launch_bounds__(256) split_tf32_kernel(const float *__restrict
     const int c = (int)(vec - r * kv) * 4;
     float4 v = ld_stream_f4(x + r * x_stride + c);
     if (relu == 1) {
-        v.x = fmaxf(v.x, 0.f), v.y = fmaxf(v.y, 0.f), v.z = fmaxf(v.z, 0.f), v.w = fmaxf(v.w, 0.f);
+        v.x = relu_nan(v.x), v.y = relu_nan(v.y), v.z = relu_nan(v.z), v.w = relu_nan(v.w);
     } else if (relu == 2) {  // exact (erf) GELU
         v.x = 0.5f * v.x * (1.f + erff(v.x * 0.70710678118654752f)), v.y = 0.5f * v.y * (1.f + erff(v.y * 0.70710678118654752f));
         v.z = 0.5f * v.z * (1.f + erff(v.z * 0.70710678118654752f)), v.w = 0.5f * v.w * (1.f + erff(v.w * 0.70710678118654752f));

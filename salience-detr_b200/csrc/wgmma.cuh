@@ -145,9 +145,14 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t &hi, uint32_
     hi = *reinterpret_cast<const uint32_t *>(&h);
     lo = *reinterpret_cast<const uint32_t *>(&l);
 }
-__device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
+// round to the nearest TF32 value, ties away from zero; NaN and inf pass unchanged (the carry of the rounding add would
+// run a NaN's high mantissa bits through the exponent into the sign: 0x7fffffff would become -0)
+__device__ __forceinline__ float tf32_rn(float x) {
+    const uint32_t u = __float_as_uint(x);
+    return (u & 0x7f800000u) == 0x7f800000u ? x : __uint_as_float((u + 0x1000u) & 0xffffe000u);
+}
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
-__device__ __forceinline__ float apply_act(float x, int act) { return act == 1 ? fmaxf(x, 0.f) : act == 2 ? gelu_erf(x) : x; }
+__device__ __forceinline__ float apply_act(float x, int act) { return act == 1 ? relu_nan(x) : act == 2 ? gelu_erf(x) : x; }
 
 // element (r, c) of a 128-row x 32-fp32 box written by TMA with SWIZZLE_128B (16-byte chunk index XOR row % 8)
 __device__ __forceinline__ const float *swz_f32(const uint8_t *box, int r, int c) {

@@ -70,28 +70,49 @@ def _act_torch(x: Tensor, act) -> Tensor:
     return F.relu(x) if act == 1 else F.gelu(x) if act == 2 else x
 
 
+def _native(x: Tensor, weight: Tensor, bias: Optional[Tensor]) -> bool:
+    """Operands the project's kernels take: fp32 CUDA tensors on the current device (any layout), a 2-D weight, at least
+    one row.  Everything else F.linear accepts (other dtypes, CPU tensors, empty inputs) goes to F.linear."""
+    return (x.is_cuda and weight.is_cuda and x.dtype == torch.float32 and weight.dtype == torch.float32 and
+            weight.dim() == 2 and x.numel() > 0 and x.device == weight.device and x.device.index == cabi._current_device()
+            and (bias is None or (bias.is_cuda and bias.dtype == torch.float32 and bias.device == x.device)))
+
+
+def _rows(x: Tensor) -> Tensor:
+    """x (..., K) as the (rows, K) operand the kernels read in place -- unit last stride, one row pitch that is a multiple
+    of 4 floats, a 16-byte aligned base -- or, for any other layout F.linear accepts (transposed, odd pitch, an offset
+    view, non-uniform batch strides), an aligned contiguous copy of it."""
+    x2 = x if x.dim() == 2 else x.reshape(-1, x.shape[-1])  # a fresh contiguous copy when the rows are not uniformly strided
+    if x2.data_ptr() != x.data_ptr() or (x2.stride(-1) == 1 and (x2.stride(0) % 4 == 0 or x2.shape[0] == 1) and
+                                         x2.data_ptr() % 16 == 0):
+        return x2
+    return x2.clone(memory_format=torch.contiguous_format)
+
+
 def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input: bool = False,
            input_act: Optional[str] = None) -> Tensor:
-    """y = act(x) @ weight.T + bias (act: None | "relu" | "gelu", fused into the operand load / split), inference only."""
+    """y = act(x) @ weight.T + bias (act: None | "relu" | "gelu", fused into the operand load / split), inference only.
+    A drop-in for F.linear: any input it accepts works (see ``_native`` and ``_rows``)."""
     relu_input = 1 if relu_input else _ACT[input_act]
-    n, k = weight.shape
-    if MODE == "auto" and x.numel() // max(k, 1) <= SMALL_M:
+    n, k = weight.shape[0], weight.shape[-1]
+    if (MODE == "auto" and x.numel() // max(k, 1) <= SMALL_M) or not _native(x, weight, bias):
         return F.linear(_act_torch(x, relu_input), weight, bias)
+    bias = bias if bias is None or bias.is_contiguous() else bias.contiguous()
     own = MODE in ("tcgen05", "auto")
-    if own and k % 32 == 0 and x.stride(-1) == 1:
-        x2 = x if x.dim() == 2 else x.reshape(-1, x.shape[-1])
-        if x2.stride(0) % 4 == 0 or x2.shape[0] == 1:
-            if k >= 1024 and LONG_K_PRESPLIT:   # long reductions: 4-stage ring, weight pre-split once (variant "SS")
-                w_hi, w_lo = split_weight_pair(weight)
-                return cabi.gemm_3xtf32(x, w_hi, w_lo, bias, relu_input)
-            if OWN_KERNEL == "f16x3" and MODE == "auto" and k % 64 == 0:
-                w_hi, w_lo, w_scale = split_weight_f16(weight)
-                return cabi.gemm_f16x3_pre(x, w_hi, w_lo, w_scale, bias, relu_input)
-            if PRESPLIT_PERSISTENT:
-                w_hi, w_lo = split_weight_pair(weight)
-                return cabi.gemm_3xtf32_pre(x, w_hi, w_lo, bias, relu_input)
-            # both operands split in the kernel
-            return cabi.gemm_3xtf32_raw(x, weight if weight.is_contiguous() else weight.contiguous(), bias, relu_input)
+    if own and k % 32 == 0:
+        x2 = _rows(x)
+        if k >= 1024 and LONG_K_PRESPLIT:   # long reductions: 4-stage ring, weight pre-split once (variant "SS")
+            w_hi, w_lo = split_weight_pair(weight)
+            y = cabi.gemm_3xtf32(x2, w_hi, w_lo, bias, relu_input)
+        elif OWN_KERNEL == "f16x3" and MODE == "auto" and k % 64 == 0:
+            w_hi, w_lo, w_scale = split_weight_f16(weight)
+            y = cabi.gemm_f16x3_pre(x2, w_hi, w_lo, w_scale, bias, relu_input)
+        elif PRESPLIT_PERSISTENT:
+            w_hi, w_lo = split_weight_pair(weight)
+            y = cabi.gemm_3xtf32_pre(x2, w_hi, w_lo, bias, relu_input)
+        else:  # both operands split in the kernel
+            y = cabi.gemm_3xtf32_raw(x2, weight if weight.is_contiguous() else weight.contiguous(), bias, relu_input)
+        return y.reshape(*x.shape[:-1], n)
     if MODE == "fp32" or k % 4 != 0:
         return F.linear(_act_torch(x, relu_input), weight, bias)
     if MODE == "tf32":
@@ -99,7 +120,7 @@ def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input:
             return F.linear(_act_torch(x, relu_input), weight, bias)
     K = weight.shape[1]
     kc = _chunk_of(K)  # (MODE "3xtf32", or "tcgen05" falling back for an unsupported shape)
-    x3 = cabi.split_tf32(x, layout_b=False, relu=relu_input, chunk=kc)
+    x3 = cabi.split_tf32(_rows(x), layout_b=False, relu=relu_input, chunk=kc)
     w3 = split_weight(weight)
     with _tf32_matmul():
         if kc == K:
@@ -146,8 +167,7 @@ class _LinearF16x3(torch.autograd.Function):
         c16 = _const16.get(x.device.index)
         if c16 is None:
             c16 = _const16[x.device.index] = torch.full((1,), 16.0, device=x.device)
-        x2 = x if x.stride(-1) == 1 else x.contiguous()
-        y = cabi.gemm_f16x3_scaled(x2, c16, w_hi, w_lo, w_scale, bias)
+        y = cabi.gemm_f16x3_scaled(_rows(x).view(x.shape), c16, w_hi, w_lo, w_scale, bias)
         ctx.save_for_backward(x, weight)
         ctx.has_bias = bias is not None
         return y
@@ -156,7 +176,8 @@ class _LinearF16x3(torch.autograd.Function):
     def backward(ctx, dy):
         x, weight = ctx.saved_tensors
         dy2 = dy.reshape(-1, dy.shape[-1])
-        dy2 = dy2 if dy2.is_contiguous() else dy2.contiguous()
+        if not (dy2.is_contiguous() and dy2.data_ptr() % 16 == 0):  # pow2_scale and the kernel read it as one aligned block
+            dy2 = dy2.clone(memory_format=torch.contiguous_format)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             bwd = ctx.bwd
@@ -173,11 +194,11 @@ class _LinearF16x3(torch.autograd.Function):
 
 def linear_train(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None) -> Tensor:
     """Differentiable ``F.linear`` for the training path: tensor cores where the shapes allow (K % 64 == 0, more than SMALL_M
-    rows, fp32 CUDA), ``F.linear`` otherwise."""
+    rows, fp32 CUDA on the current device, any layout), ``F.linear`` otherwise."""
     rows = x.numel() // max(x.shape[-1], 1)
-    if (TRAIN_TENSOR_CORE and MODE == "auto" and OWN_KERNEL == "f16x3" and x.is_cuda and x.dtype == torch.float32 and
-            weight.dtype == torch.float32 and x.shape[-1] % 64 == 0 and rows > SMALL_M and weight.dim() == 2):
-        return _LinearF16x3.apply(x, weight, bias)
+    if (TRAIN_TENSOR_CORE and MODE == "auto" and OWN_KERNEL == "f16x3" and _native(x, weight, bias) and
+            x.shape[-1] % 64 == 0 and rows > SMALL_M):
+        return _LinearF16x3.apply(x, weight, bias if bias is None or bias.is_contiguous() else bias.contiguous())
     return _orig_linear(x, weight, bias)
 
 

@@ -614,6 +614,29 @@ int sdetr_cdn_queries_backward(const float *grad_label_queries, const int32_t *n
  * One launch (none when P == 0). */
 int sdetr_cdn_loss_indices(const int32_t *num_gt_host, int num_images, int groups, int max_gt, int64_t *indices,
                            sdetr_stream_t stream);
+
+/* ---- Detection post-processing: PostProcess.forward (models/bricks/post_process.py:21-74) ------------------------------------
+ * pred_logits (b, Q, K) fp32: element (i, q, c) at i * logits_batch_stride + q * logits_query_stride + c (a query slice such as
+ * dn_post_process's outputs_class[:, :, pad:, :] needs no copy); pred_boxes (b, Q, 4) cxcywh fp32 likewise with unit coordinate
+ * stride; target_sizes (b, 2) contiguous (h, w) of dtype sizes_dtype (SDETR_SIZES_*).  Per image, in one CTA:
+ *   scores (b, k) fp32: the k largest p = sigmoid(logit) (bit-identical to torch.sigmoid on CUDA) over the Q * K flat indices,
+ *     ordered by p descending, ties by smaller flat index, NaN first (= torch.sort(p, descending=True, stable=True)[:k]);
+ *   labels (b, k) int64: flat index % K;  boxes (b, k, 4) fp32: the box of query flat index / K as
+ *     (cx - 0.5 w, cy - 0.5 h, cx + 0.5 w, cy + 0.5 h) * (img_w, img_h, img_w, img_h), every operation rounded separately.
+ * A filter is on when its threshold is > 0.  Then entry j is kept iff (confidence off or score > confidence_score) and (NMS off
+ * or no kept entry ranked before j has IoU > iou_threshold with it: greedy NMS over all k boxes in this order, torchvision's
+ * IoU); the kept entries are compacted to the front of each image's row in order and count (b) int32 holds how many.  Rows
+ * past count are left unwritten.  With both filters off count may be NULL (else it receives k).
+ * 1 <= k <= min(Q * K, SDETR_POSTPROCESS_MAX_K) (a larger k: SDETR_ERR_UNSUPPORTED), Q * K < 2^31.  workspace:
+ * sdetr_postprocess_workspace(b, Q, K) bytes.  One launch, no synchronisation. */
+#define SDETR_POSTPROCESS_MAX_K 4096
+enum { SDETR_SIZES_INT64 = 0, SDETR_SIZES_INT32 = 1, SDETR_SIZES_FLOAT32 = 2 };
+size_t sdetr_postprocess_workspace(int batch, int num_queries, int num_classes);
+int sdetr_postprocess(const float *pred_logits, int64_t logits_batch_stride, int64_t logits_query_stride, const float *pred_boxes,
+                      int64_t boxes_batch_stride, int64_t boxes_query_stride, const void *target_sizes, int sizes_dtype, int batch,
+                      int num_queries, int num_classes, int k, float confidence_score, float iou_threshold, float *scores,
+                      int64_t *labels, float *boxes, int32_t *count, void *workspace, size_t workspace_bytes,
+                      sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,7 @@ from .position_encoding import PositionEmbeddingSine  # noqa: F401
 from .criterion import SalienceCriterion, load_reference_checkpoint, sigmoid_focal_loss  # noqa: F401
 from .set_criterion import HungarianMatcher, HybridSetCriterion  # noqa: F401
 from .denoising import GenerateCDNQueries, compute_dn_loss  # noqa: F401
+from .postprocess import PostProcess  # noqa: F401
 from .decoder import (  # noqa: F401
     MLP,
     SalienceTransformerDecoder,

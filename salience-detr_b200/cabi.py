@@ -103,6 +103,8 @@ SIGNATURES = {
     "sdetr_cdn_queries": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp] + [_i] * 7 + [_vp] * 6),
     "sdetr_cdn_queries_backward": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "sdetr_cdn_loss_indices": (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    "sdetr_postprocess_workspace": (_sz, [_i, _i, _i]),
+    "sdetr_postprocess": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp] + [_i] * 5 + [_f, _f] + [_vp] * 5 + [_sz, _vp]),
 }
 
 
@@ -1177,3 +1179,53 @@ def cdn_loss_indices(counts: Sequence[int], groups: int, max_gt: int, device):
     _check(lib().sdetr_cdn_loss_indices(_host_i32(counts) if counts else None, len(counts), int(groups), int(max_gt),
                                         out.data_ptr() if out.numel() else None, _stream()), "sdetr_cdn_loss_indices")
     return out
+
+
+# ---- detection post-processing (postprocess.cu) -------------------------------------------------------------------------------
+POSTPROCESS_MAX_K = 4096  # include/sdetr_b200.h SDETR_POSTPROCESS_MAX_K
+_SIZES_DTYPES = {torch.int64: 0, torch.int32: 1, torch.float32: 2}  # SDETR_SIZES_*
+
+
+def _strided(t, name, dtype):
+    """The checks of _req but for a unit last stride instead of contiguity (a copy when the last stride is not 1)."""
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor")
+    if t.stride(-1) != 1:
+        t = t.contiguous()
+    _req(t.as_strided((1,), (1,)) if t.numel() else t, name, dtype)  # device and dtype, on a one-element view
+    return t
+
+
+def postprocess(logits, boxes, target_sizes, k: int, confidence_score: float, iou_threshold: float):
+    """logits (b, Q, K) fp32 and boxes (b, Q, 4) cxcywh fp32 with any batch / query strides, target_sizes (b, 2) (h, w) int64,
+    int32 or float32 -> (scores (b, k) fp32, labels (b, k) int64, boxes (b, k, 4) fp32, count (b,) int32 or None).  A threshold
+    > 0 turns its filter on; then the first count[i] entries of row i are its kept ones, else count is None."""
+    logits = _strided(logits, "pred_logits", torch.float32)
+    boxes = _strided(boxes, "pred_boxes", torch.float32)
+    if target_sizes.dtype not in _SIZES_DTYPES:
+        raise RuntimeError(f"target_sizes must be int64, int32 or float32, got {target_sizes.dtype}")
+    sizes = _strided(target_sizes, "target_sizes", target_sizes.dtype).contiguous()
+    b, Q, K = logits.shape
+    if tuple(boxes.shape) != (b, Q, 4):
+        raise RuntimeError(f"pred_boxes must be ({b}, {Q}, 4), got {tuple(boxes.shape)}")
+    if not 0 <= k <= Q * K:
+        raise RuntimeError(f"selected index k out of range: k={k}, {Q * K} scores per image")
+    if k > POSTPROCESS_MAX_K:
+        raise RuntimeError(f"k={k}: the post-processing kernel selects at most {POSTPROCESS_MAX_K} boxes per image")
+    filters = confidence_score > 0 or iou_threshold > 0
+    dev = logits.device
+    scores = torch.empty(b, k, device=dev, dtype=torch.float32)
+    labels = torch.empty(b, k, device=dev, dtype=torch.int64)
+    out_boxes = torch.empty(b, k, 4, device=dev, dtype=torch.float32)
+    count = torch.empty(b, device=dev, dtype=torch.int32) if filters else None
+    if b == 0 or k == 0:  # nothing to select (torch.topk with k = 0 returns empty rows)
+        if count is not None:
+            count.zero_()
+        return scores, labels, out_boxes, count
+    ws = torch.empty(lib().sdetr_postprocess_workspace(b, Q, K), device=dev, dtype=torch.uint8)
+    _check(lib().sdetr_postprocess(logits.data_ptr(), logits.stride(0), logits.stride(1), boxes.data_ptr(), boxes.stride(0),
+                                   boxes.stride(1), sizes.data_ptr(), _SIZES_DTYPES[sizes.dtype], b, Q, K, int(k),
+                                   float(confidence_score), float(iou_threshold), scores.data_ptr(), labels.data_ptr(),
+                                   out_boxes.data_ptr(), count.data_ptr() if count is not None else None, ws.data_ptr(),
+                                   ws.numel(), _stream()), "sdetr_postprocess")
+    return scores, labels, out_boxes, count

@@ -447,6 +447,15 @@ int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *W1_hi, co
 int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin, const float *a_scale_dev,
                        const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, int Cout, int groups,
                        int ksize, int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
+/* y = act(conv(x, W) + bias + z): sdetr_conv2d_f16x3 with a residual operand z (token rows, Cout wide; NULL: none) added
+ * before the activation, and act 0 none, 1 ReLU (NaN propagates, as torch.relu), 3 SiLU.  z, z_pitch, ldz 8-byte aligned; z may
+ * alias y (each element is read before it is written, by the same thread).  sdetr_conv2d_f16x3 is this call with z = NULL (and
+ * act 0 or 3): same k-block order and epilogue arithmetic, the same bits.  A Bottleneck's conv3 -> bn3 -> += identity -> ReLU
+ * is one call. */
+int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin, const float *a_scale_dev,
+                          const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, const float *z,
+                          int64_t z_pitch, int64_t ldz, int Cout, int groups, int ksize, int stride, int act, float *y,
+                          int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
 /* Context gate of a RepVggPluXBlock (SqueezeAndExcitation, models/bricks/basic.py:29-54, plus the block's residual), per image
  * of HW pixels: p = softmax over the pixels of (y . w_mask + *b_mask); ctx = sum p y; gate = sigmoid(W2 ReLU(W1 ctx)) with
  * w1 (R, C), w2 (C, R) row-major; out = gate * y + x (+ z when z is not NULL).  Three launches; every reduction is summed in a
@@ -637,6 +646,19 @@ int sdetr_postprocess(const float *pred_logits, int64_t logits_batch_stride, int
                       int num_queries, int num_classes, int k, float confidence_score, float iou_threshold, float *scores,
                       int64_t *labels, float *boxes, int32_t *count, void *workspace, size_t workspace_bytes,
                       sdetr_stream_t stream);
+/* ---- ResNet backbone in token layout (models/backbones/resnet.py; ResNetBackbone.forward_tokens) ---------------------------
+ * The stem: y = ReLU(conv(x, W) + bias), conv 7x7, stride 2, padding 3, 3 -> 64 channels.  x: the (batch, 3, H, W) NCHW
+ * contiguous fp32 image batch; weight (147, 64) = W[co, c, ky, kx] at row (c * 7 + ky) * 7 + kx, column co (the folded
+ * FrozenBatchNorm scale already in it); bias (64); y: (batch, Ho * Wo, 64) contiguous token rows, Ho = (H + 6 - 7) / 2 + 1,
+ * likewise Wo.  fp32 FMAs, taps summed in (c, ky, kx) order; NaN propagates through the ReLU.  weight, bias, y 16-byte
+ * aligned.  One launch. */
+int sdetr_resnet_stem(const float *x, int batch, int H, int W, const float *weight, const float *bias, float *y,
+                      sdetr_stream_t stream);
+/* 3x3, stride 2, padding 1 max-pool on token rows (H x W, C channels) -> (Ho x Wo) with Ho = (H + 2 - 3) / 2 + 1, likewise Wo
+ * (torch's max_pool2d, ceil_mode off).  Padding acts as -inf; a NaN in a window gives NaN.  C % 4 == 0; operands, pitches and
+ * row strides 16-byte aligned.  One launch. */
+int sdetr_maxpool3x3s2_tokens(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int C, float *y,
+                              int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -105,6 +105,10 @@ SIGNATURES = {
     "sdetr_cdn_loss_indices": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "sdetr_postprocess_workspace": (_sz, [_i, _i, _i]),
     "sdetr_postprocess": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp] + [_i] * 5 + [_f, _f] + [_vp] * 5 + [_sz, _vp]),
+    "sdetr_conv2d_f16x3_ex": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i, _i, _i, _i, _i, _vp,
+                                   _i64, _i64, _vp]),
+    "sdetr_resnet_stem": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "sdetr_maxpool3x3s2_tokens": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
 }
 
 
@@ -887,12 +891,13 @@ def _token_rows(t, name):
     return t.data_ptr(), t.stride(0), t.stride(1)
 
 
-ACT_SILU = 3
+ACT_RELU, ACT_SILU = 1, 3
 
 
-def conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, w_scale, bias, groups: int, ksize: int, stride: int, act: int = 0, out=None):
-    """y = act(conv2d(x, W) + bias) on token rows.  x: (b, H*W, Cin) view (e.g. a level slice of the encoder memory), hw = (H, W);
+def conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, w_scale, bias, groups: int, ksize: int, stride: int, act: int = 0, out=None, z=None):
+    """y = act(conv2d(x, W) + bias (+ z)) on token rows.  x: (b, H*W, Cin) view (e.g. a level slice of the encoder memory), hw = (H, W);
     W given as the (Cout, k, k, Cin / groups) pair of split_f16_pair_dev and its device scale; a_scale: pow2_scale of x (target 12).
+    act: 0, ACT_RELU or ACT_SILU.  z: optional (b, Ho*Wo, Cout) residual view, may be ``out`` itself.
     out: optional (b, Ho*Wo, Cout) view to write; returns it (or a new contiguous tensor)."""
     H, W = hw
     b, hw_in, cin = x.shape
@@ -904,14 +909,17 @@ def conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, w_scale, bias, groups: int, ksize: 
     y = out if out is not None else torch.empty(b, ho * wo, cout, device=x.device, dtype=torch.float32)
     if tuple(y.shape) != (b, ho * wo, cout):
         raise RuntimeError(f"conv2d_f16x3: out must be ({b}, {ho * wo}, {cout})")
+    if z is not None and tuple(z.shape) != (b, ho * wo, cout):
+        raise RuntimeError(f"conv2d_f16x3: z must be ({b}, {ho * wo}, {cout})")
     xp, xpitch, ldx = _token_rows(x, "x")
     yp, ypitch, ldy = _token_rows(y, "out")
-    rc = lib().sdetr_conv2d_f16x3(xp, xpitch, ldx, b, H, W, cin, _req(a_scale, "a_scale", torch.float32),
-                                  _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
-                                  _req(w_scale, "w_scale", torch.float32),
-                                  _req(bias, "bias", torch.float32) if bias is not None else None, cout, int(groups), int(ksize),
-                                  int(stride), int(act), yp, ypitch, ldy, _stream())
-    _check(rc, "sdetr_conv2d_f16x3")
+    zp = _token_rows(z, "z") if z is not None else (None, 0, 0)
+    rc = lib().sdetr_conv2d_f16x3_ex(xp, xpitch, ldx, b, H, W, cin, _req(a_scale, "a_scale", torch.float32),
+                                     _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
+                                     _req(w_scale, "w_scale", torch.float32),
+                                     _req(bias, "bias", torch.float32) if bias is not None else None, *zp, cout, int(groups),
+                                     int(ksize), int(stride), int(act), yp, ypitch, ldy, _stream())
+    _check(rc, "sdetr_conv2d_f16x3_ex")
     return y
 
 
@@ -1229,3 +1237,35 @@ def postprocess(logits, boxes, target_sizes, k: int, confidence_score: float, io
                                    out_boxes.data_ptr(), count.data_ptr() if count is not None else None, ws.data_ptr(),
                                    ws.numel(), _stream()), "sdetr_postprocess")
     return scores, labels, out_boxes, count
+
+
+# ---- ResNet backbone in token layout (backbone.ResNetBackbone.forward_tokens) ------------------------------------------------
+def resnet_stem(x, weight, bias):
+    """ReLU(conv 7x7 / 2, padding 3 (x) + bias) -> (b, Ho*Wo, 64) token rows.  x: (b, 3, H, W) NCHW contiguous fp32 CUDA;
+    weight: (147, 64) = the folded (64, 3, 7, 7) weight as W.reshape(64, 147).T, contiguous; bias (64)."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.is_contiguous()):
+        raise RuntimeError("resnet_stem: x must be a contiguous CUDA float32 (b, 3, H, W) tensor")
+    b, _, H, W = x.shape
+    if tuple(weight.shape) != (147, 64) or tuple(bias.shape) != (64,):
+        raise RuntimeError("resnet_stem: weight must be (147, 64) and bias (64)")
+    ho, wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    y = torch.empty(b, ho * wo, 64, device=x.device, dtype=torch.float32)
+    rc = lib().sdetr_resnet_stem(_req(x, "x", torch.float32), b, H, W, _req(weight, "weight", torch.float32),
+                                 _req(bias, "bias", torch.float32), y.data_ptr(), _stream())
+    _check(rc, "sdetr_resnet_stem")
+    return y
+
+
+def maxpool3x3s2_tokens(x, hw, out=None):
+    """3x3 / stride 2 / padding 1 max-pool (torch's max_pool2d) of (b, H*W, C) token rows, hw = (H, W) -> (b, Ho*Wo, C)."""
+    b, n, c = x.shape
+    H, W = hw
+    if n != H * W:
+        raise RuntimeError(f"maxpool3x3s2_tokens: x has {n} rows per image, the map is {H}x{W}")
+    ho, wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    y = out if out is not None else torch.empty(b, ho * wo, c, device=x.device, dtype=torch.float32)
+    if tuple(y.shape) != (b, ho * wo, c):
+        raise RuntimeError(f"maxpool3x3s2_tokens: out must be ({b}, {ho * wo}, {c})")
+    rc = lib().sdetr_maxpool3x3s2_tokens(*_token_rows(x, "x"), b, int(H), int(W), c, *_token_rows(y, "out"), _stream())
+    _check(rc, "sdetr_maxpool3x3s2_tokens")
+    return y

@@ -1,8 +1,8 @@
 // RepVGG-PluX neck in token layout (models/necks/repnet.py:125-245): the three kernels behind
 // RepVGGPluXNetwork.forward_tokens.
 //
-//   sdetr_conv2d_f16x3            implicit-GEMM convolution (k = 1 or 3, stride 1 or 2, padding k / 2, groups), bias and
-//                                 none / SiLU epilogue.  Same 3xFP16 arithmetic as sdetr_gemm_f16x3_scaled: the activation is
+//   sdetr_conv2d_f16x3(_ex)       implicit-GEMM convolution (k = 1 or 3, stride 1 or 2, padding k / 2, groups), bias, optional
+//                                 residual operand and none / ReLU / SiLU epilogue.  Same 3xFP16 arithmetic as sdetr_gemm_f16x3_scaled: the activation is
 //                                 multiplied by a power-of-two device scalar, split into fp16 hi / lo in registers and used as
 //                                 the wgmma A operand; the weight arrives as a pre-split pair (scale 2^s, also a device scalar);
 //                                 lo.hi + hi.lo + hi.hi per 16-wide k step, and every 64-wide k-block's tensor-core sum is added
@@ -30,13 +30,15 @@ constexpr int kCvABytes = kCvM * kCvK * 4;  // 16 KB: fp32 activation rows of 25
 constexpr int kCvBBytes = kCvN * kCvK * 2;  // 8 KB: one of W_hi / W_lo, rows of 128 bytes
 constexpr int kCvStageBytes = kCvABytes + 2 * kCvBBytes;
 constexpr int kCvSmem = kCvStages * kCvStageBytes + 1024 /* alignment */;
-constexpr int kActSiLU = 3;  // act code of the convolution's epilogue (0 none)
+constexpr int kActReLU = 1, kActSiLU = 3;  // act codes of the convolution's epilogue (0 none)
 
 struct ConvParams {
     const float *x;
     int64_t x_pitch, ldx;
     const __half *w_hi, *w_lo;  // (Cout, k, k, Cin / groups) row-major
     const float *a_scale, *w_scale, *bias;
+    const float *z;  // residual added before the activation (NULL: none); may alias y
+    int64_t z_pitch, ldz;
     float *y;
     int64_t y_pitch, ldy;
     int H, W, Ho, Wo, M, cin_g, cout_g, ksize, stride, act;
@@ -148,12 +150,19 @@ __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams
         if (m >= p.M) continue;
         const int n = m / hwo, pix = m - n * hwo;
         float *dst = p.y + (int64_t)n * p.y_pitch + (int64_t)pix * p.ldy + n0;
+        // z is read by the thread that then writes the same two floats of y, so z may alias y
+        const float *zr = p.z ? p.z + (int64_t)n * p.z_pitch + (int64_t)pix * p.ldz + n0 : nullptr;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int col = 8 * j + 2 * q;
             float v0 = acc[4 * j + 2 * h] * out_scale + (p.bias ? __ldg(p.bias + n0 + col) : 0.f);
             float v1 = acc[4 * j + 2 * h + 1] * out_scale + (p.bias ? __ldg(p.bias + n0 + col + 1) : 0.f);
+            if (zr) {
+                const float2 r = *reinterpret_cast<const float2 *>(zr + col);
+                v0 += r.x, v1 += r.y;
+            }
             if (p.act == kActSiLU) v0 = silu(v0), v1 = silu(v1);
+            else if (p.act == kActReLU) v0 = relu_nan(v0), v1 = relu_nan(v1);
             *reinterpret_cast<float2 *>(dst + col) = make_float2(v0, v1);
         }
     }
@@ -507,15 +516,15 @@ inline int elementwise_blocks(int64_t total) {
 
 using namespace sdetr;
 
-extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
-                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
-                                  const float *bias, int Cout, int groups, int ksize, int stride, int act, float *y,
-                                  int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
+extern "C" int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
+                                     const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
+                                     const float *bias, const float *z, int64_t z_pitch, int64_t ldz, int Cout, int groups,
+                                     int ksize, int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
     SDETR_REQUIRE(x && a_scale_dev && W_hi && W_lo && w_scale_dev && y, SDETR_ERR_INVALID_ARG, "conv2d_f16x3: null pointer");
     SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
                   "conv2d_f16x3: bad sizes");
-    SDETR_REQUIRE((ksize == 1 || ksize == 3) && (stride == 1 || stride == 2) && (act == 0 || act == kActSiLU),
-                  SDETR_ERR_UNSUPPORTED, "conv2d_f16x3: takes kernel 1 or 3, stride 1 or 2, act 0 (none) or 3 (SiLU)");
+    SDETR_REQUIRE((ksize == 1 || ksize == 3) && (stride == 1 || stride == 2) && (act == 0 || act == kActReLU || act == kActSiLU),
+                  SDETR_ERR_UNSUPPORTED, "conv2d_f16x3: takes kernel 1 or 3, stride 1 or 2, act 0 (none), 1 (ReLU) or 3 (SiLU)");
     SDETR_REQUIRE(Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kCvK == 0 && (Cout / groups) % kCvN == 0,
                   SDETR_ERR_UNSUPPORTED, "conv2d_f16x3: Cin/groups=%d and Cout/groups=%d must be multiples of 64",
                   Cin / groups, Cout / groups);
@@ -523,6 +532,8 @@ extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, 
                   "conv2d_f16x3: x, its pitch and row stride and the weights must be 16-byte aligned");
     SDETR_REQUIRE((reinterpret_cast<uintptr_t>(y) & 7) == 0 && y_pitch % 2 == 0 && ldy % 2 == 0 && ldy >= Cout,
                   SDETR_ERR_INVALID_ARG, "conv2d_f16x3: y, its pitch and row stride must be 8-byte aligned");
+    SDETR_REQUIRE(!z || ((reinterpret_cast<uintptr_t>(z) & 7) == 0 && z_pitch % 2 == 0 && ldz % 2 == 0 && ldz >= Cout),
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3: z, its pitch and row stride must be 8-byte aligned");
     const int pad = ksize / 2, Ho = H > 0 ? (H + 2 * pad - ksize) / stride + 1 : 0, Wo = W > 0 ? (W + 2 * pad - ksize) / stride + 1 : 0;
     const int64_t M = (int64_t)batch * Ho * Wo;
     SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3: too many output pixels");
@@ -530,10 +541,21 @@ extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, 
     static PerDeviceOnce once;
     SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<false>, kCvSmem, "conv2d_f16x3");
     const ConvParams p{x, x_pitch, ldx, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
-                       w_scale_dev, bias, y, y_pitch, ldy, H, W, Ho, Wo, (int)M, Cin / groups, Cout / groups, ksize, stride, act};
+                       w_scale_dev, bias, z, z_pitch, ldz, y, y_pitch, ldy, H, W, Ho, Wo, (int)M, Cin / groups, Cout / groups,
+                       ksize, stride, act};
     const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
     conv_f16x3_kernel<false><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
     return check_launch("conv2d_f16x3");
+}
+
+extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
+                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
+                                  const float *bias, int Cout, int groups, int ksize, int stride, int act, float *y,
+                                  int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
+    SDETR_REQUIRE(act == 0 || act == kActSiLU, SDETR_ERR_UNSUPPORTED,
+                  "conv2d_f16x3: takes kernel 1 or 3, stride 1 or 2, act 0 (none) or 3 (SiLU)");
+    return sdetr_conv2d_f16x3_ex(x, x_pitch, ldx, batch, H, W, Cin, a_scale_dev, W_hi, W_lo, w_scale_dev, bias, nullptr, 0, 0, Cout,
+                                 groups, ksize, stride, act, y, y_pitch, ldy, stream);
 }
 
 extern "C" int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
@@ -561,7 +583,7 @@ extern "C" int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, 
     static PerDeviceOnce once;
     SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<true>, kCvSmem, "conv2d_f16x3_transposed");
     const ConvParams p{dy, dy_pitch, lddy, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
-                       w_scale_dev, nullptr, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups, Cout / groups, ksize, 2, 0};
+                       w_scale_dev, nullptr, nullptr, 0, 0, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups, Cout / groups, ksize, 2, 0};
     const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
     conv_f16x3_kernel<true><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
     return check_launch("conv2d_f16x3_transposed");

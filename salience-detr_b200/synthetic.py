@@ -8,7 +8,8 @@ configs/salience_detr/salience_detr_resnet50_800_1333.py:32)."""
 from __future__ import annotations
 
 import math
-from typing import List, Sequence, Tuple
+from collections import OrderedDict
+from typing import List, Mapping, Sequence, Tuple
 
 import torch
 from torch.nn import functional as F
@@ -20,6 +21,28 @@ CONFIGS = {
     "resnet50_800_1333_bs2_ragged": ([(800, 1333), (640, 1000)], (800, 1344), (8, 16, 32, 64)),
     "resnet50_5scale_bs2": ([(800, 1333)] * 2, (800, 1344), (4, 8, 16, 32)),      # stress: Nv = 89 250
 }
+
+
+def resnet_weights(shapes: Mapping[str, Sequence[int]], seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for a ResNet state dict of the given key -> shape table (in its order): convolutions N(0, 2 / fan_in)
+    (He scale), FrozenBatchNorm buffers away from the identity -- weight 1 + U(-0.25, 0.25), bias and running_mean N(0, 0.1^2),
+    running_var U(0.5, 2) -- so that folding them into the convolutions is exercised."""
+    g = torch.Generator().manual_seed(seed)
+    out = OrderedDict()
+    for k, shape in shapes.items():
+        shape = tuple(int(v) for v in shape)
+        if len(shape) == 4:
+            t = torch.randn(shape, generator=g) * math.sqrt(2.0 / (shape[1] * shape[2] * shape[3]))
+        elif k.endswith("running_var"):
+            t = torch.rand(shape, generator=g) * 1.5 + 0.5
+        elif k.endswith("running_mean") or k.endswith("bias"):
+            t = torch.randn(shape, generator=g) * 0.1
+        elif k.endswith("weight"):
+            t = 1.0 + (torch.rand(shape, generator=g) - 0.5) * 0.5
+        else:
+            raise ValueError(f"resnet_weights: no rule for {k} {shape}")
+        out[k] = t
+    return out
 
 
 def level_shapes(h: int, w: int, strides: Sequence[int]) -> List[Tuple[int, int]]:

@@ -500,6 +500,24 @@ int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, co
                              int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin, int Cout,
                              int groups, int ksize, int stride, float *workspace, int64_t workspace_floats, float *dw,
                              sdetr_stream_t stream);
+/* sdetr_conv2d_f16x3_wgrad with every output row co multiplied by cout_scale[co] (Cout floats; NULL: none) in the split sum's
+ * write: one fp32 product of the same sum, so the result is cout_scale[co] times sdetr_conv2d_f16x3_wgrad's, bit for bit.  The
+ * gradient of a convolution weight W whose forward ran W * s (a folded FrozenBatchNorm scale s) is this call with s. */
+int sdetr_conv2d_f16x3_wgrad_ex(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
+                                int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin, int Cout,
+                                int groups, int ksize, int stride, const float *cout_scale, float *workspace,
+                                int64_t workspace_floats, float *dw, sdetr_stream_t stream);
+/* Input gradient of y = conv(x, W) with a fused epilogue: dx = (conv^T(dy, W) + z), then 0 where m <= 0.  dy: Hy x Wy with Cin
+ * channels (the forward's Cout); dx: H x W with Cout channels (the forward's Cin); W_hi / W_lo: the input-gradient pair W'
+ * (Cin, k, k, Cout / groups) of sdetr_conv2d_f16x3_split_weight.  Stride 1 is sdetr_conv2d_f16x3 on dy with W', stride 2 the
+ * transposed mode of sdetr_conv2d_f16x3_transposed: with z = m = NULL the same bits as those calls.  z (token rows, Cout wide;
+ * NULL: none) may alias dx (read before written, by the same thread); m (NULL: none) is the ReLU mask source of torch's
+ * threshold_backward(grad, m, 0): a NaN in m lets the value through, a NaN value stays NaN; m must not alias dx.  No bias, no
+ * activation.  Operand rules of sdetr_conv2d_f16x3; z, m, their pitches and row strides 8-byte aligned. */
+int sdetr_conv2d_f16x3_dgrad(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
+                             const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *z,
+                             int64_t z_pitch, int64_t ldz, const float *m, int64_t m_pitch, int64_t ldm, int Cout, int groups,
+                             int ksize, int stride, int H, int W, float *dx, int64_t dx_pitch, int64_t lddx, sdetr_stream_t stream);
 /* Gradient of the hi half of sdetr_upsample_nearest_concat: d_hi (Hi x Wi) = for each source pixel, the sum of g[:, :, 0:C] over
  * the destination pixels (Ho x Wo) that read it, rows then columns in order (no atomics: deterministic).  The lo half's gradient
  * is g[:, :, C:2C] itself.  C % 4 == 0; all row operands 16-byte aligned. */
@@ -657,6 +675,12 @@ int sdetr_resnet_stem(const float *x, int batch, int H, int W, const float *weig
 /* 3x3, stride 2, padding 1 max-pool on token rows (H x W, C channels) -> (Ho x Wo) with Ho = (H + 2 - 3) / 2 + 1, likewise Wo
  * (torch's max_pool2d, ceil_mode off).  Padding acts as -inf; a NaN in a window gives NaN.  C % 4 == 0; operands, pitches and
  * row strides 16-byte aligned.  One launch. */
+/* w (Cout, per_cout) fp32 with a FrozenBatchNorm folded in: s = weight * rsqrt(running_var + eps), w_folded = w * s, and (each
+ * optional) scale = s, bias = bias - running_mean * s, per output channel.  Computed in float64 with every operation rounded on
+ * its own, then rounded to fp32: the values of ResNetBackbone's host fold (backbone._fold), with no host read.  One launch. */
+int sdetr_frozen_bn_fold(const float *w, int Cout, int64_t per_cout, const float *bn_weight, const float *bn_bias,
+                         const float *running_mean, const float *running_var, double eps, float *w_folded, float *scale,
+                         float *bias, sdetr_stream_t stream);
 int sdetr_maxpool3x3s2_tokens(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int C, float *y,
                               int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
 #ifdef __cplusplus

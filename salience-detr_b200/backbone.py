@@ -14,6 +14,15 @@ it is ``forward_tokens(x)``: every FrozenBatchNorm folded into its convolution o
 convolution on ``sdetr_conv2d_f16x3_ex`` (3xFP16 on wgmma, fp32-class accuracy whatever ``allow_tf32`` says) with ReLU and the
 block's residual in the epilogue.  Each returned map is a channels-last NCHW view of its own ``(b, H*W, C)`` token buffer,
 which ``ChannelMapper`` reads in place.  No host synchronisation: the call can be captured in a CUDA graph.
+
+Under autograd, ``forward_tokens`` trains the convolutions of layers 1-4 in token layout when ``training_tokens_supported(x)``
+holds (a frozen stem, an image that needs no gradient): one ``torch.autograd.Function`` over the blocks from the first one
+with a trainable weight on.  Every call folds each FrozenBatchNorm into its convolution on the device
+(``sdetr_frozen_bn_fold``, the values of ``_fold``) and splits it into both fp16 layouts (``sdetr_conv2d_f16x3_split_weight``),
+so the forward writes the bits of the inference path and an optimizer step between CUDA-graph replays is seen.  The backward
+runs the whole chain: input gradients on ``sdetr_conv2d_f16x3_dgrad`` with the residual sum (``z``) and the ReLU mask (``m``)
+in its epilogue, weight gradients on ``sdetr_conv2d_f16x3_wgrad_ex`` with the FrozenBatchNorm scale in its write, and only
+the gradients something upstream needs.  ``forward`` itself stays the torch chain under autograd.
 """
 from __future__ import annotations
 
@@ -309,6 +318,94 @@ class ResNetBackbone(nn.Module):
                     return False
         return True
 
+    # ---- token-layout training -----------------------------------------------------------------------------------------
+    def training_tokens_supported(self, x) -> bool:
+        """True when forward_tokens can train this call in token layout: layers_supported() on a CUDA fp32 NCHW-contiguous
+        (b, 3, H, W) input with parameters and buffers fp32 on its device, a frozen stem (conv1.weight needs no gradient), an
+        input that needs no gradient, and autograd recording (grad enabled and some parameter requiring a gradient).  A stem
+        weight gradient and image gradients need forward()."""
+        if not _cuda_image(x) or x.requires_grad:
+            return False
+        if any(t.device != x.device or t.dtype != torch.float32 for t in list(self.parameters()) + list(self.buffers())):
+            return False
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())) or self.conv1.weight.requires_grad:
+            return False
+        return self.layers_supported()
+
+    def _train_plan(self):
+        """(blocks, first, stage_end): the Bottlenecks of the kept stages in order, the index of the first one with a trainable
+        convolution (the blocks before it neither train nor carry a gradient), and the index of each stage's last block"""
+        blocks = [blk for layer in self._stages() for blk in layer]
+        first = next(i for i, blk in enumerate(blocks) if any(c.weight.requires_grad for c in _block_convs(blk)))
+        stage_end, n = [], 0
+        for layer in self._stages():
+            n += len(layer)
+            stage_end.append(n - 1)
+        return blocks, first, stage_end
+
+    def launches_per_training_step(self) -> int:
+        """library launches of one forward_tokens under autograd and its backward (training_tokens_supported): the stem's fold,
+        the stem and the max-pool; per convolution 3 (fold, weight scale, split); per block the forward's 6 (+1 downsample);
+        per block from the first trainable one, backwards: the scale of G, and per gradient it needs 1 per input gradient, 1 per
+        activation scale of an input gradient a weight gradient reads, and 2 per weight gradient (convolution + split sum)"""
+        blocks, first, _ = self._train_plan()
+        n = 3
+        for blk in blocks:
+            ds = blk.downsample is not None
+            n += 3 * (3 + ds) + 6 + ds
+        for j in range(first, len(blocks)):
+            blk, need_in = blocks[j], j > first
+            c1, c2, c3 = (c.weight.requires_grad for c in (blk.conv1, blk.conv2, blk.conv3))
+            ds = blk.downsample is not None
+            n += 1 + 2 * c3 + (2 * blk.downsample[0].weight.requires_grad if ds else 0)
+            if c2 or c1 or need_in:
+                n += 2 + 2 * c2
+                if c1 or need_in:
+                    n += 2 + 2 * c1
+            if need_in:
+                n += 1 + ds
+        return n
+
+    def _train_tokens(self, x: Tensor) -> Dict[str, Tensor]:
+        """forward_tokens under autograd (training_tokens_supported): the blocks before the first trainable one as in inference,
+        the rest through _TrainBlocks; the same channels-last views, with the bits of the inference path"""
+        blocks, first, stage_end = self._train_plan()
+        ks = []
+        for j, blk in enumerate(blocks):
+            ds = blk.downsample
+            ks.append((_TConv(blk.conv1, blk.bn1, j >= first), _TConv(blk.conv2, blk.bn2, j >= first),
+                       _TConv(blk.conv3, blk.bn3, j >= first), _TConv(ds[0], ds[1], j >= first) if ds is not None else None))
+        stem_w, _, stem_b = cabi.frozen_bn_fold(self.conv1.weight.detach(), self.bn1, scale=False)
+        b, _, H, W = x.shape
+        hw = ((H - 1) // 2 + 1, (W - 1) // 2 + 1)
+        t = cabi.resnet_stem(x, stem_w.view(64, 147).t().contiguous(), stem_b)
+        t = cabi.maxpool3x3s2_tokens(t, hw)
+        hw = ((hw[0] - 1) // 2 + 1, (hw[1] - 1) // 2 + 1)
+        feats = {}
+        for j in range(first):  # inference: nothing saved, conv3 writes over the residual in place
+            c1, c2, c3, ds = ks[j]
+            s = cabi.pow2_scale(t, 12)
+            y1 = c1(t, hw, s)
+            y2 = c2(y1, hw, cabi.pow2_scale(y1, 12))
+            s2 = cabi.pow2_scale(y2, 12)
+            hw2 = c2.out_hw(hw)
+            ident = ds(t, hw, s, act=0) if ds is not None else t
+            t, hw = c3(y2, hw2, s2, out=ident, z=ident), hw2
+            if j in stage_end:
+                feats[stage_end.index(j)] = (t, hw)
+        weights = [c.weight for k in ks[first:] for c in k if c is not None and c.trainable]
+        ends = [stage_end.index(j) if j in stage_end and stage_end.index(j) in self.return_indices else None
+                for j in range(first, len(blocks))]
+        run = _TrainRun(ks[first:], ends, hw)
+        outs = _TrainBlocks.apply(run, t, *weights)
+        for i, o in zip(run.returned, outs):
+            feats[i] = (o, run.out_hw[i])
+        res = {}
+        for i in self.return_indices:
+            t, (h, w) = feats[i]
+            res[f"layer{i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
+        return res
+
     def _kernel_weights(self):
         """the folded stem ((147, 64) weight, bias) and per stage per block the (conv1, conv2, conv3, downsample or None)
         convolutions in kernel form, rebuilt when any parameter or buffer changes"""
@@ -347,6 +444,8 @@ class ResNetBackbone(nn.Module):
         (strides (h*w*C, 1, w*C, C)) of its own (b, h*w, C) token buffer; the values of forward() in torch.  No host
         synchronisation."""
         if not self.tokens_supported(x):
+            if self.training_tokens_supported(x):
+                return self._train_tokens(x)
             raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported)")
         (stem_w, stem_b), stages = self._kernel_weights()
         b, _, H, W = x.shape
@@ -372,3 +471,125 @@ class ResNetBackbone(nn.Module):
             t, (h, w) = feats[i]
             outs[f"layer{i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
         return outs
+
+
+def _cuda_image(x) -> bool:
+    """a non-empty NCHW-contiguous CUDA fp32 (b, 3, H, W) tensor"""
+    return (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.numel() > 0
+            and x.is_contiguous())
+
+
+def _block_convs(blk: Bottleneck) -> List[nn.Conv2d]:
+    return [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
+
+
+class _TConv:
+    """one convolution of the training path, folded and split in this call: the forward pair, the input-gradient pair (for the
+    blocks the backward runs through), the folded bias and the FrozenBatchNorm scale s (the weight gradient is s * wgrad)"""
+
+    def __init__(self, conv: nn.Conv2d, bn: FrozenBatchNorm2d, backward: bool):
+        self.weight, self.trainable = conv.weight, conv.weight.requires_grad
+        self.ksize, self.stride, self.shape = conv.kernel_size[0], conv.stride[0], tuple(conv.weight.shape)
+        wf, self.scale, self.bias = cabi.frozen_bn_fold(conv.weight.detach(), bn)
+        self.w_hi, self.w_lo, self.d_hi, self.d_lo, self.w_scale = cabi.conv2d_f16x3_split_weight(wf, 1, backward)
+
+    def out_hw(self, hw):
+        return tuple((v - 1) // self.stride + 1 for v in hw)
+
+    def __call__(self, x: Tensor, hw, scale: Tensor, act: int = cabi.ACT_RELU, out=None, z=None) -> Tensor:
+        return cabi.conv2d_f16x3(x, hw, scale, self.w_hi, self.w_lo, self.w_scale, self.bias, 1, self.ksize, self.stride, act,
+                                 out=out, z=z)
+
+    def dgrad(self, g: Tensor, g_hw, g_scale: Tensor, hw, z=None, m=None, out=None) -> Tensor:
+        return cabi.conv2d_f16x3_dgrad(g, g_hw, g_scale, self.d_hi, self.d_lo, self.w_scale, 1, self.ksize, self.stride, hw, z=z, m=m,
+                                       out=out)
+
+    def wgrad(self, g: Tensor, g_scale: Tensor, x: Tensor, x_scale: Tensor, hw) -> Tensor:
+        return cabi.conv2d_f16x3_wgrad(g, g_scale, x, x_scale, hw, self.shape, self.stride, cout_scale=self.scale)
+
+
+class _TrainRun:
+    """what _TrainBlocks needs beyond tensors: per block its convolutions and the stage it ends (or None), the input map size"""
+
+    def __init__(self, convs, ends, hw):
+        self.convs, self.ends, self.hw = convs, ends, hw
+        self.returned = [i for i in ends if i is not None]
+        self.out_hw = {}
+
+
+class _TrainBlocks(torch.autograd.Function):
+    """The Bottlenecks from the first trainable one to the last kept stage, on token rows.  Inputs: the run, the token rows of
+    the first block's input (no gradient), the trainable convolution weights in block order.  Outputs: the token rows of every
+    stage that ends in the run.  The backward walks the chain once, G being the gradient at a block's pre-ReLU sum:
+    wgrad3(G, y2); dy2 = dgrad3(G) * [y2 > 0]; wgrad2(dy2, y1); dy1 = dgrad2(dy2) * [y1 > 0]; wgrad1(dy1, t); and, when an
+    earlier block needs it, G_prev = (dgrad1(dy1) + d_id) * [t > 0] with d_id = G or dgrad_ds(G) (+ the gradient of the
+    returned map t, if it is one), each product and sum in a convolution's epilogue."""
+
+    @staticmethod
+    def forward(ctx, run: _TrainRun, t: Tensor, *weights: Tensor):
+        hw = run.hw
+        saved, outs = [], []
+        for (c1, c2, c3, ds), end in zip(run.convs, run.ends):
+            s = cabi.pow2_scale(t, 12)
+            y1 = c1(t, hw, s)
+            s1 = cabi.pow2_scale(y1, 12)
+            y2 = c2(y1, hw, s1)
+            s2 = cabi.pow2_scale(y2, 12)
+            hw2 = c2.out_hw(hw)
+            if ds is not None:
+                ident = ds(t, hw, s, act=0)
+                out = c3(y2, hw2, s2, out=ident, z=ident)
+            else:
+                out = c3(y2, hw2, s2, z=t)  # a fresh output: the block input is kept for the backward
+            saved += [t, s, y1, s1, y2, s2]
+            t, hw = out, hw2
+            if end is not None:
+                outs.append(t)
+                run.out_hw[end] = hw
+        ctx.run = run
+        ctx.save_for_backward(*saved, t)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        run = ctx.run
+        saved = ctx.saved_tensors
+        # a returned map's gradient as token rows: a view when it came channels-last, else one copy
+        ext = {end: g if g.is_contiguous() else g.contiguous() for end, g in zip(run.returned, grads)}
+        dws = []
+        nblk = len(run.convs)
+        hws = [run.hw]
+        for c1, c2, c3, ds in run.convs:
+            hws.append(c2.out_hw(hws[-1]))
+        # the deepest returned map's gradient, through the last block's ReLU
+        G = torch.ops.aten.threshold_backward(ext[run.returned[-1]], saved[-1], 0)
+        for j in range(nblk - 1, -1, -1):
+            c1, c2, c3, ds = run.convs[j]
+            t, s, y1, s1, y2, s2 = saved[6 * j: 6 * j + 6]
+            hw, hw2 = hws[j], hws[j + 1]
+            need_in = j > 0
+            gs = cabi.pow2_scale(G, 12)
+            blk_dw = {}
+            if c3.trainable:
+                blk_dw[3] = c3.wgrad(G, gs, y2, s2, hw2)
+            if c2.trainable or c1.trainable or need_in:
+                dy2 = c3.dgrad(G, hw2, gs, hw2, m=y2)
+                s_dy2 = cabi.pow2_scale(dy2, 12)
+                if c2.trainable:
+                    blk_dw[2] = c2.wgrad(dy2, s_dy2, y1, s1, hw)
+                if c1.trainable or need_in:
+                    dy1 = c2.dgrad(dy2, hw2, s_dy2, hw, m=y1)
+                    s_dy1 = cabi.pow2_scale(dy1, 12)
+                    if c1.trainable:
+                        blk_dw[1] = c1.wgrad(dy1, s_dy1, t, s, hw)
+            if ds is not None and ds.trainable:
+                blk_dw[4] = ds.wgrad(G, gs, t, s, hw)
+            if need_in:
+                z = ext.get(run.ends[j - 1]) if run.ends[j - 1] is not None else None
+                if ds is not None:
+                    d = ds.dgrad(G, hw2, gs, hw, z=z)
+                else:
+                    d = G if z is None else G + z
+                G = c1.dgrad(dy1, hw, s_dy1, hw, z=d, m=t, out=d)
+            dws.append([blk_dw[i] for i in (1, 2, 3, 4) if i in blk_dw])
+        return (None, None) + tuple(dw for blk in reversed(dws) for dw in blk)

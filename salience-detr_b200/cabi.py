@@ -109,6 +109,10 @@ SIGNATURES = {
                                    _i64, _i64, _vp]),
     "sdetr_resnet_stem": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "sdetr_maxpool3x3s2_tokens": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
+    "sdetr_conv2d_f16x3_wgrad_ex": (_i, [_vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp] + [_i] * 8 + [_vp, _vp, _i64, _vp, _vp]),
+    "sdetr_conv2d_f16x3_dgrad": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i64, _i64] + [_i] * 6 +
+                                 [_vp, _i64, _i64, _vp]),
+    "sdetr_frozen_bn_fold": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, _vp, _vp, _vp, _vp]),
 }
 
 
@@ -987,9 +991,10 @@ def conv2d_f16x3_transposed(dy, dy_hw, a_scale, w_hi, w_lo, w_scale, groups: int
     return dx
 
 
-def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int):
+def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int, cout_scale=None):
     """Weight gradient (Cout, Cin / groups, k, k) of y = conv(x, W): dy (b, Ho*Wo, Cout), x (b, H*W, Cin) views with unit channel
-    stride, hw = (H, W); dy_scale / x_scale: their pow2_scale device scalars (target 12).  Bit-reproducible."""
+    stride, hw = (H, W); dy_scale / x_scale: their pow2_scale device scalars (target 12).  Bit-reproducible.
+    cout_scale: optional (Cout,) fp32 factor per output channel, applied in the split sum's write (sdetr_conv2d_f16x3_wgrad_ex)."""
     b, _, cin = x.shape
     cout, cin_g, k, _ = (int(v) for v in weight_shape)
     groups = cin // cin_g
@@ -1000,11 +1005,60 @@ def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int):
     dw = torch.empty(cout, cin_g, k, k, device=x.device, dtype=torch.float32)
     ws = torch.empty(max(int(lib().sdetr_conv2d_f16x3_wgrad_workspace_floats(b, ho, wo, cin, cout, groups, k)), 4), device=x.device,
                      dtype=torch.float32)
-    rc = lib().sdetr_conv2d_f16x3_wgrad(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
-                                        _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
-                                        int(stride), ws.data_ptr(), ws.numel(), dw.data_ptr(), _stream())
-    _check(rc, "sdetr_conv2d_f16x3_wgrad")
+    if cout_scale is None:
+        rc = lib().sdetr_conv2d_f16x3_wgrad(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
+                                            _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
+                                            int(stride), ws.data_ptr(), ws.numel(), dw.data_ptr(), _stream())
+        _check(rc, "sdetr_conv2d_f16x3_wgrad")
+        return dw
+    if cout_scale.numel() != cout:
+        raise RuntimeError(f"conv2d_f16x3_wgrad: cout_scale must have {cout} entries")
+    rc = lib().sdetr_conv2d_f16x3_wgrad_ex(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
+                                           _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
+                                           int(stride), _req(cout_scale, "cout_scale", torch.float32), ws.data_ptr(), ws.numel(),
+                                           dw.data_ptr(), _stream())
+    _check(rc, "sdetr_conv2d_f16x3_wgrad_ex")
     return dw
+
+
+def conv2d_f16x3_dgrad(dy, dy_hw, a_scale, w_hi, w_lo, w_scale, groups: int, ksize: int, stride: int, hw, z=None, m=None, out=None):
+    """Input gradient of a stride-1 or stride-2 convolution of an (H, W) = hw map with a fused epilogue:
+    dx = conv^T(dy, W) (+ z), then 0 where m <= 0 (torch's threshold_backward(dx, m, 0)).  dy (b, Hy*Wy, Cout) view; W' = the
+    (Cin, k, k, Cout / groups) input-gradient pair of conv2d_f16x3_split_weight; a_scale: pow2_scale of dy (target 12).
+    z, m: optional (b, H*W, Cin) views, z may be ``out`` itself, m may not.  out: optional (b, H*W, Cin) view to write."""
+    b, n, cin = dy.shape
+    if n != dy_hw[0] * dy_hw[1]:
+        raise RuntimeError(f"conv2d_f16x3_dgrad: dy has {n} rows per image, the map is {dy_hw[0]}x{dy_hw[1]}")
+    cout = w_hi.shape[0]
+    dx = out if out is not None else torch.empty(b, hw[0] * hw[1], cout, device=dy.device, dtype=torch.float32)
+    for t, name in ((dx, "out"), (z, "z"), (m, "m")):
+        if t is not None and tuple(t.shape) != (b, hw[0] * hw[1], cout):
+            raise RuntimeError(f"conv2d_f16x3_dgrad: {name} must be ({b}, {hw[0] * hw[1]}, {cout})")
+    zp = _token_rows(z, "z") if z is not None else (None, 0, 0)
+    mp = _token_rows(m, "m") if m is not None else (None, 0, 0)
+    rc = lib().sdetr_conv2d_f16x3_dgrad(*_token_rows(dy, "dy"), b, int(dy_hw[0]), int(dy_hw[1]), cin,
+                                        _req(a_scale, "a_scale", torch.float32), _req(w_hi, "w_hi", torch.float16),
+                                        _req(w_lo, "w_lo", torch.float16), _req(w_scale, "w_scale", torch.float32), *zp, *mp, cout,
+                                        int(groups), int(ksize), int(stride), int(hw[0]), int(hw[1]), *_token_rows(dx, "dx"),
+                                        _stream())
+    _check(rc, "sdetr_conv2d_f16x3_dgrad")
+    return dx
+
+
+def frozen_bn_fold(w, bn, scale: bool = True, bias: bool = True):
+    """(w * s, s, bias - running_mean * s) of a weight (Cout, ...) and a FrozenBatchNorm2d ``bn`` (s = weight * rsqrt(running_var
+    + eps)), computed on the device in float64 and rounded to fp32 (sdetr_frozen_bn_fold): backbone._fold's values, no host read.
+    s / the bias are None unless asked for."""
+    cout = w.shape[0]
+    wf = torch.empty(w.shape, device=w.device, dtype=torch.float32)
+    s = torch.empty(cout, device=w.device, dtype=torch.float32) if scale else None
+    bf = torch.empty(cout, device=w.device, dtype=torch.float32) if bias else None
+    rc = lib().sdetr_frozen_bn_fold(_req(w, "w", torch.float32), cout, w.numel() // cout, _req(bn.weight, "bn.weight", torch.float32),
+                                    _req(bn.bias, "bn.bias", torch.float32), _req(bn.running_mean, "bn.running_mean", torch.float32),
+                                    _req(bn.running_var, "bn.running_var", torch.float32), float(bn.eps), wf.data_ptr(),
+                                    s.data_ptr() if scale else None, bf.data_ptr() if bias else None, _stream())
+    _check(rc, "sdetr_frozen_bn_fold")
+    return wf, s, bf
 
 
 def upsample_nearest_concat_backward(g_hi, lo_hw, hi_hw):

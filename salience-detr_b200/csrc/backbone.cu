@@ -5,6 +5,8 @@
 //                                the NCHW fp32 image batch to (b, Ho*Wo, 64) token rows.  Plain fp32 FMAs on the CUDA cores, taps
 //                                summed in (channel, ky, kx) order: the stem is under 3 % of the backbone's operations.
 //   sdetr_maxpool3x3s2_tokens    3x3 / stride 2 / padding 1 max-pool on token rows, 16-byte channel vectors.
+//   sdetr_frozen_bn_fold         a convolution weight with its FrozenBatchNorm folded in, on the device (the training path
+//                                re-folds every call): the float64 arithmetic of backbone._fold, each operation rounded alone.
 #include <math.h>
 
 #include "common.cuh"
@@ -102,6 +104,27 @@ __global__ void maxpool3x3s2_tokens_kernel(const float *__restrict__ x, int64_t 
     }
 }
 
+// s = weight * rsqrt(var + eps), w_folded = w * s, bias_folded = bias - mean * s: each in float64 with its own rounding (no
+// contraction), as torch computes them op by op, then rounded to fp32 once; rsqrt is the same libdevice function torch calls
+__device__ __forceinline__ double frozen_bn_scale(const float *weight, const float *var, double eps, int c) {
+    return __dmul_rn((double)__ldg(weight + c), rsqrt(__dadd_rn((double)__ldg(var + c), eps)));
+}
+
+__global__ void frozen_bn_fold_kernel(const float *__restrict__ w, int cout, int64_t per_co, const float *__restrict__ bn_w,
+                                      const float *__restrict__ bn_b, const float *__restrict__ mean, const float *__restrict__ var,
+                                      double eps, float *__restrict__ w_folded, float *__restrict__ scale, float *__restrict__ bias) {
+    const int64_t n = (int64_t)cout * per_co;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i / per_co);
+        const double s = frozen_bn_scale(bn_w, var, eps, c);
+        w_folded[i] = __double2float_rn(__dmul_rn((double)w[i], s));
+        if (i - (int64_t)c * per_co == 0) {
+            if (scale) scale[c] = __double2float_rn(s);
+            if (bias) bias[c] = __double2float_rn(__dsub_rn((double)__ldg(bn_b + c), __dmul_rn((double)__ldg(mean + c), s)));
+        }
+    }
+}
+
 }  // namespace sdetr
 
 using namespace sdetr;
@@ -138,4 +161,16 @@ extern "C" int sdetr_maxpool3x3s2_tokens(const float *x, int64_t x_pitch, int64_
     maxpool3x3s2_tokens_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, ldx, batch, H, W,
                                                                                                        C, Ho, Wo, y, y_pitch, ldy);
     return check_launch("maxpool3x3s2_tokens");
+}
+
+extern "C" int sdetr_frozen_bn_fold(const float *w, int Cout, int64_t per_cout, const float *bn_weight, const float *bn_bias,
+                                    const float *running_mean, const float *running_var, double eps, float *w_folded,
+                                    float *scale, float *bias, sdetr_stream_t stream) {
+    SDETR_REQUIRE(w && bn_weight && bn_bias && running_mean && running_var && w_folded, SDETR_ERR_INVALID_ARG,
+                  "frozen_bn_fold: null pointer");
+    SDETR_REQUIRE(Cout > 0 && per_cout > 0, SDETR_ERR_INVALID_ARG, "frozen_bn_fold: bad sizes");
+    const int64_t n = (int64_t)Cout * per_cout, want = (n + 255) / 256, cap = 8LL * sm_count();
+    frozen_bn_fold_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, (cudaStream_t)stream>>>(
+        w, Cout, per_cout, bn_weight, bn_bias, running_mean, running_var, eps, w_folded, scale, bias);
+    return check_launch("frozen_bn_fold");
 }

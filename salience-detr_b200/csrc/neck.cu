@@ -39,6 +39,8 @@ struct ConvParams {
     const float *a_scale, *w_scale, *bias;
     const float *z;  // residual added before the activation (NULL: none); may alias y
     int64_t z_pitch, ldz;
+    const float *m;  // ReLU mask source (NULL: none): the output is 0 where m <= 0 (torch's threshold_backward); not y
+    int64_t m_pitch, ldm;
     float *y;
     int64_t y_pitch, ldy;
     int H, W, Ho, Wo, M, cin_g, cout_g, ksize, stride, act;
@@ -152,6 +154,7 @@ __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams
         float *dst = p.y + (int64_t)n * p.y_pitch + (int64_t)pix * p.ldy + n0;
         // z is read by the thread that then writes the same two floats of y, so z may alias y
         const float *zr = p.z ? p.z + (int64_t)n * p.z_pitch + (int64_t)pix * p.ldz + n0 : nullptr;
+        const float *mr = p.m ? p.m + (int64_t)n * p.m_pitch + (int64_t)pix * p.ldm + n0 : nullptr;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int col = 8 * j + 2 * q;
@@ -163,6 +166,11 @@ __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams
             }
             if (p.act == kActSiLU) v0 = silu(v0), v1 = silu(v1);
             else if (p.act == kActReLU) v0 = relu_nan(v0), v1 = relu_nan(v1);
+            if (mr) {  // a NaN in m lets the value through, a NaN value stays NaN
+                const float2 r = *reinterpret_cast<const float2 *>(mr + col);
+                if (r.x <= 0.f) v0 = 0.f;
+                if (r.y <= 0.f) v1 = 0.f;
+            }
             *reinterpret_cast<float2 *>(dst + col) = make_float2(v0, v1);
         }
     }
@@ -456,11 +464,13 @@ __global__ void __launch_bounds__(kCvThreads) conv_wgrad_f16x3_kernel(const Wgra
     }
 }
 
-__global__ void wgrad_reduce_kernel(const float *__restrict__ part, int splits, int64_t n, float *__restrict__ dw) {
+// dw = the splits summed in split order, times cout_scale[co] when it is not NULL (one rounded product after the sum)
+__global__ void wgrad_reduce_kernel(const float *__restrict__ part, int splits, int64_t n, const float *__restrict__ cout_scale,
+                                    int64_t per_co, float *__restrict__ dw) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float s = 0.f;
         for (int k = 0; k < splits; ++k) s += part[(int64_t)k * n + i];
-        dw[i] = s;
+        dw[i] = cout_scale ? s * __ldg(cout_scale + i / per_co) : s;
     }
 }
 
@@ -541,8 +551,8 @@ extern "C" int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ld
     static PerDeviceOnce once;
     SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<false>, kCvSmem, "conv2d_f16x3");
     const ConvParams p{x, x_pitch, ldx, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
-                       w_scale_dev, bias, z, z_pitch, ldz, y, y_pitch, ldy, H, W, Ho, Wo, (int)M, Cin / groups, Cout / groups,
-                       ksize, stride, act};
+                       w_scale_dev, bias, z, z_pitch, ldz, nullptr, 0, 0, y, y_pitch, ldy, H, W, Ho, Wo, (int)M, Cin / groups,
+                       Cout / groups, ksize, stride, act};
     const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
     conv_f16x3_kernel<false><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
     return check_launch("conv2d_f16x3");
@@ -583,7 +593,8 @@ extern "C" int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, 
     static PerDeviceOnce once;
     SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<true>, kCvSmem, "conv2d_f16x3_transposed");
     const ConvParams p{dy, dy_pitch, lddy, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
-                       w_scale_dev, nullptr, nullptr, 0, 0, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups, Cout / groups, ksize, 2, 0};
+                       w_scale_dev, nullptr, nullptr, 0, 0, nullptr, 0, 0, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups,
+                       Cout / groups, ksize, 2, 0};
     const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
     conv_f16x3_kernel<true><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
     return check_launch("conv2d_f16x3_transposed");
@@ -597,10 +608,10 @@ extern "C" int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, 
     return (int64_t)splits * Cout * (Cin / groups) * ksize * ksize;
 }
 
-extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
-                                        int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin,
-                                        int Cout, int groups, int ksize, int stride, float *workspace, int64_t workspace_floats,
-                                        float *dw, sdetr_stream_t stream) {
+extern "C" int sdetr_conv2d_f16x3_wgrad_ex(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev,
+                                           const float *x, int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H,
+                                           int W, int Cin, int Cout, int groups, int ksize, int stride, const float *cout_scale,
+                                           float *workspace, int64_t workspace_floats, float *dw, sdetr_stream_t stream) {
     SDETR_REQUIRE(dy && dy_scale_dev && x && x_scale_dev && dw && workspace, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_wgrad: null pointer");
     SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
                   "conv2d_f16x3_wgrad: bad sizes");
@@ -627,8 +638,62 @@ extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64
         const int rc = check_launch("conv2d_f16x3_wgrad");
         if (rc) return rc;
     }
-    wgrad_reduce_kernel<<<elementwise_blocks(n), 256, 0, (cudaStream_t)stream>>>(workspace, splits, n, dw);
+    wgrad_reduce_kernel<<<elementwise_blocks(n), 256, 0, (cudaStream_t)stream>>>(workspace, splits, n, cout_scale,
+                                                                                  n / Cout, dw);
     return check_launch("conv2d_f16x3_wgrad (split sum)");
+}
+
+extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
+                                        int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin,
+                                        int Cout, int groups, int ksize, int stride, float *workspace, int64_t workspace_floats,
+                                        float *dw, sdetr_stream_t stream) {
+    return sdetr_conv2d_f16x3_wgrad_ex(dy, dy_pitch, lddy, dy_scale_dev, x, x_pitch, ldx, x_scale_dev, batch, H, W, Cin, Cout, groups,
+                                       ksize, stride, nullptr, workspace, workspace_floats, dw, stream);
+}
+
+extern "C" int sdetr_conv2d_f16x3_dgrad(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
+                                        const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
+                                        const float *z, int64_t z_pitch, int64_t ldz, const float *m, int64_t m_pitch, int64_t ldm,
+                                        int Cout, int groups, int ksize, int stride, int H, int W, float *dx, int64_t dx_pitch,
+                                        int64_t lddx, sdetr_stream_t stream) {
+    SDETR_REQUIRE(dy && a_scale_dev && W_hi && W_lo && w_scale_dev && dx, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: null pointer");
+    SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_dgrad: bad sizes");
+    SDETR_REQUIRE((ksize == 1 || ksize == 3) && (stride == 1 || stride == 2), SDETR_ERR_UNSUPPORTED,
+                  "conv2d_f16x3_dgrad: takes kernel 1 or 3, stride 1 or 2");
+    SDETR_REQUIRE(Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kCvK == 0 && (Cout / groups) % kCvN == 0,
+                  SDETR_ERR_UNSUPPORTED, "conv2d_f16x3_dgrad: Cin/groups=%d and Cout/groups=%d must be multiples of 64",
+                  Cin / groups, Cout / groups);
+    const int pad = ksize / 2, hy = H > 0 ? (H + 2 * pad - ksize) / stride + 1 : 0, wy = W > 0 ? (W + 2 * pad - ksize) / stride + 1 : 0;
+    SDETR_REQUIRE(Hy == hy && Wy == wy, SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_dgrad: dY is %dx%d, a stride-%d convolution of %dx%d gives %dx%d", Hy, Wy, stride, H, W, hy, wy);
+    SDETR_REQUIRE(rows_ok(dy, dy_pitch, lddy) && lddy >= Cin && aligned16(W_hi) && aligned16(W_lo), SDETR_ERR_INVALID_ARG,
+                  "conv2d_f16x3_dgrad: dy, its pitch and row stride and the weights must be 16-byte aligned");
+    SDETR_REQUIRE((reinterpret_cast<uintptr_t>(dx) & 7) == 0 && dx_pitch % 2 == 0 && lddx % 2 == 0 && lddx >= Cout,
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: dx, its pitch and row stride must be 8-byte aligned");
+    SDETR_REQUIRE(!z || ((reinterpret_cast<uintptr_t>(z) & 7) == 0 && z_pitch % 2 == 0 && ldz % 2 == 0 && ldz >= Cout),
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: z, its pitch and row stride must be 8-byte aligned");
+    SDETR_REQUIRE(!m || ((reinterpret_cast<uintptr_t>(m) & 7) == 0 && m_pitch % 2 == 0 && ldm % 2 == 0 && ldm >= Cout),
+                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: m, its pitch and row stride must be 8-byte aligned");
+    SDETR_REQUIRE(m != dx, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: m must not alias dx");
+    const int64_t M = (int64_t)batch * H * W;
+    SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_dgrad: too many output pixels");
+    if (M == 0) return SDETR_OK;
+    // stride 1: the forward kernel on dY with the flipped weights (dY and dX share the map size); stride 2: its transposed mode
+    const ConvParams p{dy, dy_pitch, lddy, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
+                       w_scale_dev, nullptr, z, z_pitch, ldz, m, m_pitch, ldm, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M,
+                       Cin / groups, Cout / groups, ksize, stride == 1 ? 1 : 2, 0};
+    const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
+    if (stride == 1) {
+        static PerDeviceOnce once;
+        SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<false>, kCvSmem, "conv2d_f16x3_dgrad");
+        conv_f16x3_kernel<false><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
+    } else {
+        static PerDeviceOnce once;
+        SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<true>, kCvSmem, "conv2d_f16x3_dgrad");
+        conv_f16x3_kernel<true><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
+    }
+    return check_launch("conv2d_f16x3_dgrad");
 }
 
 extern "C" int64_t sdetr_context_gate_workspace_floats(int batch, int HW, int C) {

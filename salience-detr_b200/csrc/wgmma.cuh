@@ -13,7 +13,11 @@
 //                             wgmma group completes each warp releases the stage on its `empty` mbarrier and adds the
 //                             k-block's product to a second set of fp32 registers with ordinary round-to-nearest adds
 //                             (the tensor core's own accumulation truncates: over K = 2048 that alone costs ~3 bits).
-//                             The epilogue scales, adds the bias and stores straight from those registers.
+//                             The epilogue scales, adds the bias and stores straight from those registers.  The loop
+//                             runs one k-block ahead, across tiles: the next k-block's fragments are split, and the
+//                             previous tile's epilogue runs, while the current k-block's wgmma group is in flight.
+//                             The fragments are read with shared-window loads, and the loop is compiled once per
+//                             input activation, so the split has no per-element activation test.
 // Registers: setmaxnreg moves them from the producer warpgroup (40) to the two consumer warpgroups (232 each).
 #pragma once
 #include <cuda.h>
@@ -159,6 +163,18 @@ __device__ __forceinline__ const float *swz_f32(const uint8_t *box, int r, int c
     return reinterpret_cast<const float *>(box + r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2)));
 }
 
+// shared-memory loads through the shared window (a generic load of the same address takes the longer generic path)
+__device__ __forceinline__ float2 lds_f32x2(const float *p) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)));
+    return v;
+}
+__device__ __forceinline__ float lds_f32(const float *p) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_u32(p)));
+    return v;
+}
+
 // ---- the kernel ------------------------------------------------------------------------------------------------------
 constexpr int kGM = 128, kGN = 128;   // CTA tile
 constexpr int kGThreads = 384;        // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue
@@ -183,6 +199,157 @@ struct Gemm3xParams {
     const float *a_scale_dev;  // fp16 form with device scales: a_scale = *a_scale_dev, out_scale = 1 / (a_scale * *w_scale_dev)
     const float *w_scale_dev;
 };
+
+// Consumer side of one k-block, first half: wait until stage `st` has landed (SPLIT_W: split its raw W in place, both
+// consumer warpgroups, before any wgmma reads it), then read this thread's A fragments and split them into hi / lo.
+template <bool F16, bool SPLIT_W>
+__device__ __forceinline__ void gemm3x_stage_in(uint8_t *st, uint64_t *full, uint32_t ph, int r0, int q, int act,
+                                                float a_scale, uint32_t (&ahi)[4][4], uint32_t (&alo)[4][4]) {
+    using S = Gemm3xShape<F16>;
+    mbar_wait(full, ph);
+    if (SPLIT_W) {
+        uint8_t *w_hi = st + S::kABoxes * kGBox, *w_lo = w_hi + kGBox;
+        for (int i = threadIdx.x - 128; i < kGBox / 16; i += 256) {
+            const float4 w = reinterpret_cast<const float4 *>(w_hi)[i];
+            float4 h, l;
+            h.x = tf32_rn(w.x), h.y = tf32_rn(w.y), h.z = tf32_rn(w.z), h.w = tf32_rn(w.w);
+            l.x = tf32_rn(w.x - h.x), l.y = tf32_rn(w.y - h.y), l.z = tf32_rn(w.z - h.z), l.w = tf32_rn(w.w - h.w);
+            reinterpret_cast<float4 *>(w_hi)[i] = h;
+            reinterpret_cast<float4 *>(w_lo)[i] = l;
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> wgmma operand reads
+        named_bar_sync(1, 256);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        if (F16) {  // m64k16: (r0, c..c+1), (r0+8, c..c+1), (r0, c+8..c+9), (r0+8, c+8..c+9)
+            const uint8_t *box = st + (kk >> 1) * kGBox;
+            const int c = (kk & 1) * 16 + 2 * q;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 x = lds_f32x2(swz_f32(box, r0 + (j & 1) * 8, c + (j >> 1) * 8));
+                split2(apply_act(x.x, act) * a_scale, apply_act(x.y, act) * a_scale, ahi[kk][j], alo[kk][j]);
+            }
+        } else {  // m64k8: (r0, c), (r0+8, c), (r0, c+4), (r0+8, c+4)
+            const int c = kk * 8 + q;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float x = apply_act(lds_f32(swz_f32(st, r0 + (j & 1) * 8, c + (j >> 1) * 4)), act), h = tf32_rn(x);
+                ahi[kk][j] = __float_as_uint(h), alo[kk][j] = __float_as_uint(tf32_rn(x - h));
+            }
+        }
+    }
+}
+
+// Second half: the k-block's 12 wgmma into d (d = alo.W_hi first, then += ahi.W_lo, += ahi.W_hi per 32 bytes of K), one
+// commit group.  The caller waits for it before it touches d or rewrites ahi / alo.
+template <bool F16>
+__device__ __forceinline__ void gemm3x_issue(float (&d)[64], const uint32_t (&ahi)[4][4], const uint32_t (&alo)[4][4],
+                                             const uint8_t *st) {
+    using S = Gemm3xShape<F16>;
+    wgmma_fence();
+    const uint32_t bh = smem_u32(st + S::kABoxes * kGBox), bl = bh + kGBox;
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {  // 32 bytes of K per step in either type
+        if (F16) {
+            wgmma_f16_rs(d, alo[kk], wgmma_desc(bh + kk * 32), kk);
+            wgmma_f16_rs(d, ahi[kk], wgmma_desc(bl + kk * 32), 1);
+            wgmma_f16_rs(d, ahi[kk], wgmma_desc(bh + kk * 32), 1);
+        } else {
+            wgmma_tf32_rs(d, alo[kk], wgmma_desc(bh + kk * 32), kk);
+            wgmma_tf32_rs(d, ahi[kk], wgmma_desc(bl + kk * 32), 1);
+            wgmma_tf32_rs(d, ahi[kk], wgmma_desc(bh + kk * 32), 1);
+        }
+    }
+    wgmma_commit();
+}
+
+// Epilogue of tile t: C = acc * out_scale + bias.  acc[4j + {0,1}] = (row r0, cols 8j + 2q + {0,1}), acc[4j + {2,3}] =
+// (row r0 + 8, same cols).
+__device__ __forceinline__ void gemm3x_epilogue(const Gemm3xParams &p, const float (&acc)[64], int t, int n_tiles, int r0, int q,
+                                                float out_scale) {
+    const int m0 = (t / n_tiles) * kGM, n0 = (t % n_tiles) * kGN;
+    const bool pair = (p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        if (col >= p.N) continue;
+        const bool two = col + 1 < p.N;
+        const float b0 = p.bias ? __ldg(p.bias + col) : 0.f, b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = m0 + r0 + 8 * h;
+            if (row >= p.M) continue;
+            float *dst = p.C + (int64_t)row * p.ldc + col;
+            const float v0 = acc[4 * j + 2 * h] * out_scale + b0, v1 = acc[4 * j + 2 * h + 1] * out_scale + b1;
+            if (two && pair) {
+                *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);
+            } else {
+                dst[0] = v0;
+                if (two) dst[1] = v1;
+            }
+        }
+    }
+}
+
+// Keeps the register A operands of a waited-for wgmma group allocated up to this point.  wgmma reads them after it
+// issues, but ptxas hands their registers to values computed under the MMA (the next k-block's fragments) unless they
+// are read again after the wait.  This is that read: stores under a predicate that is never true (`never`, false on every
+// launch), one issue slot per four registers.
+__device__ __forceinline__ void wgmma_hold(const uint32_t (&a)[4][4], bool never) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t@p st.shared.v4.b32 [%5], {%0, %1, %2, %3};\n\t}" ::"r"(a[kk][0]),
+                     "r"(a[kk][1]), "r"(a[kk][2]), "r"(a[kk][3]), "r"((int)never), "r"(0u)
+                     : "memory");
+}
+
+// The consumer loop of gemm3x_kernel, with the input activation fixed at compile time.
+template <bool F16, bool SPLIT_W, int ACT>
+__device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *smem, uint64_t *full, uint64_t *empty, int tiles,
+                                               int n_tiles, int kblocks, int r0, int q, int lane, float a_scale, float out_scale) {
+    using S = Gemm3xShape<F16>;
+    // One k-block ahead, across tile boundaries: after issuing k-block j's wgmma group, wait for k-block j + 1's stage
+    // (k-block 0 of the CTA's next tile after a tile's last one) and split its fragments into the other register set;
+    // when j is a tile's k-block 0, the previous tile's epilogue runs there too.  Only then wait for the group, release
+    // its stage and add d to acc.  The group's fragments are held to that wait (wgmma_hold), so the next k-block's split
+    // never lands in a register that an in-flight wgmma still reads.
+    float d[64], acc[64];  // d: the k-block's product (tensor-core accumulation), acc: the tile's sum
+    uint32_t ahi[4][4], alo[4][4], nhi[4][4], nlo[4][4];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int t = blockIdx.x, kb = 0, s = 0;
+    uint32_t ph = 0;
+    if (t >= tiles) return;
+    gemm3x_stage_in<F16, SPLIT_W>(smem, full, 0, r0, q, ACT, a_scale, ahi, alo);
+    for (;;) {  // k-block kb of tile t, from stage s, fragments in ahi / alo
+        gemm3x_issue<F16>(d, ahi, alo, smem + s * S::kStageBytes);
+        const int ns = s + 1 == S::kStages ? 0 : s + 1;
+        const uint32_t nph = ns == 0 ? ph ^ 1 : ph;
+        const bool last = kb + 1 == kblocks;
+        const int nt = last ? t + (int)gridDim.x : t;
+        const bool more = nt < tiles;
+        if (kb == 0 && t != (int)blockIdx.x) {
+            gemm3x_epilogue(p, acc, t - (int)gridDim.x, n_tiles, r0, q, out_scale);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;  // not acc = d below: 0.f + d turns a -0 product into +0
+        }
+        if (more) gemm3x_stage_in<F16, SPLIT_W>(smem + ns * S::kStageBytes, full + ns, nph, r0, q, ACT, a_scale, nhi, nlo);
+        wgmma_wait_all();
+        wgmma_hold(ahi, p.ldc < 0), wgmma_hold(alo, p.ldc < 0);
+        if (lane == 0) mbar_arrive(empty + s);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] += d[i];
+        if (!more) break;
+        s = ns, ph = nph;
+        t = nt, kb = last ? 0 : kb + 1;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) ahi[kk][j] = nhi[kk][j], alo[kk][j] = nlo[kk][j];
+    }
+    gemm3x_epilogue(p, acc, t, n_tiles, r0, q, out_scale);
+}
 
 // F16: fp16 pieces (W given as a pre-scaled fp16 pair).  !F16: TF32 pieces; SPLIT_W: W arrives raw (fp32) in the W_hi slot
 // and the consumer warpgroups split it in place into W_hi / W_lo with the arithmetic of sdetr_split_tf32_pair.
@@ -234,93 +401,10 @@ __global__ void __launch_bounds__(kGThreads, 1)
         a_scale = p.a_scale_dev ? __ldg(p.a_scale_dev) : p.a_scale;
         out_scale = p.a_scale_dev ? 1.f / (a_scale * __ldg(p.w_scale_dev)) : p.out_scale;
     }
-    int s = 0;
-    uint32_t ph = 0;
-    float d[64], acc[64];  // d: the k-block's product (tensor-core accumulation), acc: the tile's sum
-    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-        const int m0 = (t / n_tiles) * kGM, n0 = (t % n_tiles) * kGN;
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-        for (int kb = 0; kb < kblocks; ++kb) {
-            mbar_wait(full + s, ph);
-            const uint8_t *st = smem + s * S::kStageBytes;
-            uint8_t *w_hi = smem + s * S::kStageBytes + S::kABoxes * kGBox, *w_lo = w_hi + kGBox;
-            if (SPLIT_W) {
-                for (int i = threadIdx.x - 128; i < kGBox / 16; i += 256) {
-                    const float4 w = reinterpret_cast<const float4 *>(w_hi)[i];
-                    float4 h, l;
-                    h.x = tf32_rn(w.x), h.y = tf32_rn(w.y), h.z = tf32_rn(w.z), h.w = tf32_rn(w.w);
-                    l.x = tf32_rn(w.x - h.x), l.y = tf32_rn(w.y - h.y), l.z = tf32_rn(w.z - h.z), l.w = tf32_rn(w.w - h.w);
-                    reinterpret_cast<float4 *>(w_hi)[i] = h;
-                    reinterpret_cast<float4 *>(w_lo)[i] = l;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> wgmma operand reads
-                named_bar_sync(1, 256);
-            }
-            // all fragments of the k-block first: registers read by an in-flight wgmma must not be rewritten
-            uint32_t ahi[4][4], alo[4][4];
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                if (F16) {  // m64k16: (r0, c..c+1), (r0+8, c..c+1), (r0, c+8..c+9), (r0+8, c+8..c+9)
-                    const uint8_t *box = st + (kk >> 1) * kGBox;
-                    const int c = (kk & 1) * 16 + 2 * q;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float2 x = *reinterpret_cast<const float2 *>(swz_f32(box, r0 + (j & 1) * 8, c + (j >> 1) * 8));
-                        split2(apply_act(x.x, p.act) * a_scale, apply_act(x.y, p.act) * a_scale, ahi[kk][j], alo[kk][j]);
-                    }
-                } else {  // m64k8: (r0, c), (r0+8, c), (r0, c+4), (r0+8, c+4)
-                    const int c = kk * 8 + q;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float x = apply_act(*swz_f32(st, r0 + (j & 1) * 8, c + (j >> 1) * 4), p.act), h = tf32_rn(x);
-                        ahi[kk][j] = __float_as_uint(h), alo[kk][j] = __float_as_uint(tf32_rn(x - h));
-                    }
-                }
-            }
-            wgmma_fence();
-            const uint32_t bh = smem_u32(w_hi), bl = smem_u32(w_lo);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {  // 32 bytes of K per step in either type
-                if (F16) {
-                    wgmma_f16_rs(d, alo[kk], wgmma_desc(bh + kk * 32), kk);
-                    wgmma_f16_rs(d, ahi[kk], wgmma_desc(bl + kk * 32), 1);
-                    wgmma_f16_rs(d, ahi[kk], wgmma_desc(bh + kk * 32), 1);
-                } else {
-                    wgmma_tf32_rs(d, alo[kk], wgmma_desc(bh + kk * 32), kk);
-                    wgmma_tf32_rs(d, ahi[kk], wgmma_desc(bl + kk * 32), 1);
-                    wgmma_tf32_rs(d, ahi[kk], wgmma_desc(bh + kk * 32), 1);
-                }
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-            if (lane == 0) mbar_arrive(empty + s);
-            if (++s == S::kStages) s = 0, ph ^= 1;
-#pragma unroll
-            for (int i = 0; i < 64; ++i) acc[i] += d[i];
-        }
-        // epilogue: acc[4j + {0,1}] = (row r0, cols 8j + 2q + {0,1}), acc[4j + {2,3}] = (row r0 + 8, same cols)
-        const bool pair = (p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const int col = n0 + 8 * j + 2 * q;
-            if (col >= p.N) continue;
-            const bool two = col + 1 < p.N;
-            const float b0 = p.bias ? __ldg(p.bias + col) : 0.f, b1 = (p.bias && two) ? __ldg(p.bias + col + 1) : 0.f;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = m0 + r0 + 8 * h;
-                if (row >= p.M) continue;
-                float *dst = p.C + (int64_t)row * p.ldc + col;
-                const float v0 = acc[4 * j + 2 * h] * out_scale + b0, v1 = acc[4 * j + 2 * h + 1] * out_scale + b1;
-                if (two && pair) {
-                    *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);
-                } else {
-                    dst[0] = v0;
-                    if (two) dst[1] = v1;
-                }
-            }
-        }
+    switch (p.act) {  // one copy of the loop per activation keeps its test out of the per-element split
+        case 1: gemm3x_consume<F16, SPLIT_W, 1>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        case 2: gemm3x_consume<F16, SPLIT_W, 2>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        default: gemm3x_consume<F16, SPLIT_W, 0>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale);
     }
 }
 

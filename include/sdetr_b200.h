@@ -683,6 +683,32 @@ int sdetr_frozen_bn_fold(const float *w, int Cout, int64_t per_cout, const float
                          float *bias, sdetr_stream_t stream);
 int sdetr_maxpool3x3s2_tokens(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int C, float *y,
                               int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
+/* The projection GEMM of sdetr_gemm_f16x3_scaled (both scales device scalars, no host synchronisation) with the CNBlock
+ * additions: C = z + s * (act(A) . W^T + bias), act applied to A as it loads (0 none, 1 ReLU, 2 exact GELU), s = col_scale (N)
+ * per output column or NULL (none), z = Z (M rows, pitch ldz) or NULL (none).  Z may alias C: every element of z is read by
+ * the thread that writes the same element of C, before it writes it.  |GELU(x)| <= |x|, so a_scale_dev taken over A
+ * (sdetr_pow2_scale, target 12) also bounds the activated values.  K % 64 == 0; A, W_hi, W_lo 16-byte aligned, lda % 4 == 0.
+ * With act 0, col_scale and Z NULL it writes the bits of sdetr_gemm_f16x3_scaled.  One launch. */
+int sdetr_gemm_f16x3_ex(const float *A, int64_t lda, const float *a_scale_dev, const void *W_hi, const void *W_lo,
+                        const float *w_scale_dev, const float *bias, const float *col_scale, const float *Z, int64_t ldz, float *C,
+                        int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream);
+/* ---- ConvNeXt backbone in token layout (models/backbones/convnext.py; ConvNeXtBackbone.forward_tokens) ----------------------
+ * C % 64 == 0 and C <= 1536 for all three; token rows (batch, H * W, C) contiguous; LayerNorms over C with eps, weight and
+ * bias (C); two-pass mean / variance per row in fp32, a NaN in a row's inputs gives a NaN row.  Operands 16-byte aligned.
+ * The stem: y = LayerNorm(conv(x, W) + bias), conv 4x4, stride 4, no padding, 3 -> C.  x: (batch, 3, H, W) NCHW contiguous
+ * fp32; weight (48, C) = W[co, c, ky, kx] at row (c * 4 + ky) * 4 + kx, column co; y: (batch, (H / 4) * (W / 4), C) (torch's
+ * floor: trailing rows / columns are dropped).  fp32 FMAs, taps in (c, ky, kx) order, then the bias.  One launch. */
+int sdetr_convnext_stem(const float *x, int batch, int H, int W, int C, const float *weight, const float *bias,
+                        const float *ln_weight, const float *ln_bias, float eps, float *y, sdetr_stream_t stream);
+/* y = LayerNorm(dwconv(x) + bias): depthwise 7x7, padding 3 (zeros), weight (49, C) = W[c, 0, ky, kx] at row ky * 7 + kx.  y is
+ * (batch, H * W, C) and must not alias x.  One launch. */
+int sdetr_dwconv7x7_layernorm_tokens(const float *x, int batch, int H, int W, int C, const float *weight, const float *bias,
+                                     const float *ln_weight, const float *ln_bias, float eps, float *y, sdetr_stream_t stream);
+/* LayerNorm of token rows written space-to-depth: y (batch, (H / 2) * (W / 2), 4 C), row (oy, ox) holding LayerNorm(x[2 oy + dy,
+ * 2 ox + dx]) at columns (2 dy + dx) * C + c; an odd last row / column is dropped.  A 2x2 / stride-2 convolution is then one
+ * GEMM with K = 4 C against its weight permuted to (Cout, 2, 2, Cin).  y must not alias x.  One launch. */
+int sdetr_layernorm_tokens_s2d(const float *x, int batch, int H, int W, int C, const float *ln_weight, const float *ln_bias,
+                               float eps, float *y, sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

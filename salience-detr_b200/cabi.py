@@ -113,6 +113,10 @@ SIGNATURES = {
     "sdetr_conv2d_f16x3_dgrad": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i64, _i64] + [_i] * 6 +
                                  [_vp, _i64, _i64, _vp]),
     "sdetr_frozen_bn_fold": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, _vp, _vp, _vp, _vp]),
+    "sdetr_gemm_f16x3_ex": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _vp]),
+    "sdetr_convnext_stem": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_dwconv7x7_layernorm_tokens": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_layernorm_tokens_s2d": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp]),
 }
 
 
@@ -1322,4 +1326,102 @@ def maxpool3x3s2_tokens(x, hw, out=None):
         raise RuntimeError(f"maxpool3x3s2_tokens: out must be ({b}, {ho * wo}, {c})")
     rc = lib().sdetr_maxpool3x3s2_tokens(*_token_rows(x, "x"), b, int(H), int(W), c, *_token_rows(y, "out"), _stream())
     _check(rc, "sdetr_maxpool3x3s2_tokens")
+    return y
+
+
+# ---- ConvNeXt backbone in token layout (convnext.ConvNeXtBackbone.forward_tokens) ----------------------------------------------
+ACT_GELU = 2  # gemm_f16x3_ex: exact GELU applied to the input as it loads
+
+
+def gemm_f16x3_ex(x, a_scale, w_hi, w_lo, w_scale, bias=None, act=0, col_scale=None, z=None, out=None):
+    """out = z + col_scale * (act(x) @ W.T + bias) on the projection GEMM (3xFP16, device scales, no host synchronisation).
+    x (..., K) fp32 with unit last stride and rows of a 16-byte multiple; a_scale: pow2_scale of x (target 12); (w_hi, w_lo,
+    w_scale): split_f16_pair_dev of W (N, K); act 0 none, 1 ReLU, 2 exact GELU on x as it loads; col_scale (N) or None; z: a
+    (..., N) tensor of x's leading shape with unit last stride, or None; out: None (a fresh tensor) or such a tensor, which may be
+    z itself."""
+    K = x.shape[-1]
+    N = w_hi.shape[0]
+    if not (x.is_cuda and x.dtype == torch.float32 and x.stride(-1) == 1):
+        raise RuntimeError("gemm_f16x3_ex needs a CUDA float32 input with unit last stride")
+    x2 = x if x.dim() == 2 else x.reshape(-1, K)
+    M = x2.shape[0]
+    lead = tuple(x.shape[:-1])
+
+    def rows(t, name):
+        if not (t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == lead + (N,) and t.stride(-1) == 1):
+            raise RuntimeError(f"gemm_f16x3_ex: {name} must be a CUDA float32 {lead + (N,)} tensor with unit last stride")
+        t2 = t if t.dim() == 2 else t.view(-1, N)
+        return t2, (t2.stride(0) if M > 1 else N)
+
+    y = out if out is not None else torch.empty(*lead, N, device=x.device, dtype=torch.float32)
+    y2, ldc = rows(y, "out")
+    zp, ldz = (None, 0)
+    if z is not None:
+        z2, ldz = rows(z, "z")
+        zp = z2.data_ptr()
+    if col_scale is not None and tuple(col_scale.shape) != (N,):
+        raise RuntimeError(f"gemm_f16x3_ex: col_scale must be ({N},)")
+    rc = lib().sdetr_gemm_f16x3_ex(x2.data_ptr(), x2.stride(0) if M > 1 else K, _req(a_scale, "a_scale", torch.float32),
+                                   _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
+                                   _req(w_scale, "w_scale", torch.float32),
+                                   _req(bias, "bias", torch.float32) if bias is not None else None,
+                                   _req(col_scale, "col_scale", torch.float32) if col_scale is not None else None, zp, ldz,
+                                   y2.data_ptr(), ldc, M, N, K, int(act), _stream())
+    _check(rc, "sdetr_gemm_f16x3_ex")
+    return y
+
+
+def convnext_stem(x, weight, bias, ln_weight, ln_bias, eps: float = 1e-6):
+    """LayerNorm(conv 4x4 / 4 (x) + bias) over C -> (b, (H // 4) * (W // 4), C) token rows.  x: (b, 3, H, W) NCHW contiguous fp32
+    CUDA; weight: (48, C) = W.reshape(C, 48).T, contiguous; bias, ln_weight, ln_bias (C)."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.is_contiguous()):
+        raise RuntimeError("convnext_stem: x must be a contiguous CUDA float32 (b, 3, H, W) tensor")
+    b, _, H, W = x.shape
+    C = weight.shape[1]
+    if weight.dim() != 2 or weight.shape[0] != 48 or any(tuple(t.shape) != (C,) for t in (bias, ln_weight, ln_bias)):
+        raise RuntimeError("convnext_stem: weight must be (48, C) and bias, ln_weight, ln_bias (C)")
+    y = torch.empty(b, (H // 4) * (W // 4), C, device=x.device, dtype=torch.float32)
+    if y.numel() == 0:  # an image under 4 pixels high or wide: no output pixel
+        return y
+    rc = lib().sdetr_convnext_stem(_req(x, "x", torch.float32), b, H, W, C, _req(weight, "weight", torch.float32),
+                                   _req(bias, "bias", torch.float32), _req(ln_weight, "ln_weight", torch.float32),
+                                   _req(ln_bias, "ln_bias", torch.float32), float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_convnext_stem")
+    return y
+
+
+def dwconv7x7_layernorm_tokens(x, hw, weight, bias, ln_weight, ln_bias, eps: float = 1e-6):
+    """LayerNorm(depthwise conv 7x7, padding 3 (x) + bias) over C of (b, H*W, C) contiguous token rows, hw = (H, W) -> a new
+    (b, H*W, C) tensor.  weight: (49, C) = W.reshape(C, 49).T, contiguous."""
+    b, n, C = x.shape
+    H, W = hw
+    if n != H * W:
+        raise RuntimeError(f"dwconv7x7_layernorm_tokens: x has {n} rows per image, the map is {H}x{W}")
+    if tuple(weight.shape) != (49, C) or any(tuple(t.shape) != (C,) for t in (bias, ln_weight, ln_bias)):
+        raise RuntimeError("dwconv7x7_layernorm_tokens: weight must be (49, C) and bias, ln_weight, ln_bias (C)")
+    y = torch.empty_like(x)
+    rc = lib().sdetr_dwconv7x7_layernorm_tokens(_req(x, "x", torch.float32), b, int(H), int(W), C,
+                                                _req(weight, "weight", torch.float32), _req(bias, "bias", torch.float32),
+                                                _req(ln_weight, "ln_weight", torch.float32), _req(ln_bias, "ln_bias", torch.float32),
+                                                float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_dwconv7x7_layernorm_tokens")
+    return y
+
+
+def layernorm_tokens_s2d(x, hw, ln_weight, ln_bias, eps: float = 1e-6):
+    """LayerNorm over C of (b, H*W, C) contiguous token rows, written space-to-depth -> (b, (H // 2) * (W // 2), 4 C) with row
+    (y, x) holding the normalised pixel (2 y + dy, 2 x + dx) at columns (2 dy + dx) * C + c."""
+    b, n, C = x.shape
+    H, W = hw
+    if n != H * W:
+        raise RuntimeError(f"layernorm_tokens_s2d: x has {n} rows per image, the map is {H}x{W}")
+    if any(tuple(t.shape) != (C,) for t in (ln_weight, ln_bias)):
+        raise RuntimeError("layernorm_tokens_s2d: ln_weight and ln_bias must be (C)")
+    y = torch.empty(b, (H // 2) * (W // 2), 4 * C, device=x.device, dtype=torch.float32)
+    if y.numel() == 0:  # a map of one row or column: no output pixel
+        return y
+    rc = lib().sdetr_layernorm_tokens_s2d(_req(x, "x", torch.float32), b, int(H), int(W), C,
+                                          _req(ln_weight, "ln_weight", torch.float32), _req(ln_bias, "ln_bias", torch.float32),
+                                          float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_layernorm_tokens_s2d")
     return y

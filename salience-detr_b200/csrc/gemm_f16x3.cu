@@ -81,6 +81,28 @@ extern "C" int sdetr_gemm_f16x3_scaled(const float *A, int64_t lda, const float 
     return gemm_f16x3_impl(A, lda, W_hi, W_lo, 1.f, a_scale_dev, w_scale_dev, bias, C, ldc, M, N, K, 0, stream);
 }
 
+// The CNBlock form: C = z + s * (act(A) . W^T * out_scale + bias) with device scales (sdetr_gemm_f16x3_ex in the header).
+// |GELU(x)| = |x| Phi(x) <= |x|, so the activation scale taken over A (pow2_scale, target 12) also bounds GELU(A) * a_scale
+// below 2^12: the fp16 split cannot overflow whichever activation is applied on load.
+extern "C" int sdetr_gemm_f16x3_ex(const float *A, int64_t lda, const float *a_scale_dev, const void *W_hi, const void *W_lo,
+                                   const float *w_scale_dev, const float *bias, const float *col_scale, const float *Z, int64_t ldz,
+                                   float *C, int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream) {
+    SDETR_REQUIRE(A && a_scale_dev && W_hi && W_lo && w_scale_dev && C, SDETR_ERR_INVALID_ARG, "gemm_f16x3_ex: null pointer");
+    SDETR_REQUIRE(M >= 0 && N > 0 && K > 0 && act >= 0 && act <= 2, SDETR_ERR_INVALID_ARG, "gemm_f16x3_ex: bad sizes / activation");
+    SDETR_REQUIRE(K % Gemm3xShape<true>::kK == 0, SDETR_ERR_UNSUPPORTED, "gemm_f16x3_ex: K=%d must be a multiple of %d", K,
+                  Gemm3xShape<true>::kK);
+    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && aligned16(W_lo) && lda >= K && ldc >= N &&
+                      (Z == nullptr || ldz >= N),
+                  SDETR_ERR_INVALID_ARG, "gemm_f16x3_ex: operands must be 16-byte aligned with 16-byte row pitch");
+    if (M == 0) return SDETR_OK;
+    CUtensorMap mh, ml;
+    SDETR_REQUIRE(make_map_2d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_hi, N, K, K, 64, kGN) &&
+                      make_map_2d(&ml, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_lo, N, K, K, 64, kGN),
+                  SDETR_ERR_CUDA, "gemm_f16x3_ex: cuTensorMapEncodeTiled failed");
+    const Gemm3xParams p{bias, C, ldc, M, N, K, act, 1.f, 1.f, a_scale_dev, w_scale_dev, col_scale, Z, ldz};
+    return launch_gemm3x<true, false, true>(A, lda, mh, ml, p, stream, "gemm_f16x3_ex");
+}
+
 namespace sdetr {
 __global__ void split_f16_pair_dev_kernel(const float *__restrict__ w, int64_t n, const float *__restrict__ scale_dev,
                                           __half *__restrict__ hi, __half *__restrict__ lo) {

@@ -198,6 +198,9 @@ struct Gemm3xParams {
     float a_scale, out_scale;  // A multiplier before the split and accumulator multiplier (fp16 form; 1 for TF32)
     const float *a_scale_dev;  // fp16 form with device scales: a_scale = *a_scale_dev, out_scale = 1 / (a_scale * *w_scale_dev)
     const float *w_scale_dev;
+    const float *col_scale;    // EX only: per-column scale s (N) or NULL
+    const float *Z;            // EX only: residual z (M rows, pitch ldz) or NULL; may alias C
+    int64_t ldz;
 };
 
 // Consumer side of one k-block, first half: wait until stage `st` has landed (SPLIT_W: split its raw W in place, both
@@ -264,8 +267,10 @@ __device__ __forceinline__ void gemm3x_issue(float (&d)[64], const uint32_t (&ah
     wgmma_commit();
 }
 
-// Epilogue of tile t: C = acc * out_scale + bias.  acc[4j + {0,1}] = (row r0, cols 8j + 2q + {0,1}), acc[4j + {2,3}] =
-// (row r0 + 8, same cols).
+// Epilogue of tile t: C = acc * out_scale + bias (EX: C = z + s * (acc * out_scale + bias), s and z optional; each thread
+// reads its z elements before it writes the same C elements, so z may alias C).  acc[4j + {0,1}] = (row r0, cols
+// 8j + 2q + {0,1}), acc[4j + {2,3}] = (row r0 + 8, same cols).
+template <bool EX>
 __device__ __forceinline__ void gemm3x_epilogue(const Gemm3xParams &p, const float (&acc)[64], int t, int n_tiles, int r0, int q,
                                                 float out_scale) {
     const int m0 = (t / n_tiles) * kGM, n0 = (t % n_tiles) * kGN;
@@ -281,7 +286,14 @@ __device__ __forceinline__ void gemm3x_epilogue(const Gemm3xParams &p, const flo
             const int row = m0 + r0 + 8 * h;
             if (row >= p.M) continue;
             float *dst = p.C + (int64_t)row * p.ldc + col;
-            const float v0 = acc[4 * j + 2 * h] * out_scale + b0, v1 = acc[4 * j + 2 * h + 1] * out_scale + b1;
+            float v0 = acc[4 * j + 2 * h] * out_scale + b0, v1 = acc[4 * j + 2 * h + 1] * out_scale + b1;
+            if (EX) {
+                if (p.col_scale) v0 = __ldg(p.col_scale + col) * v0, v1 = two ? __ldg(p.col_scale + col + 1) * v1 : v1;
+                if (p.Z) {
+                    const float *z = p.Z + (int64_t)row * p.ldz + col;
+                    v0 = z[0] + v0, v1 = two ? z[1] + v1 : v1;
+                }
+            }
             if (two && pair) {
                 *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);
             } else {
@@ -305,7 +317,7 @@ __device__ __forceinline__ void wgmma_hold(const uint32_t (&a)[4][4], bool never
 }
 
 // The consumer loop of gemm3x_kernel, with the input activation fixed at compile time.
-template <bool F16, bool SPLIT_W, int ACT>
+template <bool F16, bool SPLIT_W, bool EX, int ACT>
 __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *smem, uint64_t *full, uint64_t *empty, int tiles,
                                                int n_tiles, int kblocks, int r0, int q, int lane, float a_scale, float out_scale) {
     using S = Gemm3xShape<F16>;
@@ -330,7 +342,7 @@ __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *s
         const int nt = last ? t + (int)gridDim.x : t;
         const bool more = nt < tiles;
         if (kb == 0 && t != (int)blockIdx.x) {
-            gemm3x_epilogue(p, acc, t - (int)gridDim.x, n_tiles, r0, q, out_scale);
+            gemm3x_epilogue<EX>(p, acc, t - (int)gridDim.x, n_tiles, r0, q, out_scale);
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;  // not acc = d below: 0.f + d turns a -0 product into +0
         }
@@ -348,12 +360,13 @@ __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *s
 #pragma unroll
             for (int j = 0; j < 4; ++j) ahi[kk][j] = nhi[kk][j], alo[kk][j] = nlo[kk][j];
     }
-    gemm3x_epilogue(p, acc, t, n_tiles, r0, q, out_scale);
+    gemm3x_epilogue<EX>(p, acc, t, n_tiles, r0, q, out_scale);
 }
 
 // F16: fp16 pieces (W given as a pre-scaled fp16 pair).  !F16: TF32 pieces; SPLIT_W: W arrives raw (fp32) in the W_hi slot
-// and the consumer warpgroups split it in place into W_hi / W_lo with the arithmetic of sdetr_split_tf32_pair.
-template <bool F16, bool SPLIT_W>
+// and the consumer warpgroups split it in place into W_hi / W_lo with the arithmetic of sdetr_split_tf32_pair.  EX: the
+// epilogue also applies the per-column scale and the residual of Gemm3xParams (instances without it compile as before).
+template <bool F16, bool SPLIT_W, bool EX = false>
 __global__ void __launch_bounds__(kGThreads, 1)
     gemm3x_kernel(const __grid_constant__ CUtensorMap ma, const __grid_constant__ CUtensorMap mh,
                   const __grid_constant__ CUtensorMap ml, const Gemm3xParams p) {
@@ -402,9 +415,9 @@ __global__ void __launch_bounds__(kGThreads, 1)
         out_scale = p.a_scale_dev ? 1.f / (a_scale * __ldg(p.w_scale_dev)) : p.out_scale;
     }
     switch (p.act) {  // one copy of the loop per activation keeps its test out of the per-element split
-        case 1: gemm3x_consume<F16, SPLIT_W, 1>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
-        case 2: gemm3x_consume<F16, SPLIT_W, 2>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
-        default: gemm3x_consume<F16, SPLIT_W, 0>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale);
+        case 1: gemm3x_consume<F16, SPLIT_W, EX, 1>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        case 2: gemm3x_consume<F16, SPLIT_W, EX, 2>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        default: gemm3x_consume<F16, SPLIT_W, EX, 0>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale);
     }
 }
 
@@ -440,7 +453,7 @@ inline bool make_map_2d(CUtensorMap *m, CUtensorMapDataType dt, int elem_bytes, 
 }
 
 // A (M,K) fp32 with row pitch lda; W maps made by the caller (F16: fp16 boxes of 64 x 128, else fp32 boxes of 32 x 128)
-template <bool F16, bool SPLIT_W>
+template <bool F16, bool SPLIT_W, bool EX = false>
 inline int launch_gemm3x(const float *A, int64_t lda, const CUtensorMap &mh, const CUtensorMap &ml, const Gemm3xParams &p,
                          sdetr_stream_t stream, const char *what) {
     using S = Gemm3xShape<F16>;
@@ -448,9 +461,9 @@ inline int launch_gemm3x(const float *A, int64_t lda, const CUtensorMap &mh, con
     SDETR_REQUIRE(make_map_2d(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, A, p.M, p.K, lda, 32, kGM), SDETR_ERR_CUDA,
                   "%s: cuTensorMapEncodeTiled failed", what);
     static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, (gemm3x_kernel<F16, SPLIT_W>), S::kSmem, what);
+    SDETR_OPT_IN_SMEM(once, (gemm3x_kernel<F16, SPLIT_W, EX>), S::kSmem, what);
     const int tiles = ((p.N + kGN - 1) / kGN) * ((p.M + kGM - 1) / kGM), ctas = persistent_ctas();
-    gemm3x_kernel<F16, SPLIT_W><<<tiles < ctas ? tiles : ctas, kGThreads, S::kSmem, (cudaStream_t)stream>>>(ma, mh, ml, p);
+    gemm3x_kernel<F16, SPLIT_W, EX><<<tiles < ctas ? tiles : ctas, kGThreads, S::kSmem, (cudaStream_t)stream>>>(ma, mh, ml, p);
     return check_launch(what);
 }
 

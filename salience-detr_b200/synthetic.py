@@ -45,6 +45,29 @@ def resnet_weights(shapes: Mapping[str, Sequence[int]], seed: int = 0) -> "Order
     return out
 
 
+def convnext_weights(shapes: Mapping[str, Sequence[int]], seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for a ConvNeXt state dict of the given key -> shape table (in its order): convolution and Linear weights
+    N(0, 1 / fan_in), their biases N(0, 0.1^2), LayerNorm affines away from (1, 0) -- weight 1 + U(-0.25, 0.25), bias
+    N(0, 0.1^2) -- and layer_scale U(0.05, 1) per channel.  At the 1e-6 layer_scale of the initialisation every block is the
+    identity to fp32 rounding, which would hide any error in it."""
+    g = torch.Generator().manual_seed(seed)
+    out = OrderedDict()
+    for k, shape in shapes.items():
+        shape = tuple(int(v) for v in shape)
+        if k.endswith("layer_scale"):
+            t = 0.05 + torch.rand(shape, generator=g) * 0.95
+        elif len(shape) >= 2:
+            t = torch.randn(shape, generator=g) / math.sqrt(math.prod(shape[1:]))
+        elif k.endswith("bias"):
+            t = torch.randn(shape, generator=g) * 0.1
+        elif k.endswith("weight"):
+            t = 1.0 + (torch.rand(shape, generator=g) - 0.5) * 0.5
+        else:
+            raise ValueError(f"convnext_weights: no rule for {k} {shape}")
+        out[k] = t
+    return out
+
+
 def level_shapes(h: int, w: int, strides: Sequence[int]) -> List[Tuple[int, int]]:
     out: List[Tuple[int, int]] = []
     for i, s in enumerate(strides):

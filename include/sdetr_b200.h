@@ -438,24 +438,19 @@ int sdetr_ffn_fused_layernorm(const float *x, int64_t ldx, const void *W1_hi, co
  * Operands are token rows: pixel (py, px) of image n, channel c at base + n * pitch + (py * W + px) * ld + c (floats), so a
  * level slice of a (b, Nv, C) tensor is an operand as it is.
  *
- * Convolution y = act(conv(x, W) + bias), kernel ksize x ksize (1 or 3), padding ksize / 2, stride 1 or 2, `groups` groups;
- * act 0 none, 3 SiLU.  Implicit GEMM on wgmma with the 3xFP16 arithmetic of sdetr_gemm_f16x3_scaled: x is multiplied by the
- * power-of-two device scalar *a_scale_dev (sdetr_pow2_scale with target 12) before its hi / lo split, W (Cout, ksize, ksize,
- * Cin / groups) row-major was split with *w_scale_dev (sdetr_split_f16_pair_dev), the epilogue divides both out.
- * Cin / groups and Cout / groups multiples of 64 (else SDETR_ERR_UNSUPPORTED); x, x_pitch, ldx 16-byte aligned; y, y_pitch,
- * ldy 8-byte aligned; Ho = (H + 2 (ksize / 2) - ksize) / stride + 1, likewise Wo.  bias may be NULL. */
+ * Convolution y = act(conv(x, W) + bias + z), kernel ksize x ksize (1 or 3), padding ksize / 2, stride 1 or 2, `groups` groups;
+ * act 0 none, 1 ReLU (NaN propagates, as torch.relu), 3 SiLU.  Implicit GEMM on wgmma with the 3xFP16 arithmetic of
+ * sdetr_gemm_f16x3_scaled: x is multiplied by the power-of-two device scalar *a_scale_dev (sdetr_pow2_scale with target 12)
+ * before its hi / lo split, W (Cout, ksize, ksize, Cin / groups) row-major was split with *w_scale_dev
+ * (sdetr_conv2d_f16x3_split_weight or sdetr_split_f16_pair_dev), the epilogue divides both out.  Cin / groups and Cout / groups
+ * multiples of 64 (else SDETR_ERR_UNSUPPORTED); x, x_pitch, ldx 16-byte aligned; y, y_pitch, ldy 8-byte aligned;
+ * Ho = (H + 2 (ksize / 2) - ksize) / stride + 1, likewise Wo.  bias may be NULL.  The residual operand z (token rows, Cout
+ * wide; NULL: none) is added before the activation; z, z_pitch, ldz 8-byte aligned; z may alias y (each element is read before
+ * it is written, by the same thread).  A Bottleneck's conv3 -> bn3 -> += identity -> ReLU is one call. */
 int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin, const float *a_scale_dev,
-                       const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, int Cout, int groups,
-                       int ksize, int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
-/* y = act(conv(x, W) + bias + z): sdetr_conv2d_f16x3 with a residual operand z (token rows, Cout wide; NULL: none) added
- * before the activation, and act 0 none, 1 ReLU (NaN propagates, as torch.relu), 3 SiLU.  z, z_pitch, ldz 8-byte aligned; z may
- * alias y (each element is read before it is written, by the same thread).  sdetr_conv2d_f16x3 is this call with z = NULL (and
- * act 0 or 3): same k-block order and epilogue arithmetic, the same bits.  A Bottleneck's conv3 -> bn3 -> += identity -> ReLU
- * is one call. */
-int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin, const float *a_scale_dev,
-                          const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, const float *z,
-                          int64_t z_pitch, int64_t ldz, int Cout, int groups, int ksize, int stride, int act, float *y,
-                          int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
+                       const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *bias, const float *z,
+                       int64_t z_pitch, int64_t ldz, int Cout, int groups, int ksize, int stride, int act, float *y,
+                       int64_t y_pitch, int64_t ldy, sdetr_stream_t stream);
 /* Context gate of a RepVggPluXBlock (SqueezeAndExcitation, models/bricks/basic.py:29-54, plus the block's residual), per image
  * of HW pixels: p = softmax over the pixels of (y . w_mask + *b_mask); ctx = sum p y; gate = sigmoid(W2 ReLU(W1 ctx)) with
  * w1 (R, C), w2 (C, R) row-major; out = gate * y + x (+ z when z is not NULL).  Three launches; every reduction is summed in a
@@ -471,49 +466,35 @@ int sdetr_context_gate(const float *y, int64_t y_pitch, int64_t ldy, const float
 int sdetr_upsample_nearest_concat(const float *hi, int64_t hi_pitch, int64_t ldh, int Hi, int Wi, const float *lo, int64_t lo_pitch,
                                   int64_t ldl, int Ho, int Wo, int batch, int C, float *dst, int64_t dst_pitch, int64_t ldd,
                                   sdetr_stream_t stream);
-/* Training (RepVGGPluXNetwork.forward_tokens under autograd).  The input gradient of a stride-1 convolution is
- * sdetr_conv2d_f16x3 on dY with the weights flipped in both spatial axes and transposed per group: (Cin, k, k, Cout / groups),
- * W'[g Cin_g + ci, ky, kx, co] = W[g Cout_g + co, ci, k - 1 - ky, k - 1 - kx].  The stride-2 one is this transposed
- * convolution with the same W': dY (Hy x Wy, Cin channels = the forward's Cout) -> dX (H x W, Cout channels = the forward's
- * Cin); output pixel (iy, ix) with tap (ky, kx) reads dY[(iy - pad + ky) / 2, (ix - pad + kx) / 2] when both are even and in
- * range, zero otherwise.  Hy, Wy must be the forward's output size of H, W.  Same operand rules as sdetr_conv2d_f16x3; no bias,
- * no activation. */
-/* One pass over a convolution weight w (Cout, Cin / groups, k, k) in PyTorch's layout with the device scale *scale_dev
- * (sdetr_pow2_scale, target 14): the fp16 pair (fwd_hi, fwd_lo) in sdetr_conv2d_f16x3's (Cout, k, k, Cin / groups) layout and,
- * unless dgrad_hi == dgrad_lo == NULL, the pair of the input-gradient weights W' (Cin, k, k, Cout / groups) described below.
- * The arithmetic of sdetr_split_f16_pair_dev. */
+/* Training.  One pass over a convolution weight w (Cout, Cin / groups, k, k) in PyTorch's layout with the device scale
+ * *scale_dev (sdetr_pow2_scale, target 14): the fp16 pair (fwd_hi, fwd_lo) in sdetr_conv2d_f16x3's (Cout, k, k, Cin / groups)
+ * layout and, unless dgrad_hi == dgrad_lo == NULL, the pair of the input-gradient weights W' (Cin, k, k, Cout / groups),
+ * flipped in both spatial axes and transposed per group: W'[g Cin_g + ci, ky, kx, co] = W[g Cout_g + co, ci, k - 1 - ky,
+ * k - 1 - kx].  The arithmetic of sdetr_split_f16_pair_dev. */
 int sdetr_conv2d_f16x3_split_weight(const float *w, int Cout, int Cin, int groups, int ksize, const float *scale_dev, void *fwd_hi,
                                     void *fwd_lo, void *dgrad_hi, void *dgrad_lo, sdetr_stream_t stream);
-int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
-                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev, int Cout,
-                                  int groups, int ksize, int H, int W, float *dx, int64_t dx_pitch, int64_t lddx,
-                                  sdetr_stream_t stream);
 /* Weight gradient of y = conv(x, W) (the family of sdetr_conv2d_f16x3; x: H x W, Cin channels; dy: Ho x Wo, Cout channels):
  * dw[co, ci, ky, kx] = sum over output pixels of dy[pixel, co] x[shifted pixel, g Cin_g + ci], written fp32 in PyTorch's
  * (Cout, Cin / groups, k, k) layout.  3xFP16 on wgmma: dy and x are multiplied by their power-of-two device scalars
  * (sdetr_pow2_scale, target 12) before the hi / lo split.  The pixel range is split over CTAs by a rule of the shape alone and
- * the partial sums are added in split order: bit-reproducible.  Two launches.  dy, x, their pitches and row strides 16-byte
- * aligned; workspace: sdetr_conv2d_f16x3_wgrad_workspace_floats(batch, Ho, Wo, Cin, Cout, groups, ksize) floats, 16-byte
- * aligned (0 for an unsupported shape). */
+ * the partial sums are added in split order: bit-reproducible.  Each output row co is multiplied by cout_scale[co] (Cout
+ * floats; NULL: none) in the split sum's write, one fp32 product of the same sum: the gradient of a weight W whose forward
+ * ran W * s (a folded FrozenBatchNorm scale s) is this call with s.  Two launches.  dy, x, their pitches and row strides
+ * 16-byte aligned; workspace: sdetr_conv2d_f16x3_wgrad_workspace_floats(batch, Ho, Wo, Cin, Cout, groups, ksize) floats,
+ * 16-byte aligned (0 for an unsupported shape). */
 int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, int Wo, int Cin, int Cout, int groups, int ksize);
 int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
                              int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin, int Cout,
-                             int groups, int ksize, int stride, float *workspace, int64_t workspace_floats, float *dw,
-                             sdetr_stream_t stream);
-/* sdetr_conv2d_f16x3_wgrad with every output row co multiplied by cout_scale[co] (Cout floats; NULL: none) in the split sum's
- * write: one fp32 product of the same sum, so the result is cout_scale[co] times sdetr_conv2d_f16x3_wgrad's, bit for bit.  The
- * gradient of a convolution weight W whose forward ran W * s (a folded FrozenBatchNorm scale s) is this call with s. */
-int sdetr_conv2d_f16x3_wgrad_ex(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
-                                int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin, int Cout,
-                                int groups, int ksize, int stride, const float *cout_scale, float *workspace,
-                                int64_t workspace_floats, float *dw, sdetr_stream_t stream);
+                             int groups, int ksize, int stride, const float *cout_scale, float *workspace, int64_t workspace_floats,
+                             float *dw, sdetr_stream_t stream);
 /* Input gradient of y = conv(x, W) with a fused epilogue: dx = (conv^T(dy, W) + z), then 0 where m <= 0.  dy: Hy x Wy with Cin
- * channels (the forward's Cout); dx: H x W with Cout channels (the forward's Cin); W_hi / W_lo: the input-gradient pair W'
- * (Cin, k, k, Cout / groups) of sdetr_conv2d_f16x3_split_weight.  Stride 1 is sdetr_conv2d_f16x3 on dy with W', stride 2 the
- * transposed mode of sdetr_conv2d_f16x3_transposed: with z = m = NULL the same bits as those calls.  z (token rows, Cout wide;
- * NULL: none) may alias dx (read before written, by the same thread); m (NULL: none) is the ReLU mask source of torch's
- * threshold_backward(grad, m, 0): a NaN in m lets the value through, a NaN value stays NaN; m must not alias dx.  No bias, no
- * activation.  Operand rules of sdetr_conv2d_f16x3; z, m, their pitches and row strides 8-byte aligned. */
+ * channels (the forward's Cout); dx: H x W with Cout channels (the forward's Cin); Hy, Wy must be the forward's output size of
+ * H, W; W_hi / W_lo: the input-gradient pair W' of sdetr_conv2d_f16x3_split_weight.  Stride 1 is sdetr_conv2d_f16x3 on dy with
+ * W'.  Stride 2 is the transposed convolution with W': output pixel (iy, ix) with tap (ky, kx) reads dY[(iy - pad + ky) / 2,
+ * (ix - pad + kx) / 2] when both are even and in range, zero otherwise.  z (token rows, Cout wide; NULL: none) may alias dx
+ * (read before written, by the same thread); m (NULL: none) is the ReLU mask source of torch's threshold_backward(grad, m, 0):
+ * a NaN in m lets the value through, a NaN value stays NaN; m must not alias dx.  No bias, no activation.  Operand rules of
+ * sdetr_conv2d_f16x3; z, m, their pitches and row strides 8-byte aligned. */
 int sdetr_conv2d_f16x3_dgrad(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
                              const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev, const float *z,
                              int64_t z_pitch, int64_t ldz, const float *m, int64_t m_pitch, int64_t ldm, int Cout, int groups,
@@ -677,7 +658,7 @@ int sdetr_resnet_stem(const float *x, int batch, int H, int W, const float *weig
  * row strides 16-byte aligned.  One launch. */
 /* w (Cout, per_cout) fp32 with a FrozenBatchNorm folded in: s = weight * rsqrt(running_var + eps), w_folded = w * s, and (each
  * optional) scale = s, bias = bias - running_mean * s, per output channel.  Computed in float64 with every operation rounded on
- * its own, then rounded to fp32: the values of ResNetBackbone's host fold (backbone._fold), with no host read.  One launch. */
+ * its own, then rounded to fp32: the values of the same fold in float64 torch, with no host read.  One launch. */
 int sdetr_frozen_bn_fold(const float *w, int Cout, int64_t per_cout, const float *bn_weight, const float *bn_bias,
                          const float *running_mean, const float *running_var, double eps, float *w_folded, float *scale,
                          float *bias, sdetr_stream_t stream);

@@ -9,20 +9,21 @@ reference's tensors.  ``forward(x)`` returns ``{"layer{i+1}": map}`` for ``i`` i
 
 ``forward`` is the reference's op chain in torch whenever ``tokens_supported(x)`` does not hold: with autograd, on the CPU, for
 BasicBlock / ResNeXt / dilated / deformable networks and for norms other than this module's ``FrozenBatchNorm2d``.  Otherwise
-it is ``forward_tokens(x)``: every FrozenBatchNorm folded into its convolution once per parameter / buffer version, the stem
-(``sdetr_resnet_stem``, fp32 FMAs from the NCHW image batch), the max-pool (``sdetr_maxpool3x3s2_tokens``) and every
-convolution on ``sdetr_conv2d_f16x3_ex`` (3xFP16 on wgmma, fp32-class accuracy whatever ``allow_tf32`` says) with ReLU and the
-block's residual in the epilogue.  Each returned map is a channels-last NCHW view of its own ``(b, H*W, C)`` token buffer,
+it is ``forward_tokens(x)``: every FrozenBatchNorm folded into its convolution on the device (``sdetr_frozen_bn_fold``, in
+float64 with each operation rounded alone) once per parameter / buffer version, the stem (``sdetr_resnet_stem``, fp32 FMAs
+from the NCHW image batch), the max-pool (``sdetr_maxpool3x3s2_tokens``) and every convolution a ``neck.TokenConv`` on
+``sdetr_conv2d_f16x3`` (3xFP16 on wgmma, fp32-class accuracy whatever ``allow_tf32`` says) with ReLU and the block's residual
+in the epilogue.  Each returned map is a channels-last NCHW view of its own ``(b, H*W, C)`` token buffer,
 which ``ChannelMapper`` reads in place.  No host synchronisation: the call can be captured in a CUDA graph.
 
 Under autograd, ``forward_tokens`` trains the convolutions of layers 1-4 in token layout when ``training_tokens_supported(x)``
 holds (a frozen stem, an image that needs no gradient): one ``torch.autograd.Function`` over the blocks from the first one
-with a trainable weight on.  Every call folds each FrozenBatchNorm into its convolution on the device
-(``sdetr_frozen_bn_fold``, the values of ``_fold``) and splits it into both fp16 layouts (``sdetr_conv2d_f16x3_split_weight``),
-so the forward writes the bits of the inference path and an optimizer step between CUDA-graph replays is seen.  The backward
-runs the whole chain: input gradients on ``sdetr_conv2d_f16x3_dgrad`` with the residual sum (``z``) and the ReLU mask (``m``)
-in its epilogue, weight gradients on ``sdetr_conv2d_f16x3_wgrad_ex`` with the FrozenBatchNorm scale in its write, and only
-the gradients something upstream needs.  ``forward`` itself stays the torch chain under autograd.
+with a trainable weight on.  Every call folds each FrozenBatchNorm into its convolution as inference does and splits it into
+both fp16 layouts (``sdetr_conv2d_f16x3_split_weight``), so the forward writes the bits of the inference path and an
+optimizer step between CUDA-graph replays is seen.  The backward runs the whole chain: input gradients on
+``sdetr_conv2d_f16x3_dgrad`` with the residual sum (``z``) and the ReLU mask (``m``) in its epilogue, weight gradients on
+``sdetr_conv2d_f16x3_wgrad`` with the FrozenBatchNorm scale in its write, and only the gradients something upstream needs.
+``forward`` itself stays the torch chain under autograd.
 """
 from __future__ import annotations
 
@@ -33,7 +34,7 @@ import torch
 from torch import Tensor, nn
 
 from . import cabi, derived
-from .neck import _KConv
+from .neck import TokenConv
 
 
 class FrozenBatchNorm2d(nn.Module):
@@ -206,12 +207,6 @@ class ResNet(nn.Module):
         return nn.Sequential(*layers)
 
 
-def _fold(conv: nn.Conv2d, bn: FrozenBatchNorm2d) -> Tuple[Tensor, Tensor]:
-    """(W * scale, bias - running_mean * scale) in float64, scale = weight * rsqrt(running_var + eps)"""
-    scale = bn.weight.double() * (bn.running_var.double() + bn.eps).rsqrt()
-    return conv.weight.double() * scale.view(-1, 1, 1, 1), bn.bias.double() - bn.running_mean.double() * scale
-
-
 class ResNetBackbone(nn.Module):
     # name -> ResNet arguments (the reference's model_arch table, without the download URLs)
     model_arch = {
@@ -337,11 +332,34 @@ class ResNetBackbone(nn.Module):
         convolution (the blocks before it neither train nor carry a gradient), and the index of each stage's last block"""
         blocks = [blk for layer in self._stages() for blk in layer]
         first = next(i for i, blk in enumerate(blocks) if any(c.weight.requires_grad for c in _block_convs(blk)))
-        stage_end, n = [], 0
+        return blocks, first, self._stage_ends()
+
+    def _stage_ends(self) -> List[int]:
+        """the index of each kept stage's last Bottleneck, counting the blocks of all kept stages in order"""
+        ends, n = [], 0
         for layer in self._stages():
             n += len(layer)
-            stage_end.append(n - 1)
-        return blocks, first, stage_end
+            ends.append(n - 1)
+        return ends
+
+    def _folded(self, dgrad_from: Optional[int] = None):
+        """(stem, convs): every FrozenBatchNorm folded into its convolution on the device (sdetr_frozen_bn_fold).  stem: the
+        folded (147, 64) weight and bias of sdetr_resnet_stem; convs: per Bottleneck of the kept stages in order, its (conv1,
+        conv2, conv3, downsample or None) as TokenConvs with the FrozenBatchNorm scale for the weight gradient, the blocks from
+        index ``dgrad_from`` on with the input-gradient weights too"""
+        w, _, b = cabi.frozen_bn_fold(self.conv1.weight.detach().contiguous(), self.bn1, scale=False)
+        stem = (w.view(64, 147).t().contiguous(), b)
+
+        def conv(c: nn.Conv2d, bn: FrozenBatchNorm2d, act: int, dgrad: bool) -> TokenConv:
+            wf, scale, bias = cabi.frozen_bn_fold(c.weight.detach().contiguous(), bn)
+            return TokenConv(wf, bias, 1, c.stride[0], act, dgrad, scale)
+
+        relu, convs = cabi.ACT_RELU, []
+        for j, blk in enumerate(blk for layer in self._stages() for blk in layer):
+            d, ds = dgrad_from is not None and j >= dgrad_from, blk.downsample
+            convs.append((conv(blk.conv1, blk.bn1, relu, d), conv(blk.conv2, blk.bn2, relu, d), conv(blk.conv3, blk.bn3, relu, d),
+                          conv(ds[0], ds[1], 0, d) if ds is not None else None))
+        return stem, convs
 
     def launches_per_training_step(self) -> int:
         """library launches of one forward_tokens under autograd and its backward (training_tokens_supported): the stem's fold,
@@ -370,33 +388,18 @@ class ResNetBackbone(nn.Module):
         """forward_tokens under autograd (training_tokens_supported): the blocks before the first trainable one as in inference,
         the rest through _TrainBlocks; the same channels-last views, with the bits of the inference path"""
         blocks, first, stage_end = self._train_plan()
-        ks = []
-        for j, blk in enumerate(blocks):
-            ds = blk.downsample
-            ks.append((_TConv(blk.conv1, blk.bn1, j >= first), _TConv(blk.conv2, blk.bn2, j >= first),
-                       _TConv(blk.conv3, blk.bn3, j >= first), _TConv(ds[0], ds[1], j >= first) if ds is not None else None))
-        stem_w, _, stem_b = cabi.frozen_bn_fold(self.conv1.weight.detach(), self.bn1, scale=False)
-        b, _, H, W = x.shape
-        hw = ((H - 1) // 2 + 1, (W - 1) // 2 + 1)
-        t = cabi.resnet_stem(x, stem_w.view(64, 147).t().contiguous(), stem_b)
-        t = cabi.maxpool3x3s2_tokens(t, hw)
-        hw = ((hw[0] - 1) // 2 + 1, (hw[1] - 1) // 2 + 1)
+        stem, ks = self._folded(dgrad_from=first)
+        t, hw = _stem(x, stem)
         feats = {}
-        for j in range(first):  # inference: nothing saved, conv3 writes over the residual in place
-            c1, c2, c3, ds = ks[j]
-            s = cabi.pow2_scale(t, 12)
-            y1 = c1(t, hw, s)
-            y2 = c2(y1, hw, cabi.pow2_scale(y1, 12))
-            s2 = cabi.pow2_scale(y2, 12)
-            hw2 = c2.out_hw(hw)
-            ident = ds(t, hw, s, act=0) if ds is not None else t
-            t, hw = c3(y2, hw2, s2, out=ident, z=ident), hw2
+        for j in range(first):  # as in inference: nothing saved
+            t, hw = _bottleneck(ks[j], t, hw)
             if j in stage_end:
                 feats[stage_end.index(j)] = (t, hw)
-        weights = [c.weight for k in ks[first:] for c in k if c is not None and c.trainable]
+        trainable = [[c.weight.requires_grad for c in _block_convs(blk)] for blk in blocks[first:]]
+        weights = [c.weight for blk in blocks[first:] for c in _block_convs(blk) if c.weight.requires_grad]
         ends = [stage_end.index(j) if j in stage_end and stage_end.index(j) in self.return_indices else None
                 for j in range(first, len(blocks))]
-        run = _TrainRun(ks[first:], ends, hw)
+        run = _TrainRun(ks[first:], trainable, ends, hw)
         outs = _TrainBlocks.apply(run, t, *weights)
         for i, o in zip(run.returned, outs):
             feats[i] = (o, run.out_hw[i])
@@ -407,24 +410,8 @@ class ResNetBackbone(nn.Module):
         return res
 
     def _kernel_weights(self):
-        """the folded stem ((147, 64) weight, bias) and per stage per block the (conv1, conv2, conv3, downsample or None)
-        convolutions in kernel form, rebuilt when any parameter or buffer changes"""
-        def build():
-            w, b = _fold(self.conv1, self.bn1)
-            stem = (w.reshape(64, 147).t().float().contiguous(), b.float().contiguous())
-            relu = cabi.ACT_RELU
-            stages = []
-            for layer in self._stages():
-                blocks = []
-                for blk in layer:
-                    ds = blk.downsample
-                    blocks.append((_KConv(*_fold(blk.conv1, blk.bn1), 1, 1, relu),
-                                   _KConv(*_fold(blk.conv2, blk.bn2), 1, blk.conv2.stride[0], relu),
-                                   _KConv(*_fold(blk.conv3, blk.bn3), 1, 1, relu),
-                                   _KConv(*_fold(ds[0], ds[1]), 1, ds[0].stride[0], 0) if ds is not None else None))
-                stages.append(blocks)
-            return stem, stages
-        return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), build)
+        """_folded() for inference, rebuilt when any parameter or buffer changes"""
+        return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), self._folded)
 
     def launches_per_forward(self) -> int:
         """library launches of one forward_tokens: the stem, the max-pool, and per convolution 2 (activation scale +
@@ -435,10 +422,6 @@ class ResNetBackbone(nn.Module):
                 n += 6 + (1 if blk.downsample is not None else 0)
         return n
 
-    @staticmethod
-    def _conv(k: _KConv, x: Tensor, hw, scale: Tensor, out=None, z=None) -> Tensor:
-        return cabi.conv2d_f16x3(x, hw, scale, k.w_hi, k.w_lo, k.w_scale, k.bias, 1, k.ksize, k.stride, k.act, out=out, z=z)
-
     def forward_tokens(self, x: Tensor) -> Dict[str, Tensor]:
         """The backbone on ``x`` (b, 3, H, W) -> {"layer{i+1}": (b, C, h, w)} for i in return_indices, each a channels-last view
         (strides (h*w*C, 1, w*C, C)) of its own (b, h*w, C) token buffer; the values of forward() in torch.  No host
@@ -447,25 +430,13 @@ class ResNetBackbone(nn.Module):
             if self.training_tokens_supported(x):
                 return self._train_tokens(x)
             raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported)")
-        (stem_w, stem_b), stages = self._kernel_weights()
-        b, _, H, W = x.shape
-        hw = ((H - 1) // 2 + 1, (W - 1) // 2 + 1)
-        t = cabi.resnet_stem(x, stem_w, stem_b)
-        t = cabi.maxpool3x3s2_tokens(t, hw)
-        hw = ((hw[0] - 1) // 2 + 1, (hw[1] - 1) // 2 + 1)
-        feats = []
-        for blocks in stages:
-            for c1, c2, c3, ds in blocks:
-                s = cabi.pow2_scale(t, 12)
-                y1 = self._conv(c1, t, hw, s)
-                y2 = self._conv(c2, y1, hw, cabi.pow2_scale(y1, 12))
-                s2 = cabi.pow2_scale(y2, 12)
-                hw2 = ((hw[0] - 1) // c2.stride + 1, (hw[1] - 1) // c2.stride + 1)
-                # the residual is the downsample's fresh output, or a block input that only this block reads (an earlier block
-                # of the same stage): conv3 writes over it in place
-                ident = self._conv(ds, t, hw, s) if ds is not None else t
-                t, hw = self._conv(c3, y2, hw2, s2, out=ident, z=ident), hw2
-            feats.append((t, hw))
+        stem, convs = self._kernel_weights()
+        t, hw = _stem(x, stem)
+        feats, stage_end = [], self._stage_ends()
+        for j, ks in enumerate(convs):
+            t, hw = _bottleneck(ks, t, hw)
+            if j in stage_end:
+                feats.append((t, hw))
         outs = {}
         for i in self.return_indices:
             t, (h, w) = feats[i]
@@ -483,36 +454,33 @@ def _block_convs(blk: Bottleneck) -> List[nn.Conv2d]:
     return [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
 
 
-class _TConv:
-    """one convolution of the training path, folded and split in this call: the forward pair, the input-gradient pair (for the
-    blocks the backward runs through), the folded bias and the FrozenBatchNorm scale s (the weight gradient is s * wgrad)"""
+def _stem(x: Tensor, stem) -> Tuple[Tensor, Tuple[int, int]]:
+    """the stem and the max-pool: the image batch x -> layer 1's input token rows and map size"""
+    _, _, H, W = x.shape
+    hw = ((H - 1) // 2 + 1, (W - 1) // 2 + 1)
+    t = cabi.maxpool3x3s2_tokens(cabi.resnet_stem(x, *stem), hw)
+    return t, ((hw[0] - 1) // 2 + 1, (hw[1] - 1) // 2 + 1)
 
-    def __init__(self, conv: nn.Conv2d, bn: FrozenBatchNorm2d, backward: bool):
-        self.weight, self.trainable = conv.weight, conv.weight.requires_grad
-        self.ksize, self.stride, self.shape = conv.kernel_size[0], conv.stride[0], tuple(conv.weight.shape)
-        wf, self.scale, self.bias = cabi.frozen_bn_fold(conv.weight.detach(), bn)
-        self.w_hi, self.w_lo, self.d_hi, self.d_lo, self.w_scale = cabi.conv2d_f16x3_split_weight(wf, 1, backward)
 
-    def out_hw(self, hw):
-        return tuple((v - 1) // self.stride + 1 for v in hw)
-
-    def __call__(self, x: Tensor, hw, scale: Tensor, act: int = cabi.ACT_RELU, out=None, z=None) -> Tensor:
-        return cabi.conv2d_f16x3(x, hw, scale, self.w_hi, self.w_lo, self.w_scale, self.bias, 1, self.ksize, self.stride, act,
-                                 out=out, z=z)
-
-    def dgrad(self, g: Tensor, g_hw, g_scale: Tensor, hw, z=None, m=None, out=None) -> Tensor:
-        return cabi.conv2d_f16x3_dgrad(g, g_hw, g_scale, self.d_hi, self.d_lo, self.w_scale, 1, self.ksize, self.stride, hw, z=z, m=m,
-                                       out=out)
-
-    def wgrad(self, g: Tensor, g_scale: Tensor, x: Tensor, x_scale: Tensor, hw) -> Tensor:
-        return cabi.conv2d_f16x3_wgrad(g, g_scale, x, x_scale, hw, self.shape, self.stride, cout_scale=self.scale)
+def _bottleneck(convs, t: Tensor, hw) -> Tuple[Tensor, Tuple[int, int]]:
+    """one Bottleneck without autograd: (conv1, conv2, conv3, downsample or None) TokenConvs on the token rows t of an hw map
+    -> the block's output rows and map size.  The residual is the downsample's fresh output, or a block input that only this
+    block reads (an earlier block of the same stage): conv3 writes over it in place."""
+    c1, c2, c3, ds = convs
+    s = cabi.pow2_scale(t, 12)
+    y1 = c1(t, hw, s)
+    y2 = c2(y1, hw, cabi.pow2_scale(y1, 12))
+    s2 = cabi.pow2_scale(y2, 12)
+    ident = ds(t, hw, s) if ds is not None else t
+    return c3(y2, c2.out_hw(hw), s2, out=ident, z=ident), c2.out_hw(hw)
 
 
 class _TrainRun:
-    """what _TrainBlocks needs beyond tensors: per block its convolutions and the stage it ends (or None), the input map size"""
+    """what _TrainBlocks needs beyond tensors: per block its TokenConvs, whether each of their weights trains (conv1, conv2,
+    conv3, the downsample's if any) and the stage it ends (or None), the input map size"""
 
-    def __init__(self, convs, ends, hw):
-        self.convs, self.ends, self.hw = convs, ends, hw
+    def __init__(self, convs, trainable, ends, hw):
+        self.convs, self.trainable, self.ends, self.hw = convs, trainable, ends, hw
         self.returned = [i for i in ends if i is not None]
         self.out_hw = {}
 
@@ -537,7 +505,7 @@ class _TrainBlocks(torch.autograd.Function):
             s2 = cabi.pow2_scale(y2, 12)
             hw2 = c2.out_hw(hw)
             if ds is not None:
-                ident = ds(t, hw, s, act=0)
+                ident = ds(t, hw, s)
                 out = c3(y2, hw2, s2, out=ident, z=ident)
             else:
                 out = c3(y2, hw2, s2, z=t)  # a fresh output: the block input is kept for the backward
@@ -565,31 +533,32 @@ class _TrainBlocks(torch.autograd.Function):
         G = torch.ops.aten.threshold_backward(ext[run.returned[-1]], saved[-1], 0)
         for j in range(nblk - 1, -1, -1):
             c1, c2, c3, ds = run.convs[j]
+            tr = run.trainable[j]
             t, s, y1, s1, y2, s2 = saved[6 * j: 6 * j + 6]
             hw, hw2 = hws[j], hws[j + 1]
             need_in = j > 0
             gs = cabi.pow2_scale(G, 12)
             blk_dw = {}
-            if c3.trainable:
+            if tr[2]:
                 blk_dw[3] = c3.wgrad(G, gs, y2, s2, hw2)
-            if c2.trainable or c1.trainable or need_in:
-                dy2 = c3.dgrad(G, hw2, gs, hw2, m=y2)
+            if tr[1] or tr[0] or need_in:
+                dy2 = c3.dgrad(G, hw2, gs, m=y2)
                 s_dy2 = cabi.pow2_scale(dy2, 12)
-                if c2.trainable:
+                if tr[1]:
                     blk_dw[2] = c2.wgrad(dy2, s_dy2, y1, s1, hw)
-                if c1.trainable or need_in:
-                    dy1 = c2.dgrad(dy2, hw2, s_dy2, hw, m=y1)
+                if tr[0] or need_in:
+                    dy1 = c2.dgrad(dy2, hw, s_dy2, m=y1)
                     s_dy1 = cabi.pow2_scale(dy1, 12)
-                    if c1.trainable:
+                    if tr[0]:
                         blk_dw[1] = c1.wgrad(dy1, s_dy1, t, s, hw)
-            if ds is not None and ds.trainable:
+            if ds is not None and tr[3]:
                 blk_dw[4] = ds.wgrad(G, gs, t, s, hw)
             if need_in:
                 z = ext.get(run.ends[j - 1]) if run.ends[j - 1] is not None else None
                 if ds is not None:
-                    d = ds.dgrad(G, hw2, gs, hw, z=z)
+                    d = ds.dgrad(G, hw, gs, z=z)
                 else:
                     d = G if z is None else G + z
-                G = c1.dgrad(dy1, hw, s_dy1, hw, z=d, m=t, out=d)
+                G = c1.dgrad(dy1, hw, s_dy1, z=d, m=t, out=d)
             dws.append([blk_dw[i] for i in (1, 2, 3, 4) if i in blk_dw])
         return (None, None) + tuple(dw for blk in reversed(dws) for dw in blk)

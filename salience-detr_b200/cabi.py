@@ -80,16 +80,15 @@ SIGNATURES = {
     "sdetr_mha_out_proj_ln_scatter": (_i, [_vp] * 6 + [_f, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "sdetr_rows_gather_add": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sdetr_rows_scatter": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    "sdetr_conv2d_f16x3": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
+    "sdetr_conv2d_f16x3": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i, _i, _i, _i, _i,
+                                _vp, _i64, _i64, _vp]),
     "sdetr_context_gate_workspace_floats": (_i64, [_i, _i, _i]),
     "sdetr_context_gate": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp,
                                 _i64, _i64, _vp]),
     "sdetr_upsample_nearest_concat": (_i, [_vp, _i64, _i64, _i, _i, _vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
     "sdetr_conv2d_f16x3_split_weight": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "sdetr_conv2d_f16x3_transposed": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i64, _i64,
-                                           _vp]),
     "sdetr_conv2d_f16x3_wgrad_workspace_floats": (_i64, [_i] * 7),
-    "sdetr_conv2d_f16x3_wgrad": (_i, [_vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp] + [_i] * 8 + [_vp, _i64, _vp, _vp]),
+    "sdetr_conv2d_f16x3_wgrad": (_i, [_vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp] + [_i] * 8 + [_vp, _vp, _i64, _vp, _vp]),
     "sdetr_upsample_nearest_concat_backward": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
     "sdetr_group_norm_tokens_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
     "sdetr_group_norm_tokens": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _i, _f, _vp, _i64, _vp]),
@@ -105,11 +104,8 @@ SIGNATURES = {
     "sdetr_cdn_loss_indices": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "sdetr_postprocess_workspace": (_sz, [_i, _i, _i]),
     "sdetr_postprocess": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp] + [_i] * 5 + [_f, _f] + [_vp] * 5 + [_sz, _vp]),
-    "sdetr_conv2d_f16x3_ex": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i, _i, _i, _i, _i, _vp,
-                                   _i64, _i64, _vp]),
     "sdetr_resnet_stem": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "sdetr_maxpool3x3s2_tokens": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
-    "sdetr_conv2d_f16x3_wgrad_ex": (_i, [_vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp] + [_i] * 8 + [_vp, _vp, _i64, _vp, _vp]),
     "sdetr_conv2d_f16x3_dgrad": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i64, _i64] + [_i] * 6 +
                                  [_vp, _i64, _i64, _vp]),
     "sdetr_frozen_bn_fold": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, _vp, _vp, _vp, _vp]),
@@ -922,12 +918,12 @@ def conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, w_scale, bias, groups: int, ksize: 
     xp, xpitch, ldx = _token_rows(x, "x")
     yp, ypitch, ldy = _token_rows(y, "out")
     zp = _token_rows(z, "z") if z is not None else (None, 0, 0)
-    rc = lib().sdetr_conv2d_f16x3_ex(xp, xpitch, ldx, b, H, W, cin, _req(a_scale, "a_scale", torch.float32),
-                                     _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
-                                     _req(w_scale, "w_scale", torch.float32),
-                                     _req(bias, "bias", torch.float32) if bias is not None else None, *zp, cout, int(groups),
-                                     int(ksize), int(stride), int(act), yp, ypitch, ldy, _stream())
-    _check(rc, "sdetr_conv2d_f16x3_ex")
+    rc = lib().sdetr_conv2d_f16x3(xp, xpitch, ldx, b, H, W, cin, _req(a_scale, "a_scale", torch.float32),
+                                  _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
+                                  _req(w_scale, "w_scale", torch.float32),
+                                  _req(bias, "bias", torch.float32) if bias is not None else None, *zp, cout, int(groups),
+                                  int(ksize), int(stride), int(act), yp, ypitch, ldy, _stream())
+    _check(rc, "sdetr_conv2d_f16x3")
     return y
 
 
@@ -979,26 +975,10 @@ def conv2d_f16x3_split_weight(w, groups: int, dgrad: bool = True):
     return f_hi, f_lo, d_hi, d_lo, scale
 
 
-def conv2d_f16x3_transposed(dy, dy_hw, a_scale, w_hi, w_lo, w_scale, groups: int, ksize: int, hw):
-    """Input gradient of a stride-2 convolution of an (H, W) = hw map: dy (b, Hy*Wy, Cout) view, W' = the (Cin, k, k, Cout / groups)
-    flipped, per-group transposed weights as a split_f16_pair_dev pair; a_scale: pow2_scale of dy (target 12).  -> (b, H*W, Cin)."""
-    b, n, cin = dy.shape
-    if n != dy_hw[0] * dy_hw[1]:
-        raise RuntimeError(f"conv2d_f16x3_transposed: dy has {n} rows per image, the map is {dy_hw[0]}x{dy_hw[1]}")
-    cout = w_hi.shape[0]
-    dx = torch.empty(b, hw[0] * hw[1], cout, device=dy.device, dtype=torch.float32)
-    rc = lib().sdetr_conv2d_f16x3_transposed(*_token_rows(dy, "dy")[:3], b, int(dy_hw[0]), int(dy_hw[1]), cin,
-                                             _req(a_scale, "a_scale", torch.float32), _req(w_hi, "w_hi", torch.float16),
-                                             _req(w_lo, "w_lo", torch.float16), _req(w_scale, "w_scale", torch.float32), cout,
-                                             int(groups), int(ksize), int(hw[0]), int(hw[1]), *_token_rows(dx, "dx"), _stream())
-    _check(rc, "sdetr_conv2d_f16x3_transposed")
-    return dx
-
-
 def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int, cout_scale=None):
     """Weight gradient (Cout, Cin / groups, k, k) of y = conv(x, W): dy (b, Ho*Wo, Cout), x (b, H*W, Cin) views with unit channel
     stride, hw = (H, W); dy_scale / x_scale: their pow2_scale device scalars (target 12).  Bit-reproducible.
-    cout_scale: optional (Cout,) fp32 factor per output channel, applied in the split sum's write (sdetr_conv2d_f16x3_wgrad_ex)."""
+    cout_scale: optional (Cout,) fp32 factor per output channel, applied in the split sum's write."""
     b, _, cin = x.shape
     cout, cin_g, k, _ = (int(v) for v in weight_shape)
     groups = cin // cin_g
@@ -1009,19 +989,13 @@ def conv2d_f16x3_wgrad(dy, dy_scale, x, x_scale, hw, weight_shape, stride: int, 
     dw = torch.empty(cout, cin_g, k, k, device=x.device, dtype=torch.float32)
     ws = torch.empty(max(int(lib().sdetr_conv2d_f16x3_wgrad_workspace_floats(b, ho, wo, cin, cout, groups, k)), 4), device=x.device,
                      dtype=torch.float32)
-    if cout_scale is None:
-        rc = lib().sdetr_conv2d_f16x3_wgrad(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
-                                            _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
-                                            int(stride), ws.data_ptr(), ws.numel(), dw.data_ptr(), _stream())
-        _check(rc, "sdetr_conv2d_f16x3_wgrad")
-        return dw
-    if cout_scale.numel() != cout:
+    if cout_scale is not None and cout_scale.numel() != cout:
         raise RuntimeError(f"conv2d_f16x3_wgrad: cout_scale must have {cout} entries")
-    rc = lib().sdetr_conv2d_f16x3_wgrad_ex(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
-                                           _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
-                                           int(stride), _req(cout_scale, "cout_scale", torch.float32), ws.data_ptr(), ws.numel(),
-                                           dw.data_ptr(), _stream())
-    _check(rc, "sdetr_conv2d_f16x3_wgrad_ex")
+    cs = _req(cout_scale, "cout_scale", torch.float32) if cout_scale is not None else None
+    rc = lib().sdetr_conv2d_f16x3_wgrad(*_token_rows(dy, "dy"), _req(dy_scale, "dy_scale", torch.float32), *_token_rows(x, "x"),
+                                        _req(x_scale, "x_scale", torch.float32), b, int(hw[0]), int(hw[1]), cin, cout, groups, k,
+                                        int(stride), cs, ws.data_ptr(), ws.numel(), dw.data_ptr(), _stream())
+    _check(rc, "sdetr_conv2d_f16x3_wgrad")
     return dw
 
 
@@ -1051,7 +1025,7 @@ def conv2d_f16x3_dgrad(dy, dy_hw, a_scale, w_hi, w_lo, w_scale, groups: int, ksi
 
 def frozen_bn_fold(w, bn, scale: bool = True, bias: bool = True):
     """(w * s, s, bias - running_mean * s) of a weight (Cout, ...) and a FrozenBatchNorm2d ``bn`` (s = weight * rsqrt(running_var
-    + eps)), computed on the device in float64 and rounded to fp32 (sdetr_frozen_bn_fold): backbone._fold's values, no host read.
+    + eps)), computed on the device in float64 and rounded to fp32 (sdetr_frozen_bn_fold), with no host read.
     s / the bias are None unless asked for."""
     cout = w.shape[0]
     wf = torch.empty(w.shape, device=w.device, dtype=torch.float32)

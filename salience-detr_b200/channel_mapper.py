@@ -24,7 +24,7 @@ import torch
 from torch import Tensor, nn
 
 from . import cabi, derived
-from .neck import Conv2dNormActivation, _KConv
+from .neck import Conv2dNormActivation, TokenConv
 
 
 # ---- the token-buffer view layout: both directions ----------------------------------------------------------------------
@@ -138,8 +138,8 @@ class ChannelMapper(nn.Module):
     def _kernel_weights(self):
         """convolutions in kernel form and the (L, C) GroupNorm affine tables, rebuilt when any parameter changes"""
         def build():
-            convs = [_KConv(m[0].weight.detach(), m[0].bias.detach() if m[0].bias is not None else None, m[0].groups,
-                            m[0].stride[0], 0) for m in self.convs]
+            convs = [TokenConv(m[0].weight.detach().float(), m[0].bias.detach().float() if m[0].bias is not None else None,
+                               m[0].groups, m[0].stride[0]) for m in self.convs]
             gn = [m[1] for m in self.convs]
             ones = torch.ones(gn[0].num_channels, device=self.convs[0][0].weight.device)
             gamma = torch.stack([n.weight.detach() if n.affine else ones for n in gn]).float().contiguous()
@@ -183,13 +183,13 @@ class ChannelMapper(nn.Module):
         level = [out[:, s:s + n] for s, n in zip(starts, sizes)]
         rows = [self._token_rows(x) for x in xs]
         for i in range(n_in):
-            convs[i](rows[i], rows[i], shapes[i], out=level[i])
+            convs[i](rows[i], shapes[i], cabi.pow2_scale(rows[i], 12), out=level[i])
         if n_out > n_in:  # the first extra level reads the last input's token rows
-            convs[n_in](rows[-1], rows[-1], shapes[n_in - 1], out=level[n_in])
+            convs[n_in](rows[-1], shapes[n_in - 1], cabi.pow2_scale(rows[-1], 12), out=level[n_in])
         first = min(n_out, n_in + 1)
         cabi.group_norm_tokens_(out[:, :starts[first - 1] + sizes[first - 1]], sizes[:first], gamma[:first], beta[:first], groups,
                                 eps)
         for i in range(n_in + 1, n_out):
-            convs[i](level[i - 1], out, shapes[i - 1], out=level[i])
+            convs[i](level[i - 1], shapes[i - 1], cabi.pow2_scale(out, 12), out=level[i])
             cabi.group_norm_tokens_(level[i], sizes[i:i + 1], gamma[i:i + 1], beta[i:i + 1], groups, eps)
         return out, shapes

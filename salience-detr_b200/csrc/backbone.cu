@@ -1,12 +1,12 @@
 // ResNet backbone in token layout (ResNetBackbone.forward_tokens): the two kernels before the first Bottleneck.  Every
-// convolution of the blocks is sdetr_conv2d_f16x3_ex (neck.cu).
+// convolution of the blocks is sdetr_conv2d_f16x3 (neck.cu).
 //
 //   sdetr_resnet_stem            conv 7x7, stride 2, padding 3, 3 -> 64 channels, folded FrozenBatchNorm bias and ReLU, from
 //                                the NCHW fp32 image batch to (b, Ho*Wo, 64) token rows.  Plain fp32 FMAs on the CUDA cores, taps
 //                                summed in (channel, ky, kx) order: the stem is under 3 % of the backbone's operations.
 //   sdetr_maxpool3x3s2_tokens    3x3 / stride 2 / padding 1 max-pool on token rows, 16-byte channel vectors.
 //   sdetr_frozen_bn_fold         a convolution weight with its FrozenBatchNorm folded in, on the device (the training path
-//                                re-folds every call): the float64 arithmetic of backbone._fold, each operation rounded alone.
+//                                re-folds every call): float64 arithmetic, each operation rounded alone.
 #include <math.h>
 
 #include "common.cuh"

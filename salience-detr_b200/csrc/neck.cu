@@ -1,15 +1,20 @@
-// RepVGG-PluX neck in token layout (models/necks/repnet.py:125-245): the three kernels behind
-// RepVGGPluXNetwork.forward_tokens.
+// Token-layout convolutions (the RepVGG-PluX neck, the ChannelMapper and the ResNet backbone) and the neck's other kernels
+// (models/necks/repnet.py:125-245).
 //
-//   sdetr_conv2d_f16x3(_ex)       implicit-GEMM convolution (k = 1 or 3, stride 1 or 2, padding k / 2, groups), bias, optional
+//   sdetr_conv2d_f16x3            implicit-GEMM convolution (k = 1 or 3, stride 1 or 2, padding k / 2, groups), bias, optional
 //                                 residual operand and none / ReLU / SiLU epilogue.  Same 3xFP16 arithmetic as sdetr_gemm_f16x3_scaled: the activation is
 //                                 multiplied by a power-of-two device scalar, split into fp16 hi / lo in registers and used as
 //                                 the wgmma A operand; the weight arrives as a pre-split pair (scale 2^s, also a device scalar);
 //                                 lo.hi + hi.lo + hi.hi per 16-wide k step, and every 64-wide k-block's tensor-core sum is added
 //                                 into fp32 registers with round-to-nearest adds.
+//   sdetr_conv2d_f16x3_dgrad      its input gradient (stride 1: the same kernel on dY with flipped weights; stride 2: the
+//                                 kernel's transposed mode), residual gradient and ReLU mask in the epilogue.
+//   sdetr_conv2d_f16x3_wgrad      its weight gradient (split over the pixel range, splits summed in order), with an optional
+//                                 per-output-channel scale.
+//   sdetr_conv2d_f16x3_split_weight  the fp16 weight pairs of the forward and the input gradient, in one pass.
 //   sdetr_context_gate            SqueezeAndExcitation (models/bricks/basic.py:29-54, a GCNet attention pool) + the block's
 //                                 residual: out = sigmoid(W2 ReLU(W1 ctx)) * y + x (+ z), ctx = softmax(y . w_mask + b_mask) . y.
-//   sdetr_upsample_nearest_concat [nearest(hi) | lo] into one 2C-wide operand (torch's nearest index rule).
+//   sdetr_upsample_nearest_concat [nearest(hi) | lo] into one 2C-wide operand (torch's nearest index rule), and its backward.
 //
 // Operands are token rows: pixel (py, px) of image n, channel c at base + n * pitch + (py * W + px) * ld + c (floats), so a
 // level slice of a (b, Nv, C) tensor is a valid operand without a copy.
@@ -54,7 +59,7 @@ __device__ __forceinline__ void cp_async_wait_1() { asm volatile("cp.async.wait_
 __device__ __forceinline__ float silu(float x) { return x / (1.f + expf(-x)); }
 
 // TRANSPOSED: the input gradient of a stride-2 convolution.  x is dY (H x W), y is dX (Ho x Wo), W the flipped, per-group
-// transposed weights (see sdetr_conv2d_f16x3_transposed); output pixel (oy, ox) with tap (ky, kx) reads x[(oy - pad + ky) / 2,
+// transposed weights (see sdetr_conv2d_f16x3_dgrad); output pixel (oy, ox) with tap (ky, kx) reads x[(oy - pad + ky) / 2,
 // (ox - pad + kx) / 2] when both are even and in range, and zero otherwise.
 template <bool TRANSPOSED>
 __global__ void __launch_bounds__(kCvThreads) conv_f16x3_kernel(const ConvParams p) {
@@ -526,10 +531,10 @@ inline int elementwise_blocks(int64_t total) {
 
 using namespace sdetr;
 
-extern "C" int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
-                                     const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
-                                     const float *bias, const float *z, int64_t z_pitch, int64_t ldz, int Cout, int groups,
-                                     int ksize, int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
+extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
+                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
+                                  const float *bias, const float *z, int64_t z_pitch, int64_t ldz, int Cout, int groups, int ksize,
+                                  int stride, int act, float *y, int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
     SDETR_REQUIRE(x && a_scale_dev && W_hi && W_lo && w_scale_dev && y, SDETR_ERR_INVALID_ARG, "conv2d_f16x3: null pointer");
     SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
                   "conv2d_f16x3: bad sizes");
@@ -558,48 +563,6 @@ extern "C" int sdetr_conv2d_f16x3_ex(const float *x, int64_t x_pitch, int64_t ld
     return check_launch("conv2d_f16x3");
 }
 
-extern "C" int sdetr_conv2d_f16x3(const float *x, int64_t x_pitch, int64_t ldx, int batch, int H, int W, int Cin,
-                                  const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
-                                  const float *bias, int Cout, int groups, int ksize, int stride, int act, float *y,
-                                  int64_t y_pitch, int64_t ldy, sdetr_stream_t stream) {
-    SDETR_REQUIRE(act == 0 || act == kActSiLU, SDETR_ERR_UNSUPPORTED,
-                  "conv2d_f16x3: takes kernel 1 or 3, stride 1 or 2, act 0 (none) or 3 (SiLU)");
-    return sdetr_conv2d_f16x3_ex(x, x_pitch, ldx, batch, H, W, Cin, a_scale_dev, W_hi, W_lo, w_scale_dev, bias, nullptr, 0, 0, Cout,
-                                 groups, ksize, stride, act, y, y_pitch, ldy, stream);
-}
-
-extern "C" int sdetr_conv2d_f16x3_transposed(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,
-                                             const float *a_scale_dev, const void *W_hi, const void *W_lo, const float *w_scale_dev,
-                                             int Cout, int groups, int ksize, int H, int W, float *dx, int64_t dx_pitch,
-                                             int64_t lddx, sdetr_stream_t stream) {
-    SDETR_REQUIRE(dy && a_scale_dev && W_hi && W_lo && w_scale_dev && dx, SDETR_ERR_INVALID_ARG,
-                  "conv2d_f16x3_transposed: null pointer");
-    SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
-                  "conv2d_f16x3_transposed: bad sizes");
-    SDETR_REQUIRE(ksize == 1 || ksize == 3, SDETR_ERR_UNSUPPORTED, "conv2d_f16x3_transposed: takes kernel 1 or 3");
-    SDETR_REQUIRE(Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kCvK == 0 && (Cout / groups) % kCvN == 0,
-                  SDETR_ERR_UNSUPPORTED, "conv2d_f16x3_transposed: Cin/groups=%d and Cout/groups=%d must be multiples of 64",
-                  Cin / groups, Cout / groups);
-    const int pad = ksize / 2, hy = H > 0 ? (H + 2 * pad - ksize) / 2 + 1 : 0, wy = W > 0 ? (W + 2 * pad - ksize) / 2 + 1 : 0;
-    SDETR_REQUIRE(Hy == hy && Wy == wy, SDETR_ERR_INVALID_ARG,
-                  "conv2d_f16x3_transposed: dY is %dx%d, a stride-2 convolution of %dx%d gives %dx%d", Hy, Wy, H, W, hy, wy);
-    SDETR_REQUIRE(rows_ok(dy, dy_pitch, lddy) && lddy >= Cin && aligned16(W_hi) && aligned16(W_lo), SDETR_ERR_INVALID_ARG,
-                  "conv2d_f16x3_transposed: dy, its pitch and row stride and the weights must be 16-byte aligned");
-    SDETR_REQUIRE((reinterpret_cast<uintptr_t>(dx) & 7) == 0 && dx_pitch % 2 == 0 && lddx % 2 == 0 && lddx >= Cout,
-                  SDETR_ERR_INVALID_ARG, "conv2d_f16x3_transposed: dx, its pitch and row stride must be 8-byte aligned");
-    const int64_t M = (int64_t)batch * H * W;
-    SDETR_REQUIRE(M < (1LL << 31) - kCvM, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_transposed: too many output pixels");
-    if (M == 0) return SDETR_OK;
-    static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, conv_f16x3_kernel<true>, kCvSmem, "conv2d_f16x3_transposed");
-    const ConvParams p{dy, dy_pitch, lddy, reinterpret_cast<const __half *>(W_hi), reinterpret_cast<const __half *>(W_lo), a_scale_dev,
-                       w_scale_dev, nullptr, nullptr, 0, 0, nullptr, 0, 0, dx, dx_pitch, lddx, Hy, Wy, H, W, (int)M, Cin / groups,
-                       Cout / groups, ksize, 2, 0};
-    const dim3 grid((unsigned)((M + kCvM - 1) / kCvM), (unsigned)(Cout / kCvN));
-    conv_f16x3_kernel<true><<<grid, kCvThreads, kCvSmem, (cudaStream_t)stream>>>(p);
-    return check_launch("conv2d_f16x3_transposed");
-}
-
 extern "C" int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, int Wo, int Cin, int Cout, int groups, int ksize) {
     if (batch <= 0 || Ho <= 0 || Wo <= 0 || !wgrad_shape_ok(Cin, Cout, groups, ksize)) return 0;
     const int tiles = (Cout / kCvM) * ((Cin / groups) / kCvN) * ksize * ksize;
@@ -608,10 +571,10 @@ extern "C" int64_t sdetr_conv2d_f16x3_wgrad_workspace_floats(int batch, int Ho, 
     return (int64_t)splits * Cout * (Cin / groups) * ksize * ksize;
 }
 
-extern "C" int sdetr_conv2d_f16x3_wgrad_ex(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev,
-                                           const float *x, int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H,
-                                           int W, int Cin, int Cout, int groups, int ksize, int stride, const float *cout_scale,
-                                           float *workspace, int64_t workspace_floats, float *dw, sdetr_stream_t stream) {
+extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev,
+                                        const float *x, int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H,
+                                        int W, int Cin, int Cout, int groups, int ksize, int stride, const float *cout_scale,
+                                        float *workspace, int64_t workspace_floats, float *dw, sdetr_stream_t stream) {
     SDETR_REQUIRE(dy && dy_scale_dev && x && x_scale_dev && dw && workspace, SDETR_ERR_INVALID_ARG, "conv2d_f16x3_wgrad: null pointer");
     SDETR_REQUIRE(batch >= 0 && H >= 0 && W >= 0 && Cin > 0 && Cout > 0 && groups > 0, SDETR_ERR_INVALID_ARG,
                   "conv2d_f16x3_wgrad: bad sizes");
@@ -641,14 +604,6 @@ extern "C" int sdetr_conv2d_f16x3_wgrad_ex(const float *dy, int64_t dy_pitch, in
     wgrad_reduce_kernel<<<elementwise_blocks(n), 256, 0, (cudaStream_t)stream>>>(workspace, splits, n, cout_scale,
                                                                                   n / Cout, dw);
     return check_launch("conv2d_f16x3_wgrad (split sum)");
-}
-
-extern "C" int sdetr_conv2d_f16x3_wgrad(const float *dy, int64_t dy_pitch, int64_t lddy, const float *dy_scale_dev, const float *x,
-                                        int64_t x_pitch, int64_t ldx, const float *x_scale_dev, int batch, int H, int W, int Cin,
-                                        int Cout, int groups, int ksize, int stride, float *workspace, int64_t workspace_floats,
-                                        float *dw, sdetr_stream_t stream) {
-    return sdetr_conv2d_f16x3_wgrad_ex(dy, dy_pitch, lddy, dy_scale_dev, x, x_pitch, ldx, x_scale_dev, batch, H, W, Cin, Cout, groups,
-                                       ksize, stride, nullptr, workspace, workspace_floats, dw, stream);
 }
 
 extern "C" int sdetr_conv2d_f16x3_dgrad(const float *dy, int64_t dy_pitch, int64_t lddy, int batch, int Hy, int Wy, int Cin,

@@ -12,12 +12,13 @@ each RepVGG block's ``conv1 (3x3) + alpha * conv2 (1x1)`` into one grouped 3x3 c
 CSP layer's ``conv1 || conv2`` (two 1x1 over the same input) into one projection.  The kernels (``include/sdetr_b200.h``):
 ``sdetr_conv2d_f16x3`` (implicit-GEMM convolution, 3xFP16 on wgmma, bias + SiLU epilogue), ``sdetr_context_gate``
 (SqueezeAndExcitation + the block's residual) and ``sdetr_upsample_nearest_concat`` (the top-down path's operand).
+``TokenConv`` is the convolution in kernel form, which the ChannelMapper and the ResNet backbone use too.
 
 In training, or whenever autograd records (``training_tokens_supported``), ``forward_tokens`` follows the reference's op
 structure instead of the folded one: every convolution (a RepVGG block's 3x3 and 1x1, a CSP layer's conv1 and conv2 apart) runs
 on the same kernel through an autograd Function.  Its forward splits the weight once (``sdetr_conv2d_f16x3_split_weight``) into
-both fp16 layouts; its backward is the input gradient (``sdetr_conv2d_f16x3`` on dY with the flipped, per-group transposed
-weights; ``sdetr_conv2d_f16x3_transposed`` for stride 2) and ``sdetr_conv2d_f16x3_wgrad``.  Each
+both fp16 layouts; its backward is the input gradient (``sdetr_conv2d_f16x3_dgrad`` with the flipped, per-group transposed
+weights) and the weight gradient (``sdetr_conv2d_f16x3_wgrad``).  Each
 BatchNorm is the module itself on the channels-last ``(b, C, H, W)`` view of the token rows (no copy), so batch statistics, running statistics,
 ``momentum``, eval mode with gradients and ``nn.SyncBatchNorm`` behave as the modules define.  SiLU, the context gate, the
 residuals and the concatenations are torch ops on token rows; the top-down operand's backward is
@@ -172,6 +173,38 @@ def nearest_ranges(n_in: int, n_out: int) -> Tuple[Tensor, Tensor]:
     return torch.searchsorted(src, s, right=False), torch.searchsorted(src, s, right=True)
 
 
+class TokenConv:
+    """One convolution on token rows (sdetr_conv2d_f16x3 and its gradients), padding k / 2.  Built from an fp32 (Cout, Cin /
+    groups, k, k) weight, split here (conv2d_f16x3_split_weight) into the forward's fp16 pair and, with ``dgrad``, the input
+    gradient's; ``bias``: fp32 (Cout) or None; ``act``: 0, cabi.ACT_RELU or cabi.ACT_SILU; ``bn_scale``: an optional (Cout)
+    factor of the weight gradient (a FrozenBatchNorm scale folded into the weight).  The caller passes each activation scale
+    (cabi.pow2_scale, target 12), so convolutions that read the same tensor share one."""
+
+    def __init__(self, w: Tensor, bias: Optional[Tensor], groups: int = 1, stride: int = 1, act: int = 0, dgrad: bool = False,
+                 bn_scale: Optional[Tensor] = None):
+        self.shape, self.groups, self.stride, self.act = tuple(w.shape), groups, stride, act
+        self.w_hi, self.w_lo, self.d_hi, self.d_lo, self.w_scale = cabi.conv2d_f16x3_split_weight(w.contiguous(), groups, dgrad)
+        self.bias, self.bn_scale = bias, bn_scale
+
+    def out_hw(self, hw):
+        k = self.shape[-1]
+        return tuple((v + 2 * (k // 2) - k) // self.stride + 1 for v in hw)
+
+    def __call__(self, x: Tensor, hw, a_scale: Tensor, out=None, z=None) -> Tensor:
+        """act(conv(x) + bias (+ z)): x (b, H*W, Cin) view of an (H, W) = hw map; out, z: optional (b, Ho*Wo, Cout) views"""
+        return cabi.conv2d_f16x3(x, hw, a_scale, self.w_hi, self.w_lo, self.w_scale, self.bias, self.groups, self.shape[-1],
+                                 self.stride, self.act, out=out, z=z)
+
+    def dgrad(self, g: Tensor, hw, g_scale: Tensor, z=None, m=None, out=None) -> Tensor:
+        """the input gradient (+ z, then 0 where m <= 0) of the (H, W) = hw map from g (b, Ho*Wo, Cout)"""
+        return cabi.conv2d_f16x3_dgrad(g, self.out_hw(hw), g_scale, self.d_hi, self.d_lo, self.w_scale, self.groups,
+                                       self.shape[-1], self.stride, hw, z=z, m=m, out=out)
+
+    def wgrad(self, g: Tensor, g_scale: Tensor, x: Tensor, x_scale: Tensor, hw) -> Tensor:
+        """the weight gradient (times bn_scale) from g (b, Ho*Wo, Cout) and the input x of the (H, W) = hw map"""
+        return cabi.conv2d_f16x3_wgrad(g, g_scale, x, x_scale, hw, self.shape, self.stride, cout_scale=self.bn_scale)
+
+
 class _TokenConv2d(torch.autograd.Function):
     """y = conv2d(x, weight) on token rows, no bias (every convolution of the training path is followed by a BatchNorm).
     x: (b, H*W, Cin) view; a_scale: pow2_scale (target 12) of a contiguous tensor that holds x, shared by the convolutions that
@@ -179,11 +212,11 @@ class _TokenConv2d(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, a_scale, hw, stride):
-        groups, k = x.shape[2] // weight.shape[1], weight.shape[-1]
-        w_hi, w_lo, ctx.d_hi, ctx.d_lo, ctx.w_scale = cabi.conv2d_f16x3_split_weight(weight.detach(), groups, ctx.needs_input_grad[0])
-        y = cabi.conv2d_f16x3(x, hw, a_scale, w_hi, w_lo, ctx.w_scale, None, groups, k, stride, 0)
+        conv = TokenConv(weight.detach(), None, x.shape[2] // weight.shape[1], stride, dgrad=ctx.needs_input_grad[0])
+        y = conv(x, hw, a_scale)
+        conv.w_hi = conv.w_lo = None  # the backward reads only the input-gradient pair
         ctx.save_for_backward(x, a_scale)
-        ctx.hw, ctx.stride, ctx.groups, ctx.w_shape = hw, stride, groups, weight.shape
+        ctx.conv, ctx.hw = conv, hw
         return y
 
     @staticmethod
@@ -191,16 +224,8 @@ class _TokenConv2d(torch.autograd.Function):
         x, a_scale = ctx.saved_tensors
         gy = gy.contiguous()  # the BatchNorm gradients this path produces already are: no copy
         g_scale = cabi.pow2_scale(gy, 12)
-        k, pad = ctx.w_shape[-1], ctx.w_shape[-1] // 2
-        ho, wo = ((v + 2 * pad - k) // ctx.stride + 1 for v in ctx.hw)
-        dx = dw = None
-        if ctx.needs_input_grad[0]:
-            if ctx.stride == 1:
-                dx = cabi.conv2d_f16x3(gy, (ho, wo), g_scale, ctx.d_hi, ctx.d_lo, ctx.w_scale, None, ctx.groups, k, 1, 0)
-            else:
-                dx = cabi.conv2d_f16x3_transposed(gy, (ho, wo), g_scale, ctx.d_hi, ctx.d_lo, ctx.w_scale, ctx.groups, k, ctx.hw)
-        if ctx.needs_input_grad[1]:
-            dw = cabi.conv2d_f16x3_wgrad(gy, g_scale, x, a_scale, ctx.hw, ctx.w_shape, ctx.stride)
+        dx = ctx.conv.dgrad(gy, ctx.hw, g_scale) if ctx.needs_input_grad[0] else None
+        dw = ctx.conv.wgrad(gy, g_scale, x, a_scale, ctx.hw) if ctx.needs_input_grad[1] else None
         return dx, dw, None, None, None
 
 
@@ -233,20 +258,6 @@ def _gate_rows(se: SqueezeAndExcitation, y: Tensor) -> Tensor:
     ctx = torch.bmm(p.unsqueeze(1), y).squeeze(1)
     gate = torch.sigmoid(F.linear(F.relu(F.linear(ctx, se.se_module[0].weight.view(-1, c))), se.se_module[2].weight.view(c, -1)))
     return gate.unsqueeze(1) * y
-
-
-class _KConv:
-    """one folded convolution in kernel form: (Cout, k, k, Cin / groups) fp16 pair with its device scale, fp32 bias (or None)"""
-
-    def __init__(self, w: Tensor, b: Optional[Tensor], groups: int, stride: int, act: int):
-        self.ksize, self.groups, self.stride, self.act = w.shape[-1], groups, stride, act
-        self.w_hi, self.w_lo, self.w_scale = cabi.split_f16_pair_dev(w.float().permute(0, 2, 3, 1).contiguous())
-        self.bias = b.float().contiguous() if b is not None else None
-
-    def __call__(self, x: Tensor, base: Tensor, hw, out=None) -> Tensor:
-        """x: (b, H*W, Cin) token view inside the contiguous tensor ``base`` (its activation scale is taken over base)"""
-        return cabi.conv2d_f16x3(x, hw, cabi.pow2_scale(base, 12), self.w_hi, self.w_lo, self.w_scale, self.bias, self.groups,
-                                 self.ksize, self.stride, self.act, out=out)
 
 
 class _KGate:
@@ -377,12 +388,13 @@ class RepVGGPluXNetwork(nn.Module):
     def _kernel_weights(self):
         """folded eval weights in kernel form, rebuilt when any parameter or buffer changes (in place or replaced)"""
         def build():
-            silu = cabi.ACT_SILU
-            f = dict(lateral=[_KConv(*fold_conv_norm(m, torch.float64), 1, 1, silu) for m in self.lateral_convs],
-                     down=[_KConv(*fold_conv_norm(m, torch.float64), 1, 2, silu) for m in self.downsample_blocks])
+            def conv(wb, groups=1, stride=1):  # (weight, bias) folded in float64
+                return TokenConv(wb[0].float(), wb[1].float(), groups, stride, cabi.ACT_SILU)
+            f = dict(lateral=[conv(fold_conv_norm(m, torch.float64)) for m in self.lateral_convs],
+                     down=[conv(fold_conv_norm(m, torch.float64), stride=2) for m in self.downsample_blocks])
             for name in ("layer_blocks", "pan_blocks"):
-                f[name] = [(_KConv(*fold_csp_projection(layer, torch.float64), 1, 1, silu),
-                            [(_KConv(*fold_repvgg(blk, torch.float64), blk.conv1[0].groups, 1, silu), _KGate(blk.se_module))
+                f[name] = [(conv(fold_csp_projection(layer, torch.float64)),
+                            [(conv(fold_repvgg(blk, torch.float64), blk.conv1[0].groups), _KGate(blk.se_module))
                              for blk in layer.bottlenecks]) for layer in getattr(self, name)]
             return f
         return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), build)
@@ -396,11 +408,11 @@ class RepVGGPluXNetwork(nn.Module):
 
     def _csp(self, f, x: Tensor, hw, dst: Tensor):
         proj_conv, blocks = f
-        proj = proj_conv(x, x, hw)  # (b, HW, 2C): [SiLU(BN(conv1(x))) | SiLU(BN(conv2(x)))]
+        proj = proj_conv(x, hw, cabi.pow2_scale(x, 12))  # (b, HW, 2C): [SiLU(BN(conv1(x))) | SiLU(BN(conv2(x)))]
         c = proj.shape[2] // 2
         cur, base = proj[:, :, :c], proj
         for i, (conv, gate) in enumerate(blocks):
-            y = conv(cur, base, hw)
+            y = conv(cur, hw, cabi.pow2_scale(base, 12))
             last = i == len(blocks) - 1
             cur = cabi.context_gate(y, cur, gate.w_mask, gate.b_mask, gate.w1, gate.w2, z=proj[:, :, c:] if last else None,
                                     out=dst if last else None)
@@ -466,12 +478,12 @@ class RepVGGPluXNetwork(nn.Module):
         feat_high, base = lv[-1], memory
         for idx in range(levels - 1, 0, -1):
             lat = bu[idx][:, :, c:]
-            f["lateral"][idx - 1](feat_high, base, shapes_list[idx], out=lat)
+            f["lateral"][idx - 1](feat_high, shapes_list[idx], cabi.pow2_scale(base, 12), out=lat)
             cat = cabi.upsample_nearest_concat(lat, shapes_list[idx], lv[idx - 1], shapes_list[idx - 1])
             dst = outs[0] if idx == 1 else torch.empty(b, sizes[idx - 1], c, device=memory.device, dtype=torch.float32)
             self._csp(f["layer_blocks"][idx - 1], cat, shapes_list[idx - 1], dst)
             feat_high, base = dst, dst
         for idx in range(levels - 1):
-            f["down"][idx](outs[idx], out, shapes_list[idx], out=bu[idx + 1][:, :, :c])
+            f["down"][idx](outs[idx], shapes_list[idx], cabi.pow2_scale(out, 12), out=bu[idx + 1][:, :, :c])
             self._csp(f["pan_blocks"][idx], bu[idx + 1], shapes_list[idx + 1], outs[idx + 1])
         return out

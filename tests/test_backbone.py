@@ -241,9 +241,9 @@ def test_conv_epilogue_vs_fp64(k, stride, cin, cout, mode):
 @pytest.mark.gpu
 @pytest.mark.parametrize("k,stride,groups,c,act", [(3, 1, 4, 256, 3), (3, 2, 1, 256, 3), (1, 1, 1, 512, 3), (1, 1, 1, 256, 0),
                                                    (3, 1, 4, 256, 0)])
-def test_old_entry_point_bit_identical(k, stride, groups, c, act):
-    """sdetr_conv2d_f16x3 (the neck's and the mapper's entry point) and sdetr_conv2d_f16x3_ex with z = NULL or z = 0 write the
-    same bits, at the neck's shapes (config-2 level 1: 50 x 84, C 256, groups 4)"""
+def test_conv_zero_residual_bit_identical(k, stride, groups, c, act):
+    """sdetr_conv2d_f16x3 with z = NULL (the neck's and the mapper's calls) and with z = 0 write the same bits, at the neck's
+    shapes (config-2 level 1: 50 x 84, C 256, groups 4)"""
     gen = torch.Generator().manual_seed(k + 10 * stride + groups + c + act)
     b, h, w = 2, 50, 84
     x = torch.randn(b, h * w, c, generator=gen).to(DEV)
@@ -254,17 +254,12 @@ def test_old_entry_point_bit_identical(k, stride, groups, c, act):
     ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
     old = torch.full((b, ho * wo, c), float("nan"), device=DEV)
     rc = pkg.cabi.lib().sdetr_conv2d_f16x3(x.data_ptr(), x.stride(0), x.stride(1), b, h, w, c, s.data_ptr(), w_hi.data_ptr(),
-                                           w_lo.data_ptr(), w_scale.data_ptr(), bias.data_ptr(), c, groups, k, stride, act,
-                                           old.data_ptr(), old.stride(0), old.stride(1), pkg.cabi._stream())
+                                           w_lo.data_ptr(), w_scale.data_ptr(), bias.data_ptr(), None, 0, 0, c, groups, k, stride,
+                                           act, old.data_ptr(), old.stride(0), old.stride(1), pkg.cabi._stream())
     assert rc == 0
     new = pkg.cabi.conv2d_f16x3(x, (h, w), s, w_hi, w_lo, w_scale, bias, groups, k, stride, act)
     zero = pkg.cabi.conv2d_f16x3(x, (h, w), s, w_hi, w_lo, w_scale, bias, groups, k, stride, act, z=torch.zeros_like(old))
     assert torch.equal(old, new) and torch.equal(old, zero)
-    # the old entry point still takes only act 0 / 3
-    rc = pkg.cabi.lib().sdetr_conv2d_f16x3(x.data_ptr(), x.stride(0), x.stride(1), b, h, w, c, s.data_ptr(), w_hi.data_ptr(),
-                                           w_lo.data_ptr(), w_scale.data_ptr(), None, c, groups, k, stride, 1, old.data_ptr(),
-                                           old.stride(0), old.stride(1), pkg.cabi._stream())
-    assert rc != 0
 
 
 # ---- GPU: forward_tokens ------------------------------------------------------------------------------------------------

@@ -298,22 +298,18 @@ def test_dgrad_mask_nan_rules():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("k,stride,c", [(3, 1, 64), (1, 1, 256), (3, 2, 128), (1, 2, 256), (3, 1, 256)])
-def test_dgrad_without_epilogue_is_the_old_entry_points(k, stride, c):
-    """z = m = NULL: the bits of sdetr_conv2d_f16x3 (stride 1, flipped weights) / sdetr_conv2d_f16x3_transposed (stride 2)"""
-    gen = torch.Generator().manual_seed(k + 10 * stride + c)
+@pytest.mark.parametrize("k,c", [(3, 64), (1, 256), (3, 256), (1, 64), (3, 128)])
+def test_stride1_dgrad_is_the_forward_on_flipped_weights(k, c):
+    """z = m = NULL, stride 1: the bits of sdetr_conv2d_f16x3 on dY with the flipped weights"""
+    gen = torch.Generator().manual_seed(k + 10 + c)
     b, h, w = 2, 50, 84
-    ho, wo = (h - 1) // stride + 1, (w - 1) // stride + 1
     wt = (torch.randn(c, c, k, k, generator=gen) / (c * k * k) ** 0.5).to(DEV)
-    dy = torch.randn(b, ho * wo, c, generator=gen).to(DEV)
+    dy = torch.randn(b, h * w, c, generator=gen).to(DEV)
     _, _, d_hi, d_lo, ws = cabi.conv2d_f16x3_split_weight(wt, 1, True)
     s = cabi.pow2_scale(dy, 12)
-    new = cabi.conv2d_f16x3_dgrad(dy, (ho, wo), s, d_hi, d_lo, ws, 1, k, stride, (h, w))
-    if stride == 1:
-        old = cabi.conv2d_f16x3(dy, (ho, wo), s, d_hi, d_lo, ws, None, 1, k, 1, 0)
-    else:
-        old = cabi.conv2d_f16x3_transposed(dy, (ho, wo), s, d_hi, d_lo, ws, 1, k, (h, w))
-    assert torch.equal(old, new)
+    dgrad = cabi.conv2d_f16x3_dgrad(dy, (h, w), s, d_hi, d_lo, ws, 1, k, 1, (h, w))
+    forward = cabi.conv2d_f16x3(dy, (h, w), s, d_hi, d_lo, ws, None, 1, k, 1, 0)
+    assert torch.equal(forward, dgrad)
 
 
 @pytest.mark.gpu
@@ -335,12 +331,18 @@ def test_wgrad_scale_is_the_scaled_unscaled_result(k, stride, cin, cout):
     assert float((scaled.cpu().double() - ref).abs().max()) <= 1e-5 * float(ref.abs().max())
 
 
+def _fold(conv, bn):
+    """(W * scale, bias - running_mean * scale) in float64 torch, scale = weight * rsqrt(running_var + eps)"""
+    scale = bn.weight.double() * (bn.running_var.double() + bn.eps).rsqrt()
+    return conv.weight.double() * scale.view(-1, 1, 1, 1), bn.bias.double() - bn.running_mean.double() * scale
+
+
 @pytest.mark.gpu
-def test_fold_is_the_host_fold():
+def test_device_fold_is_the_float64_fold():
     m = _backbone().to(DEV)
     for conv, bn in ((m.conv1, m.bn1), (m.layer3[1].conv2, m.layer3[1].bn2), (m.layer4[0].downsample[0], m.layer4[0].downsample[1])):
         bn.running_var.mul_(torch.rand_like(bn.running_var) + 0.5)
-        w, b = bbm._fold(conv, bn)
+        w, b = _fold(conv, bn)
         wf, s, bf = cabi.frozen_bn_fold(conv.weight.detach(), bn)
         s64 = bn.weight.double() * (bn.running_var.double() + bn.eps).rsqrt()
         assert torch.equal(wf, w.float()) and torch.equal(bf, b.float()) and torch.equal(s, s64.float())

@@ -26,7 +26,7 @@ def _equal(a, b) -> bool:
         return torch.is_tensor(b) and a.shape == b.shape and a.dtype == b.dtype and torch.equal(a, b)
     if isinstance(a, np.ndarray):
         return np.array_equal(a, b)
-    if hasattr(a, "__dict__"):  # neck.py's _KConv / _KGate
+    if hasattr(a, "__dict__"):  # neck.py's TokenConv / _KGate
         return type(a) is type(b) and _equal(vars(a), vars(b))
     return a == b
 

@@ -1,5 +1,5 @@
 """RepVGG-PluX neck training in token layout: RepVGGPluXNetwork.forward_tokens under autograd and its kernels
-(sdetr_conv2d_f16x3_wgrad, sdetr_conv2d_f16x3_transposed, sdetr_upsample_nearest_concat_backward).
+(sdetr_conv2d_f16x3_wgrad, sdetr_conv2d_f16x3_dgrad, sdetr_upsample_nearest_concat_backward).
 
 Gradient tolerances follow tests/test_training_gradients.py: each tensor is compared as max|g - g64| / max|g64| against a float64
 twin, and the bound is a multiple of the same quantity for the fp32 torch path (forward() on cuDNN with TF32 off)."""
@@ -30,7 +30,7 @@ FP32_MULTIPLE = 16.0
 
 
 # ---- no GPU needed --------------------------------------------------------------------------------------------------------
-def test_argument_validation():
+def test_training_entry_points_reject_bad_arguments():
     import __graft_entry__ as entry
     entry.build()
     lib = pkg.cabi.lib()
@@ -40,8 +40,8 @@ def test_argument_validation():
     assert ws >= 256 * 64 * 9
     assert lib.sdetr_conv2d_f16x3_wgrad_workspace_floats(2, 13, 21, 96, 96, 1, 3) == 0
     assert lib.sdetr_conv2d_f16x3_wgrad_workspace_floats(2, 13, 21, 256, 128, 4, 3) == 0  # Cout / groups = 32: rejected below too
-    rc = lib.sdetr_conv2d_f16x3_wgrad(p, 1092 * 128, 128, p, p, 4 * 273 * 256, 256, p, 2, 26, 42, 256, 128, 4, 3, 2, p, 1 << 30, p,
-                                      None)
+    rc = lib.sdetr_conv2d_f16x3_wgrad(p, 1092 * 128, 128, p, p, 4 * 273 * 256, 256, p, 2, 26, 42, 256, 128, 4, 3, 2, None, p,
+                                      1 << 30, p, None)
     assert rc != 0 and b"multiples of 64" in lib.sdetr_last_error()
     split = [p, 256, 256, 4, 3, p, p, p, p, p, None]
     for i in (0, 5, 6, 7):
@@ -55,8 +55,8 @@ def test_argument_validation():
     args[2] = 254
     assert lib.sdetr_conv2d_f16x3_split_weight(*args) == -1 and b"bad sizes" in lib.sdetr_last_error()
     wgrad = lambda *a: lib.sdetr_conv2d_f16x3_wgrad(*a)  # noqa: E731
-    good = [p, 1092 * 256, 256, p, p, 4 * 273 * 256, 256, p, 2, 26, 42, 256, 256, 4, 3, 2, p, ws, p, None]
-    for i, bad in ((0, None), (3, None), (4, None), (16, None), (18, None)):
+    good = [p, 1092 * 256, 256, p, p, 4 * 273 * 256, 256, p, 2, 26, 42, 256, 256, 4, 3, 2, None, p, ws, p, None]
+    for i, bad in ((0, None), (3, None), (4, None), (17, None), (19, None)):
         args = list(good)
         args[i] = bad
         assert wgrad(*args) == -1 and b"null pointer" in lib.sdetr_last_error()
@@ -70,26 +70,27 @@ def test_argument_validation():
     args[1] = 6  # image pitch not 16-byte aligned
     assert wgrad(*args) == -1 and b"16-byte aligned" in lib.sdetr_last_error()
     args = list(good)
-    args[17] = ws - 1
+    args[18] = ws - 1
     assert wgrad(*args) == -1 and b"workspace too small" in lib.sdetr_last_error()
     args = list(good)
     args[15] = 3
     assert wgrad(*args) != 0 and b"stride 1 or 2" in lib.sdetr_last_error()
 
-    tr = [p, 256 * 256, 256, 2, 13, 21, 256, p, p, p, p, 256, 4, 3, 26, 42, p, 1092 * 256, 256, None]
-    for i in (0, 7, 8, 16):
-        args = list(tr)
+    # the input gradient of a stride-2 convolution
+    dg = [p, 256 * 256, 256, 2, 13, 21, 256, p, p, p, p, None, 0, 0, None, 0, 0, 256, 4, 3, 2, 26, 42, p, 1092 * 256, 256, None]
+    for i in (0, 7, 8, 23):
+        args = list(dg)
         args[i] = None
-        assert lib.sdetr_conv2d_f16x3_transposed(*args) == -1 and b"null pointer" in lib.sdetr_last_error()
-    args = list(tr)
-    args[6], args[11] = 160, 160
-    assert lib.sdetr_conv2d_f16x3_transposed(*args) != 0 and b"multiples of 64" in lib.sdetr_last_error()
-    args = list(tr)
+        assert lib.sdetr_conv2d_f16x3_dgrad(*args) == -1 and b"null pointer" in lib.sdetr_last_error()
+    args = list(dg)
+    args[6], args[17] = 160, 160
+    assert lib.sdetr_conv2d_f16x3_dgrad(*args) != 0 and b"multiples of 64" in lib.sdetr_last_error()
+    args = list(dg)
     args[4] = 12  # dY is not the stride-2 output size of 26 x 42
-    assert lib.sdetr_conv2d_f16x3_transposed(*args) == -1 and b"stride-2 convolution" in lib.sdetr_last_error()
-    args = list(tr)
+    assert lib.sdetr_conv2d_f16x3_dgrad(*args) == -1 and b"stride-2 convolution" in lib.sdetr_last_error()
+    args = list(dg)
     args[2] = 250
-    assert lib.sdetr_conv2d_f16x3_transposed(*args) == -1 and b"16-byte aligned" in lib.sdetr_last_error()
+    assert lib.sdetr_conv2d_f16x3_dgrad(*args) == -1 and b"16-byte aligned" in lib.sdetr_last_error()
 
     up = [p, 1092 * 512, 512, 26, 42, 13, 21, 2, 256, p, 273 * 256, 256, None]
     args = list(up)
@@ -155,7 +156,7 @@ OP_KINDS = {"3x3_s1_g4": (3, 1, 4, 256, 256), "3x3_s2_g1": (3, 2, 1, 256, 256), 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", sorted(OP_KINDS))
 @pytest.mark.parametrize("b", [1, 2])
-def test_conv_gradients_vs_fp64(kind, b):
+def test_conv_dgrad_and_wgrad_vs_fp64(kind, b):
     """weight and input gradients of the token convolution against fp64 autograd of F.conv2d.  Operands are a level slice and
     a channel half of wider buffers.  Elementwise bound as test_neck.py::test_conv_kernel_vs_fp64 states it: 2^-17 x the sum of
     the absolute products (the 3xFP16 products keep ~22 bits, k-block sums are added in fp32)."""
@@ -190,11 +191,8 @@ def test_conv_gradients_vs_fp64(kind, b):
         for got, ref in (((f_hi, f_lo), w.permute(0, 2, 3, 1)), ((w_hi, w_lo), dgrad_weight(w, groups))):
             r_hi, r_lo, r_scale = pkg.cabi.split_f16_pair_dev(ref.contiguous(), w_scale)
             assert torch.equal(got[0], r_hi) and torch.equal(got[1], r_lo)
-        if stride == 1:
-            dx = pkg.cabi.conv2d_f16x3(gy, (ho, wo), pkg.cabi.pow2_scale(gbuf, 12), w_hi, w_lo, w_scale, None, groups, k, 1, 0)
-        else:
-            dx = pkg.cabi.conv2d_f16x3_transposed(gy, (ho, wo), pkg.cabi.pow2_scale(gbuf, 12), w_hi, w_lo, w_scale, groups, k,
-                                                  (h, wd))
+        dx = pkg.cabi.conv2d_f16x3_dgrad(gy, (ho, wo), pkg.cabi.pow2_scale(gbuf, 12), w_hi, w_lo, w_scale, groups, k, stride,
+                                         (h, wd))
         dx = dx.double().transpose(1, 2).reshape(b, cin, h, wd)
         err = (dx - dx64).abs()
         assert bool((err <= 2.0 ** -17 * bdx + 1e-30).all()), (kind, b, h, wd, float(err.max()))

@@ -110,7 +110,9 @@ int sdetr_msda_set_host_shapes(int num_levels, const int32_t *level_h_host, cons
  * 249-295 = torchvision.ops.batched_nms over boxes (x-1,y-1,x+1,y+1) on each (image, level) grid).  topk_index (b,k) int64:
  * candidate tokens in descending score order (the rank decides who suppresses whom).  kept_index (b,k) int64 receives the
  * surviving tokens in the same order (first kept_count[b] entries valid), keep_flag (b,k) uint8 (nullable) the per-
- * candidate verdict.  k < 65535; the rank table (2 bytes per token) lives in shared memory: num_value up to ~98 000. */
+ * candidate verdict.  k < 65535; the rank table (2 bytes per token) lives in shared memory: num_value up to ~98 000.
+ * A box is suppressed when its float32 IoU > iou_threshold; torchvision compares with a double threshold, so a caller
+ * holding a double passes the largest float not above it (cabi.nms_iou_threshold_f32), not the nearest one. */
 int sdetr_nms_topk_index(const int64_t *topk_index, int batch, int k, int num_value, int num_levels,
                          const int32_t *level_h_host, const int32_t *level_w_host, float iou_threshold, int64_t *kept_index,
                          int32_t *kept_count, uint8_t *keep_flag, sdetr_stream_t stream);

@@ -261,6 +261,17 @@ def msda_set_host_shapes(shapes):
            "sdetr_msda_set_host_shapes")
 
 
+def nms_iou_threshold_f32(iou_threshold) -> float:
+    """The float32 threshold t32 with `iou > t32` == `iou > iou_threshold` for every float32 IoU: torchvision compares its
+    float32 IoU with the double threshold, so a threshold between two floats (1/3 as a Python float) rounds DOWN, never to
+    the nearest float (which may be the IoU itself and turn a suppression into a keep)."""
+    t = float(iou_threshold)
+    t32 = torch.tensor(t, dtype=torch.float32)
+    if float(t32) > t:
+        t32 = torch.nextafter(t32, torch.tensor(-float("inf")))
+    return float(t32)
+
+
 def nms_topk_index(topk_index, shapes, iou_threshold=0.3):
     """topk_index (b,k) int64, candidates in descending score order -> (kept_index (b,k), kept_count (b,) int32, keep_flag (b,k) u8)."""
     b, k = topk_index.shape
@@ -269,8 +280,9 @@ def nms_topk_index(topk_index, shapes, iou_threshold=0.3):
     count = torch.empty(b, device=dev, dtype=torch.int32)
     flag = torch.empty(b, k, device=dev, dtype=torch.uint8)
     rc = lib().sdetr_nms_topk_index(_req(topk_index, "topk_index", torch.int64), b, k, sum(h * w for h, w in shapes), len(shapes),
-                                    _host_i32([h for h, _ in shapes]), _host_i32([w for _, w in shapes]), float(iou_threshold),
-                                    kept.data_ptr(), count.data_ptr(), flag.data_ptr(), _stream())
+                                    _host_i32([h for h, _ in shapes]), _host_i32([w for _, w in shapes]),
+                                    nms_iou_threshold_f32(iou_threshold), kept.data_ptr(), count.data_ptr(), flag.data_ptr(),
+                                    _stream())
     _check(rc, "sdetr_nms_topk_index")
     return kept, count, flag
 

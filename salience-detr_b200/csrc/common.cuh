@@ -67,6 +67,12 @@ __device__ __forceinline__ float relu_nan(float x) {
     asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
     return r;
 }
+// torch.max: a NaN operand propagates (as the canonical NaN; fmaxf would return the other operand).  One max.NaN instruction.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
 
 __device__ __forceinline__ float4 ldg_f4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
 

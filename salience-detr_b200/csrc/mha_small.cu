@@ -374,12 +374,12 @@ using namespace sdetr;
 extern "C" int sdetr_mha_in_proj(const float *tokens, const float *pos, const int64_t *index, int batch, int num_rows, int k,
                                  int channels, const float *w_in_t, const float *b_in, float *t_out, float *qkv,
                                  sdetr_stream_t stream) {
-    SDETR_REQUIRE(tokens && pos && index && w_in_t && b_in && t_out && qkv, SDETR_ERR_INVALID_ARG, "mha_in_proj: null pointer");
     SDETR_REQUIRE(batch > 0 && num_rows > 0 && k >= 0 && k <= num_rows, SDETR_ERR_INVALID_ARG, "mha_in_proj: bad sizes");
     SDETR_REQUIRE(channels == 256, SDETR_ERR_UNSUPPORTED, "mha_in_proj: channels %d (only 256)", channels);
+    if (k == 0) return SDETR_OK;  // no rows: the empty index and outputs may be null
+    SDETR_REQUIRE(tokens && pos && index && w_in_t && b_in && t_out && qkv, SDETR_ERR_INVALID_ARG, "mha_in_proj: null pointer");
     SDETR_REQUIRE(aligned16(tokens) && aligned16(pos) && aligned16(w_in_t) && aligned16(b_in) && aligned16(t_out) && aligned16(qkv),
                   SDETR_ERR_INVALID_ARG, "mha_in_proj: 16-byte alignment required");
-    if (k == 0) return SDETR_OK;
     constexpr int C = 256;
     const int rows = batch * k;
     const size_t smem = (size_t)(C * kInPitch + C * kInCols) * sizeof(float);
@@ -435,16 +435,16 @@ extern "C" int sdetr_mha_out_proj_ln_scatter(const float *attn, const float *t, 
                                              const float *gamma, const float *beta, float eps, const int64_t *index,
                                              float *dst, const float *pos, float *dst_sum, int batch, int num_rows, int k,
                                              int channels, sdetr_stream_t stream) {
+    SDETR_REQUIRE(batch > 0 && num_rows > 0 && k >= 0 && k <= num_rows, SDETR_ERR_INVALID_ARG, "mha_out_proj_ln_scatter: bad sizes");
+    SDETR_REQUIRE(channels == 256, SDETR_ERR_UNSUPPORTED, "mha_out_proj_ln_scatter: channels %d (only 256)", channels);
+    if (k == 0) return SDETR_OK;  // no rows: the empty index and inputs may be null
     SDETR_REQUIRE(attn && t && w_out_t && b_out && gamma && beta && index && dst, SDETR_ERR_INVALID_ARG,
                   "mha_out_proj_ln_scatter: null pointer");
-    SDETR_REQUIRE(batch > 0 && num_rows > 0 && k >= 0 && k <= num_rows, SDETR_ERR_INVALID_ARG, "mha_out_proj_ln_scatter: bad sizes");
     SDETR_REQUIRE((pos == nullptr) == (dst_sum == nullptr) && aligned16(pos) && aligned16(dst_sum), SDETR_ERR_INVALID_ARG,
                   "mha_out_proj_ln_scatter: pos and dst_sum go together (16-byte aligned)");
-    SDETR_REQUIRE(channels == 256, SDETR_ERR_UNSUPPORTED, "mha_out_proj_ln_scatter: channels %d (only 256)", channels);
     SDETR_REQUIRE(aligned16(attn) && aligned16(t) && aligned16(w_out_t) && aligned16(b_out) && aligned16(gamma) && aligned16(beta) &&
                       aligned16(dst),
                   SDETR_ERR_INVALID_ARG, "mha_out_proj_ln_scatter: 16-byte alignment required");
-    if (k == 0) return SDETR_OK;
     constexpr int C = 256;
     const int rows = batch * k;
     const size_t smem = (size_t)(C * kOutRows + 2 * kOutChunk * C + kOutRows * C) * sizeof(float);

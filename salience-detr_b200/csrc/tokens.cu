@@ -193,6 +193,7 @@ __global__ void __launch_bounds__(kRowThreads) zero_masked_rows_kernel(float *__
 }
 
 // ---- mc_score = max_c(logits) * fg (:366) ---------------------------------------------------------------
+// The max propagates a NaN logit, as torch's max does: a NaN row must not become a finite top-k score.
 __global__ void __launch_bounds__(kRowThreads) class_max_kernel(const float *__restrict__ logits, int64_t pitch,
                                                                 const float *__restrict__ fg, int64_t rows, int nc,
                                                                 float *__restrict__ out) {
@@ -200,9 +201,9 @@ __global__ void __launch_bounds__(kRowThreads) class_max_kernel(const float *__r
     const int64_t row = (int64_t)blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
     if (row >= rows) return;
     float m = -INFINITY;
-    for (int c = lane; c < nc; c += 32) m = fmaxf(m, __ldg(logits + row * pitch + c));
+    for (int c = lane; c < nc; c += 32) m = fmax_nan(m, __ldg(logits + row * pitch + c));
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    for (int o = 16; o > 0; o >>= 1) m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (lane == 0) out[row] = m * __ldg(fg + row);
 }
 
@@ -266,14 +267,14 @@ extern "C" int sdetr_token_gather(const float *tokens, const float *pos, const f
                                   const int64_t *level_start_index, int batch, int num_value, int channels,
                                   int num_levels, int num_query, float *query, float *query_pos, float *fg_q,
                                   float *ref_q, float *query_sum, sdetr_stream_t stream) {
-    SDETR_REQUIRE(tokens && pos && fg && valid_ratios && inds && spatial_shapes && level_start_index && query &&
-                      query_pos && fg_q && ref_q,
-                  SDETR_ERR_INVALID_ARG, "token_gather: null pointer");
     SDETR_REQUIRE(batch > 0 && num_value > 0 && num_query >= 0 && num_levels > 0 && num_levels <= kMaxLevels,
                   SDETR_ERR_INVALID_ARG, "token_gather: bad sizes");
     SDETR_REQUIRE(channels % 4 == 0 && aligned16(tokens) && aligned16(pos) && aligned16(query) && aligned16(query_pos),
                   SDETR_ERR_INVALID_ARG, "token_gather: rows must be 16-byte aligned, channels %% 4 == 0");
-    if (num_query == 0) return SDETR_OK;
+    if (num_query == 0) return SDETR_OK;  // nothing to gather: the empty index and outputs may be null
+    SDETR_REQUIRE(tokens && pos && fg && valid_ratios && inds && spatial_shapes && level_start_index && query &&
+                      query_pos && fg_q && ref_q,
+                  SDETR_ERR_INVALID_ARG, "token_gather: null pointer");
     token_gather_kernel<<<row_blocks((int64_t)batch * num_query), kRowThreads, 0, (cudaStream_t)stream>>>(
         tokens, pos, fg, valid_ratios, inds, inds_stride, spatial_shapes, level_start_index, batch, num_value, channels,
         num_levels, num_query, query, query_pos, fg_q, ref_q, query_sum);
@@ -283,11 +284,11 @@ extern "C" int sdetr_token_gather(const float *tokens, const float *pos, const f
 extern "C" int sdetr_token_scatter(float *tokens, const float *query, const int64_t *inds, int64_t inds_stride,
                                    const int32_t *focus_token_nums, int batch, int num_value, int channels,
                                    int num_query, sdetr_stream_t stream) {
-    SDETR_REQUIRE(tokens && query && inds && focus_token_nums, SDETR_ERR_INVALID_ARG, "token_scatter: null pointer");
     SDETR_REQUIRE(batch > 0 && num_value > 0 && num_query >= 0, SDETR_ERR_INVALID_ARG, "token_scatter: bad sizes");
     SDETR_REQUIRE(channels % 4 == 0 && aligned16(tokens) && aligned16(query), SDETR_ERR_INVALID_ARG,
                   "token_scatter: rows must be 16-byte aligned, channels %% 4 == 0");
-    if (num_query == 0) return SDETR_OK;
+    if (num_query == 0) return SDETR_OK;  // nothing to write back: the empty query rows and index may be null
+    SDETR_REQUIRE(tokens && query && inds && focus_token_nums, SDETR_ERR_INVALID_ARG, "token_scatter: null pointer");
     token_scatter_kernel<<<row_blocks((int64_t)batch * num_query), kRowThreads, 0, (cudaStream_t)stream>>>(
         tokens, query, inds, inds_stride, focus_token_nums, batch, num_value, channels, num_query);
     return check_launch("token_scatter");
@@ -299,7 +300,8 @@ extern "C" int sdetr_background_embed(float *tokens, const uint8_t *mask, const 
                                       const int64_t *spatial_shapes_host, const int64_t *level_start_index, int batch,
                                       int num_value, int channels, int num_levels, uint8_t *flags,
                                       sdetr_stream_t stream) {
-    SDETR_REQUIRE(tokens && mask && last_inds && row_embed && col_embed && spatial_shapes && level_start_index && flags,
+    SDETR_REQUIRE(tokens && mask && (last_inds || num_last == 0) && row_embed && col_embed && spatial_shapes &&
+                      level_start_index && flags,
                   SDETR_ERR_INVALID_ARG, "background_embed: null pointer");
     SDETR_REQUIRE(batch > 0 && num_value > 0 && num_last >= 0 && num_levels > 0 && num_levels <= kMaxLevels &&
                       num_embeddings > 0,

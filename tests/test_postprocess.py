@@ -256,18 +256,28 @@ def test_tied_scores_follow_sequential_greedy(shape, k):
 @gpu
 @pytest.mark.parametrize("filters", [(-1, -1), (0.5, 0.3)])
 def test_strided_query_slice(filters):
-    """outputs_class[:, :, pad:, :] as dn_post_process leaves it: no copy, same result as the contiguous tensor."""
+    """outputs_class[:, :, pad:, :] as dn_post_process leaves it: no copy, same result as the contiguous tensor.  One
+    library launch, and the call's peak allocation is no larger than on the contiguous tensors: a copy of either slice
+    would add at least the size of the smaller one (the boxes) while the call runs."""
     pad = 37
     logits, boxes, sizes = gpu_inputs(2, 900 + pad, 91, seed=3)
     ls, bs = logits[:, pad:, :], boxes[:, pad:, :]
     assert not ls.is_contiguous() and not bs.is_contiguous()
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        got = run(ls, bs, sizes, 300, *filters)
+    lc, bc = ls.contiguous(), bs.contiguous()
+    pkg = _pkg()
+
+    def peak_and_launches(lg, bx):
         torch.cuda.synchronize()
-    kernels = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "Memcpy" not in e.name]
-    assert len(kernels) == 1, [e.name for e in kernels]  # the library's kernel only: no copy of the slice
-    want = run(ls.contiguous(), bs.contiguous(), sizes, 300, *filters)
+        torch.cuda.reset_peak_memory_stats()
+        base, n0 = torch.cuda.memory_allocated(), pkg.cabi.launch_count()
+        out = run(lg, bx, sizes, 300, *filters)
+        torch.cuda.synchronize()
+        return out, torch.cuda.max_memory_allocated() - base, pkg.cabi.launch_count() - n0
+
+    want, peak_contiguous, _ = peak_and_launches(lc, bc)
+    got, peak, launches = peak_and_launches(ls, bs)
+    assert launches == 1
+    assert peak <= peak_contiguous, (peak, peak_contiguous)
     for r, w in zip(got, want):
         assert all(same_bits(r[key], w[key]) for key in ("scores", "labels", "boxes"))
 

@@ -692,6 +692,32 @@ int sdetr_dwconv7x7_layernorm_tokens(const float *x, int batch, int H, int W, in
  * GEMM with K = 4 C against its weight permuted to (Cout, 2, 2, Cin).  y must not alias x.  One launch. */
 int sdetr_layernorm_tokens_s2d(const float *x, int batch, int H, int W, int C, const float *ln_weight, const float *ln_bias,
                                float eps, float *y, sdetr_stream_t stream);
+/* ---- Swin Transformer backbone in token layout (models/backbones/swin.py; SwinTransformerBackbone.forward_tokens) -----------
+ * Token rows (batch, H * W, C) contiguous in raster order.  The Linears run on sdetr_gemm_f16x3_ex, the stem on
+ * sdetr_convnext_stem.
+ * Shifted-window multi-head attention of V1 Swin (shifted_window_attention without its projections): qkv (batch, H * W, 3 C) is
+ * the QKV Linear's output with q, k, v of head h at columns s * C + 32 h + d; qkv_bias (3 C); rel_bias (num_heads, N, N), N =
+ * window_h * window_w <= 144, the expanded relative position bias; C = 32 num_heads; 0 <= shift < window per dimension, the
+ * block's nominal shift.  The map is padded to pad_H = ceil(H / window_h) window_h (pad_W likewise); the shift is zeroed in a
+ * dimension where the window is at least the padded size; window coordinate r of the rolled frame reads source row
+ * (r + shift_h) mod pad_H (columns likewise).  A pad position is a zero row before the QKV Linear, so its key and value are the
+ * qkv bias; it is not masked, and its query output is dropped.  Logits (q * 32^-0.5) . k + rel_bias[h, i, j], plus -100 where the
+ * region ids 3 id_h + id_w of i and j differ (id_h: 0 on [0, pad_H - window_h), 1 on [pad_H - window_h, pad_H - shift_h), 2 on
+ * the rest, of the rolled row; id_w likewise).  Softmax with expf, fp32 FMAs.  y (batch, H * W, C), every row written; y must
+ * not alias qkv.  One launch. */
+int sdetr_window_attention_tokens(const float *qkv, const float *qkv_bias, const float *rel_bias, int batch, int H, int W, int C,
+                                  int num_heads, int window_h, int window_w, int shift_h, int shift_w, float *y,
+                                  sdetr_stream_t stream);
+/* PatchMerging's LayerNorm: y (batch, ceil(H / 2) * ceil(W / 2), 4 C), row (oy, ox) the LayerNorm over 4 C (weight and bias
+ * (4 C)) of the concatenation [x(2 oy, 2 ox), x(2 oy + 1, 2 ox), x(2 oy, 2 ox + 1), x(2 oy + 1, 2 ox + 1)], i.e. column
+ * (2 dx + dy) C + c; pixels outside the map are zeros that take part in the statistics.  C % 16 == 0, 4 C <= 3072.  Two-pass
+ * mean / variance in fp32; a NaN input pixel gives a NaN row.  Operands 16-byte aligned, y must not alias x.  One launch. */
+int sdetr_patch_merge_layernorm_tokens(const float *x, int batch, int H, int W, int C, const float *ln_weight,
+                                       const float *ln_bias, float eps, float *y, sdetr_stream_t stream);
+/* y = LayerNorm(x) over C of rows contiguous token rows (weight and bias (C)), C % 64 == 0, C <= 1536.  Two-pass mean / variance
+ * in fp32; a NaN in a row gives a NaN row.  Operands 16-byte aligned, y must not alias x.  One launch. */
+int sdetr_layernorm_tokens(const float *x, int64_t rows, int C, const float *ln_weight, const float *ln_bias, float eps, float *y,
+                           sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

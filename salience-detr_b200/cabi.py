@@ -113,6 +113,9 @@ SIGNATURES = {
     "sdetr_convnext_stem": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
     "sdetr_dwconv7x7_layernorm_tokens": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
     "sdetr_layernorm_tokens_s2d": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_window_attention_tokens": (_i, [_vp, _vp, _vp] + [_i] * 9 + [_vp, _vp]),
+    "sdetr_patch_merge_layernorm_tokens": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_layernorm_tokens": (_i, [_vp, _i64, _i, _vp, _vp, _f, _vp, _vp]),
 }
 
 
@@ -1410,4 +1413,56 @@ def layernorm_tokens_s2d(x, hw, ln_weight, ln_bias, eps: float = 1e-6):
                                           _req(ln_weight, "ln_weight", torch.float32), _req(ln_bias, "ln_bias", torch.float32),
                                           float(eps), y.data_ptr(), _stream())
     _check(rc, "sdetr_layernorm_tokens_s2d")
+    return y
+
+
+# ---- Swin Transformer backbone in token layout (swin.SwinTransformerBackbone.forward_tokens) -------------------------------
+def window_attention_tokens(qkv, hw, qkv_bias, rel_bias, num_heads: int, window, shift):
+    """Shifted-window multi-head attention of V1 Swin from the QKV Linear's output: qkv (b, H*W, 3C) contiguous token rows in
+    raster order, hw = (H, W), qkv_bias (3C), rel_bias (num_heads, N, N) the expanded relative position bias (N = window[0] *
+    window[1]), window and shift the block's (h, w) window and nominal shift -> a new (b, H*W, C) tensor, the attention output
+    before the projection at each pixel.  Padding, roll and the shift mask follow the reference (see sdetr_b200.h)."""
+    b, n, c3 = qkv.shape
+    H, W = hw
+    C = c3 // 3
+    if n != H * W or c3 != 3 * C:
+        raise RuntimeError(f"window_attention_tokens: qkv must be (b, {H * W}, 3C), got {tuple(qkv.shape)}")
+    N = int(window[0]) * int(window[1])
+    if tuple(qkv_bias.shape) != (3 * C,) or tuple(rel_bias.shape) != (num_heads, N, N):
+        raise RuntimeError(f"window_attention_tokens: qkv_bias must be ({3 * C},) and rel_bias ({num_heads}, {N}, {N})")
+    y = torch.empty(b, n, C, device=qkv.device, dtype=torch.float32)
+    rc = lib().sdetr_window_attention_tokens(_req(qkv, "qkv", torch.float32), _req(qkv_bias, "qkv_bias", torch.float32),
+                                             _req(rel_bias, "rel_bias", torch.float32), b, int(H), int(W), C, int(num_heads),
+                                             int(window[0]), int(window[1]), int(shift[0]), int(shift[1]), y.data_ptr(), _stream())
+    _check(rc, "sdetr_window_attention_tokens")
+    return y
+
+
+def patch_merge_layernorm_tokens(x, hw, ln_weight, ln_bias, eps: float = 1e-5):
+    """PatchMerging's pad, 2x2 concatenation and LayerNorm over 4C: x (b, H*W, C) contiguous token rows, hw = (H, W) -> a new
+    (b, ceil(H / 2) * ceil(W / 2), 4C) tensor, row (y, x) holding pixel (2y + dy, 2x + dx) at columns (2 dx + dy) * C + c."""
+    b, n, C = x.shape
+    H, W = hw
+    if n != H * W:
+        raise RuntimeError(f"patch_merge_layernorm_tokens: x has {n} rows per image, the map is {H}x{W}")
+    if any(tuple(t.shape) != (4 * C,) for t in (ln_weight, ln_bias)):
+        raise RuntimeError(f"patch_merge_layernorm_tokens: ln_weight and ln_bias must be ({4 * C},)")
+    y = torch.empty(b, ((H + 1) // 2) * ((W + 1) // 2), 4 * C, device=x.device, dtype=torch.float32)
+    rc = lib().sdetr_patch_merge_layernorm_tokens(_req(x, "x", torch.float32), b, int(H), int(W), C,
+                                                  _req(ln_weight, "ln_weight", torch.float32),
+                                                  _req(ln_bias, "ln_bias", torch.float32), float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_patch_merge_layernorm_tokens")
+    return y
+
+
+def layernorm_tokens(x, ln_weight, ln_bias, eps: float = 1e-5):
+    """LayerNorm over the last dimension C (a multiple of 64 up to 1536) of contiguous fp32 rows -> a new tensor of x's shape."""
+    C = x.shape[-1]
+    if any(tuple(t.shape) != (C,) for t in (ln_weight, ln_bias)):
+        raise RuntimeError(f"layernorm_tokens: ln_weight and ln_bias must be ({C},)")
+    y = torch.empty_like(x, memory_format=torch.contiguous_format)
+    rc = lib().sdetr_layernorm_tokens(_req(x, "x", torch.float32), x.numel() // C if C else 0, C,
+                                      _req(ln_weight, "ln_weight", torch.float32), _req(ln_bias, "ln_bias", torch.float32),
+                                      float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_layernorm_tokens")
     return y

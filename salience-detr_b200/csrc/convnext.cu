@@ -8,49 +8,17 @@
 //   sdetr_layernorm_tokens_s2d         LayerNorm over C of token rows, written space-to-depth: output row (y, x) of the
 //                                      (H / 2) x (W / 2) map holds LayerNorm(x[2y + dy, 2x + dx]) at columns (2 dy + dx) C + c.
 //
-// One warp per token row: lane l owns the channel pairs 64 j + 2 l, j < C / 64, in registers; the LayerNorm is two-pass
-// (mean, then the mean of squared deviations) with butterfly warp sums, so it is order-fixed and a NaN anywhere in the row
-// (or in a convolution window feeding it) makes the whole row NaN, as in torch.  A constant row has variance 0 and gives
-// (x - mean) * rsqrt(eps) = 0 times the weight plus the bias.
+// One warp per token row with the two-pass LayerNorm of layernorm_rows.cuh: a NaN anywhere in the row (or in a convolution
+// window feeding it) makes the whole row NaN, as in torch.
 #include <math.h>
 
 #include "common.cuh"
+#include "layernorm_rows.cuh"
 
 namespace sdetr {
 
 constexpr int kCnMaxJ = 24;     // C <= 64 * 24 = 1536
 constexpr int kCnWarps = 8;     // token rows per CTA of 256 threads
-
-__device__ __forceinline__ float cn_warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// LayerNorm of the row held in v (lane's pairs 64 j + 2 lane) -> dst[c]
-__device__ __forceinline__ void cn_layernorm_store(const float2 (&v)[kCnMaxJ], int nj, int C, int lane, const float *__restrict__ g,
-                                                   const float *__restrict__ b, float eps, float *__restrict__ dst) {
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < kCnMaxJ; ++j)
-        if (j < nj) s += v[j].x + v[j].y;
-    const float mean = cn_warp_sum(s) / (float)C;
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < kCnMaxJ; ++j)
-        if (j < nj) {
-            const float dx = v[j].x - mean, dy = v[j].y - mean;
-            q = fmaf(dx, dx, q), q = fmaf(dy, dy, q);
-        }
-    const float rstd = rsqrtf(cn_warp_sum(q) / (float)C + eps);
-#pragma unroll
-    for (int j = 0; j < kCnMaxJ; ++j)
-        if (j < nj) {
-            const int c = 64 * j + 2 * lane;
-            const float2 gw = __ldg(reinterpret_cast<const float2 *>(g + c)), bw = __ldg(reinterpret_cast<const float2 *>(b + c));
-            *reinterpret_cast<float2 *>(dst + c) = make_float2((v[j].x - mean) * rstd * gw.x + bw.x, (v[j].y - mean) * rstd * gw.y + bw.y);
-        }
-}
 
 __global__ void __launch_bounds__(32 * kCnWarps) convnext_stem_kernel(const float *__restrict__ x, int batch, int H, int W, int Ho,
                                                                        int Wo, int C, const float *__restrict__ w /* (48, C) */,

@@ -68,6 +68,31 @@ def convnext_weights(shapes: Mapping[str, Sequence[int]], seed: int = 0) -> "Ord
     return out
 
 
+def swin_weights(state: Mapping[str, torch.Tensor], seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for a V1 Swin Transformer state dict (in its order): Linear and convolution weights N(0, 1 / fan_in), their
+    biases N(0, 0.1^2), LayerNorm affines away from (1, 0) -- weight 1 + U(-0.25, 0.25), bias N(0, 0.1^2) -- and every
+    relative_position_bias_table N(0, 1), a spread that moves the softmax: at the 0.02 of the initialisation a wrong bias index
+    would go unseen.  The relative_position_index buffers are copied from ``state``, the network's own state dict."""
+    g = torch.Generator().manual_seed(seed)
+    out = OrderedDict()
+    for k, v in state.items():
+        shape = tuple(v.shape)
+        if k.endswith("relative_position_index"):
+            t = v.clone()
+        elif k.endswith("relative_position_bias_table"):
+            t = torch.randn(shape, generator=g)
+        elif len(shape) >= 2:
+            t = torch.randn(shape, generator=g) / math.sqrt(math.prod(shape[1:]))
+        elif k.endswith("bias"):
+            t = torch.randn(shape, generator=g) * 0.1
+        elif k.endswith("weight"):
+            t = 1.0 + (torch.rand(shape, generator=g) - 0.5) * 0.5
+        else:
+            raise ValueError(f"swin_weights: no rule for {k} {shape}")
+        out[k] = t
+    return out
+
+
 def level_shapes(h: int, w: int, strides: Sequence[int]) -> List[Tuple[int, int]]:
     out: List[Tuple[int, int]] = []
     for i, s in enumerate(strides):

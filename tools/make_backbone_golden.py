@@ -51,7 +51,8 @@ def image():
 
 
 def _stub_missing_modules():
-    """omegaconf.DictConfig (a dict with attribute reads), accelerate.logging.get_logger, terminaltables.AsciiTable"""
+    """omegaconf.DictConfig (a dict with attribute reads), OmegaConf.to_object (the identity), accelerate.logging.get_logger,
+    terminaltables.AsciiTable"""
     import logging
 
     class DictConfig(dict):
@@ -66,8 +67,13 @@ def _stub_missing_modules():
             except KeyError as e:
                 raise AttributeError(name) from e
 
+    class OmegaConf:
+        @staticmethod
+        def to_object(cfg):
+            return cfg  # the stub's configs are plain dicts and lists already
+
     omegaconf = types.ModuleType("omegaconf")
-    omegaconf.DictConfig, omegaconf.ListConfig, omegaconf.OmegaConf = DictConfig, type("ListConfig", (list,), {}), object
+    omegaconf.DictConfig, omegaconf.ListConfig, omegaconf.OmegaConf = DictConfig, type("ListConfig", (list,), {}), OmegaConf
     accelerate = types.ModuleType("accelerate")
     acc_logging = types.ModuleType("accelerate.logging")
     acc_logging.get_logger = logging.getLogger

@@ -7,13 +7,13 @@ extractor's sub-module names (``conv1``, ``bn1``, ``layer1`` ... up to the last 
 V1.5: the stride sits in a Bottleneck's 3x3 convolution) and its initialisation, in the same RNG order, so a seed gives the
 reference's tensors.  ``forward(x)`` returns ``{"layer{i+1}": map}`` for ``i`` in ``return_indices``, in that order.
 
-``forward`` is the reference's op chain in torch whenever ``tokens_supported(x)`` does not hold: with autograd, on the CPU, for
-BasicBlock / ResNeXt / dilated / deformable networks and for norms other than this module's ``FrozenBatchNorm2d``.  Otherwise
-it is ``forward_tokens(x)``: every FrozenBatchNorm folded into its convolution on the device (``sdetr_frozen_bn_fold``, in
-float64 with each operation rounded alone) once per parameter / buffer version, the stem (``sdetr_resnet_stem``, fp32 FMAs
-from the NCHW image batch), the max-pool (``sdetr_maxpool3x3s2_tokens``) and every convolution a ``neck.TokenConv`` on
-``sdetr_conv2d_f16x3`` (3xFP16 on wgmma, fp32-class accuracy whatever ``allow_tf32`` says) with ReLU and the block's residual
-in the epilogue.  Each returned map is a channels-last NCHW view of its own ``(b, H*W, C)`` token buffer,
+``forward`` is the reference's op chain in torch, ``forward_torch(x)``, whenever ``tokens_supported(x)`` does not hold: with
+autograd, on the CPU, for BasicBlock / ResNeXt / dilated / deformable networks and for norms other than this module's
+``FrozenBatchNorm2d``.  Otherwise it is ``forward_tokens(x)``: every FrozenBatchNorm folded into its convolution on the device
+(``sdetr_frozen_bn_fold``, in float64 with each operation rounded alone) once per parameter / buffer version, the stem
+(``sdetr_resnet_stem``, fp32 FMAs from the NCHW image batch), the max-pool (``sdetr_maxpool3x3s2_tokens``) and every convolution
+a ``neck.TokenConv`` on ``sdetr_conv2d_f16x3`` (3xFP16 on wgmma, fp32-class accuracy whatever ``allow_tf32`` says) with ReLU and
+the block's residual in the epilogue.  Each returned map is a channels-last NCHW view of its own ``(b, H*W, C)`` token buffer,
 which ``ChannelMapper`` reads in place.  No host synchronisation: the call can be captured in a CUDA graph.
 
 Under autograd, ``forward_tokens`` trains the convolutions of layers 1-4 in token layout when ``training_tokens_supported(x)``
@@ -27,13 +27,16 @@ optimizer step between CUDA-graph replays is seen.  The backward runs the whole 
 """
 from __future__ import annotations
 
-from collections.abc import Mapping
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Type, Union
 
 import torch
 from torch import Tensor, nn
 
 from . import cabi, derived
+from . import token_backbone as tb
+# training_tokens_supported reads the image check through this module's own name, which the CPU tests replace to stand a
+# CPU image in for a CUDA one
+from .token_backbone import cuda_image as _cuda_image
 from .neck import TokenConv
 
 
@@ -230,38 +233,14 @@ class ResNetBackbone(nn.Module):
             raise ValueError(f"Expected architecture in {list(self.model_arch)} but got {arch}")
         cfg = {**self.model_arch[arch], **kwargs}
         resnet = ResNet(**cfg)
-        self._load_weights(resnet, weights)
+        tb.load_weights(resnet, weights, ("fc.",), "ResNetBackbone")
         if len(freeze_indices) > 0:
-            for m in [resnet.conv1, resnet.bn1] + [resnet.get_submodule(f"layer{i + 1}") for i in freeze_indices]:
-                m.eval()
-                for p in m.parameters():
-                    p.requires_grad = False
+            tb.freeze([resnet.conv1, resnet.bn1] + [resnet.get_submodule(f"layer{i + 1}") for i in freeze_indices])
         self.return_indices = tuple(int(i) for i in return_indices)
         # the modules the feature extractor keeps: the stem and the stages up to the last returned one
         for name in ["conv1", "bn1", "relu", "maxpool"] + [f"layer{i + 1}" for i in range(max(self.return_indices) + 1)]:
             setattr(self, name, getattr(resnet, name))
         self.num_channels = [64 * cfg["block"].expansion * 2 ** i for i in self.return_indices]
-
-    @staticmethod
-    def _load_weights(resnet: ResNet, weights):
-        """None: keep the initialisation.  A state dict (or one under "model"), or a local path read with torch.load: every key
-        but fc.* must match the network exactly."""
-        if weights is None:
-            return
-        if isinstance(weights, str):
-            if weights.startswith(("http://", "https://")):
-                raise RuntimeError(f"ResNetBackbone: downloading weights is not supported ({weights}); pass a state dict or "
-                                   "a local file")
-            weights = torch.load(weights, map_location="cpu")
-        if not isinstance(weights, Mapping):
-            raise TypeError(f"ResNetBackbone: weights must be None, a state dict or a path, got {type(weights).__name__}")
-        if "model" in weights:
-            weights = weights["model"]
-        res = resnet.load_state_dict({k: v for k, v in weights.items() if not k.startswith("fc.")}, strict=False)
-        missing = [k for k in res.missing_keys if not k.startswith("fc.")]
-        if missing or res.unexpected_keys:
-            raise RuntimeError(f"ResNetBackbone: weights do not match the network: missing {missing}, "
-                               f"unexpected {res.unexpected_keys}")
 
     def _stages(self) -> List[nn.Sequential]:
         return [getattr(self, f"layer{i + 1}") for i in range(max(self.return_indices) + 1)]
@@ -269,27 +248,23 @@ class ResNetBackbone(nn.Module):
     def forward(self, x: Tensor) -> Dict[str, Tensor]:
         if self.tokens_supported(x):
             return self.forward_tokens(x)
+        return self.forward_torch(x)
+
+    def forward_torch(self, x: Tensor) -> Dict[str, Tensor]:
+        """the reference's op chain in torch: {"layer{i+1}": map} for i in return_indices"""
         x = self.maxpool(self.relu(self.bn1(self.conv1(x))))
         feats = []
         for layer in self._stages():
             x = layer(x)
             feats.append(x)
-        return {f"layer{i + 1}": feats[i] for i in self.return_indices}
+        return {_layer_name(i): feats[i] for i in self.return_indices}
 
     # ---- token-layout inference --------------------------------------------------------------------------------------
     def tokens_supported(self, x) -> bool:
         """True when forward_tokens can run this call: a CUDA fp32 NCHW-contiguous (b, 3, H, W) input, parameters and buffers
         fp32 on its device, nothing that needs a gradient (autograd off, or neither the input nor a parameter requires one),
         and layers_supported()."""
-        if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3):
-            return False
-        if x.numel() == 0 or not x.is_contiguous():
-            return False
-        if any(t.device != x.device or t.dtype != torch.float32 for t in list(self.parameters()) + list(self.buffers())):
-            return False
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            return False
-        return self.layers_supported()
+        return tb.tokens_ready(self, x) and self.layers_supported()
 
     def layers_supported(self) -> bool:
         """The layer half of tokens_supported: Bottleneck blocks of plain convolutions with groups 1, dilation 1 and widths that
@@ -319,9 +294,7 @@ class ResNetBackbone(nn.Module):
         (b, 3, H, W) input with parameters and buffers fp32 on its device, a frozen stem (conv1.weight needs no gradient), an
         input that needs no gradient, and autograd recording (grad enabled and some parameter requiring a gradient).  A stem
         weight gradient and image gradients need forward()."""
-        if not _cuda_image(x) or x.requires_grad:
-            return False
-        if any(t.device != x.device or t.dtype != torch.float32 for t in list(self.parameters()) + list(self.buffers())):
+        if not _cuda_image(x) or x.requires_grad or not tb.on_device_fp32(self, x.device):
             return False
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())) or self.conv1.weight.requires_grad:
             return False
@@ -403,11 +376,7 @@ class ResNetBackbone(nn.Module):
         outs = _TrainBlocks.apply(run, t, *weights)
         for i, o in zip(run.returned, outs):
             feats[i] = (o, run.out_hw[i])
-        res = {}
-        for i in self.return_indices:
-            t, (h, w) = feats[i]
-            res[f"layer{i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
-        return res
+        return tb.token_maps(feats, self.return_indices, _layer_name)
 
     def _kernel_weights(self):
         """_folded() for inference, rebuilt when any parameter or buffer changes"""
@@ -437,17 +406,11 @@ class ResNetBackbone(nn.Module):
             t, hw = _bottleneck(ks, t, hw)
             if j in stage_end:
                 feats.append((t, hw))
-        outs = {}
-        for i in self.return_indices:
-            t, (h, w) = feats[i]
-            outs[f"layer{i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
-        return outs
+        return tb.token_maps(feats, self.return_indices, _layer_name)
 
 
-def _cuda_image(x) -> bool:
-    """a non-empty NCHW-contiguous CUDA fp32 (b, 3, H, W) tensor"""
-    return (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.numel() > 0
-            and x.is_contiguous())
+def _layer_name(i: int) -> str:
+    return f"layer{i + 1}"
 
 
 def _block_convs(blk: Bottleneck) -> List[nn.Conv2d]:

@@ -8,9 +8,10 @@ has exactly the reference feature extractor's keys and shapes.  The full network
 does it (``trunc_normal_(std=0.02)``, zero biases, ``layer_scale`` 1e-6) in the same RNG order, so a seed gives the reference's
 tensors.  ``forward(x)`` returns ``{"features.{2i+1}": map}`` for ``i`` in ``return_indices``, in that order.
 
-``forward`` is the reference's op chain in torch whenever ``tokens_supported(x)`` does not hold: with autograd, on the CPU, in
-train mode with a nonzero stochastic-depth probability, for norms or blocks other than the defaults, and for stage widths that
-are not multiples of 64 (conv_t, conv_s).  Otherwise it is ``forward_tokens(x)``, on token rows ``(b, h*w, C)``:
+``forward`` is the reference's op chain in torch, ``forward_torch(x)``, whenever ``tokens_supported(x)`` does not hold: with
+autograd, on the CPU, in train mode with a nonzero stochastic-depth probability, for norms or blocks other than the defaults,
+and for stage widths that are not multiples of 64 (conv_t, conv_s).  Otherwise it is ``forward_tokens(x)``, on token rows
+``(b, h*w, C)``:
 
 - the stem (``sdetr_convnext_stem``): conv 4x4 / 4 and its LayerNorm2d in fp32 FMAs, read straight from the NCHW batch;
 - per CNBlock 5 launches: the depthwise 7x7 and its LayerNorm (``sdetr_dwconv7x7_layernorm_tokens``, into a buffer of its
@@ -26,17 +27,16 @@ parameter version through ``derived.cached``.  No host synchronisation: the call
 """
 from __future__ import annotations
 
-from collections.abc import Mapping
 from functools import partial
-from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, List, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor, nn
 from torch.nn import functional as F
 from torchvision.ops.stochastic_depth import StochasticDepth
 
-from . import cabi, derived
-from .backbone import _cuda_image
+from . import cabi
+from .token_backbone import FeatureBackbone, tokens_ready
 
 
 class LayerNorm2d(nn.LayerNorm):
@@ -155,7 +155,7 @@ class _KDown:
         self.b = conv.bias.detach()
 
 
-class ConvNeXtBackbone(nn.Module):
+class ConvNeXtBackbone(FeatureBackbone):
     # name -> ConvNeXt arguments (the reference's model_arch table, without the download URLs)
     model_arch = {
         "conv_t": dict(block_setting=[CNBlockConfig(96, 192, 3), CNBlockConfig(192, 384, 3), CNBlockConfig(384, 768, 9),
@@ -167,78 +167,26 @@ class ConvNeXtBackbone(nn.Module):
         "conv_l": dict(block_setting=[CNBlockConfig(192, 384, 3), CNBlockConfig(384, 768, 3), CNBlockConfig(768, 1536, 27),
                                       CNBlockConfig(1536, None, 3)], stochastic_depth_prob=0.5),
     }
+    network, skip_prefixes, kblock, kdown = ConvNeXt, ("classifier.",), _KBlock, _KDown
 
-    def __init__(self, arch: str, weights=None, return_indices: Tuple[int, ...] = (0, 1, 2, 3), freeze_indices: Tuple = (),
-                 **kwargs):
-        super().__init__()
-        if arch not in self.model_arch:
-            raise ValueError(f"Expected architecture in {list(self.model_arch)} but got {arch}")
-        cfg = {**self.model_arch[arch], **kwargs}
-        convnext = ConvNeXt(**cfg)
-        self._load_weights(convnext, weights)
-        feats = convnext.features
-        if len(freeze_indices) > 0:
-            frozen = [feats[0]] + [feats[j] for i in freeze_indices for j in (2 * i + 1, 2 * i + 2) if j < len(feats)]
-            for m in frozen:
-                m.eval()
-                for p in m.parameters():
-                    p.requires_grad = False
-        self.return_indices = tuple(int(i) for i in return_indices)
-        # the modules the feature extractor keeps: the stem and everything up to the last returned stage
-        self.features = nn.Sequential(*list(feats)[:2 * max(self.return_indices) + 2])
-        self.num_channels = [cfg["block_setting"][i].input_channels for i in self.return_indices]
+    def _config(self, arch: str, kwargs: dict) -> dict:
+        return {**self.model_arch[arch], **kwargs}
 
     @staticmethod
-    def _load_weights(convnext: ConvNeXt, weights):
-        """None: keep the initialisation.  A state dict (or one under "model"), or a local path read with torch.load: every key
-        but classifier.* must match the network exactly."""
-        if weights is None:
-            return
-        if isinstance(weights, str):
-            if weights.startswith(("http://", "https://")):
-                raise RuntimeError(f"ConvNeXtBackbone: downloading weights is not supported ({weights}); pass a state dict or "
-                                   "a local file")
-            weights = torch.load(weights, map_location="cpu")
-        if not isinstance(weights, Mapping):
-            raise TypeError(f"ConvNeXtBackbone: weights must be None, a state dict or a path, got {type(weights).__name__}")
-        if "model" in weights:
-            weights = weights["model"]
-        res = convnext.load_state_dict({k: v for k, v in weights.items() if not k.startswith("classifier.")}, strict=False)
-        missing = [k for k in res.missing_keys if not k.startswith("classifier.")]
-        if missing or res.unexpected_keys:
-            raise RuntimeError(f"ConvNeXtBackbone: weights do not match the network: missing {missing}, "
-                               f"unexpected {res.unexpected_keys}")
-
-    def _num_stages(self) -> int:
-        return max(self.return_indices) + 1
-
-    def forward(self, x: Tensor) -> Dict[str, Tensor]:
-        if self.tokens_supported(x):
-            return self.forward_tokens(x)
-        feats = {}
-        x = self.features[0](x)
-        for i in range(self._num_stages()):
-            x = self.features[2 * i + 1](x)
-            feats[i] = x
-            if i + 1 < self._num_stages():
-                x = self.features[2 * i + 2](x)
-        return {f"features.{2 * i + 1}": feats[i] for i in self.return_indices}
+    def _stage_channels(cfg: dict, i: int) -> int:
+        return cfg["block_setting"][i].input_channels
 
     # ---- token-layout inference --------------------------------------------------------------------------------------
     def tokens_supported(self, x) -> bool:
         """True when forward_tokens can run this call: a CUDA fp32 NCHW-contiguous (b, 3, H, W) input whose every map is at least
         1x1, parameters fp32 on its device, nothing that needs a gradient (autograd off, or neither the input nor a parameter
         requires one), no active stochastic depth (train mode with p > 0), and layers_supported()."""
-        if not _cuda_image(x):
+        if not tokens_ready(self, x):
             return False
-        if any(t.device != x.device or t.dtype != torch.float32 for t in list(self.parameters()) + list(self.buffers())):
-            return False
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            return False
-        h, w = x.shape[2] // 4, x.shape[3] // 4
+        hw = (x.shape[2] // 4, x.shape[3] // 4)
         for _ in range(self._num_stages() - 1):
-            h, w = h // 2, w // 2
-        if h < 1 or w < 1:
+            hw = self._down_hw(hw)
+        if hw[0] < 1 or hw[1] < 1:
             return False
         for i in range(self._num_stages()):
             if any(blk.stochastic_depth.training and blk.stochastic_depth.p > 0 for blk in self.features[2 * i + 1]
@@ -303,44 +251,18 @@ class ConvNeXtBackbone(nn.Module):
             n += 5 * len(self.features[2 * i + 1]) + (3 if i + 1 < self._num_stages() else 0)
         return n
 
-    def _kernel_weights(self):
-        """the stem ((48, C) weight, bias, LayerNorm weight, bias, eps) and per kept stage its blocks and the downsample after
-        it (None after the last), rebuilt when any parameter or buffer changes"""
-        def build():
-            conv, ln = self.features[0]
-            c = conv.out_channels
-            stem = (conv.weight.detach().reshape(c, 48).t().contiguous(), conv.bias.detach(), ln.weight.detach(),
-                    ln.bias.detach(), ln.eps)
-            stages = []
-            for i in range(self._num_stages()):
-                blocks = [_KBlock(blk) for blk in self.features[2 * i + 1]]
-                stages.append((blocks, _KDown(self.features[2 * i + 2]) if i + 1 < self._num_stages() else None))
-            return stem, stages
-        return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), build)
+    @staticmethod
+    def _block_tokens(k: _KBlock, t: Tensor, hw: Tuple[int, int]) -> Tensor:
+        u = cabi.dwconv7x7_layernorm_tokens(t, hw, k.dw_w, k.dw_b, k.ln_w, k.ln_b, k.eps)
+        h = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.w1, k.b1)
+        # t = t + gamma * (GELU(h) W2^T + b2): the block writes over its input, which only it reads
+        return cabi.gemm_f16x3_ex(h, cabi.pow2_scale(h, 12), *k.w2, k.b2, act=cabi.ACT_GELU, col_scale=k.gamma, z=t, out=t)
 
-    def forward_tokens(self, x: Tensor) -> Dict[str, Tensor]:
-        """The backbone on ``x`` (b, 3, H, W) -> {"features.{2i+1}": (b, C, h, w)} for i in return_indices, each a channels-last
-        view (strides (h*w*C, 1, w*C, C)) of its own (b, h*w, C) token buffer; the values of forward() in torch.  No host
-        synchronisation."""
-        if not self.tokens_supported(x):
-            raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported)")
-        (stem_w, stem_b, ln_w, ln_b, eps), stages = self._kernel_weights()
-        hw = (x.shape[2] // 4, x.shape[3] // 4)
-        t = cabi.convnext_stem(x, stem_w, stem_b, ln_w, ln_b, eps)
-        feats = []
-        for blocks, ds in stages:
-            for k in blocks:
-                u = cabi.dwconv7x7_layernorm_tokens(t, hw, k.dw_w, k.dw_b, k.ln_w, k.ln_b, k.eps)
-                h = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.w1, k.b1)
-                # t = t + gamma * (GELU(h) W2^T + b2): the block writes over its input, which only it reads
-                cabi.gemm_f16x3_ex(h, cabi.pow2_scale(h, 12), *k.w2, k.b2, act=cabi.ACT_GELU, col_scale=k.gamma, z=t, out=t)
-            feats.append((t, hw))
-            if ds is not None:
-                r = cabi.layernorm_tokens_s2d(t, hw, ds.ln_w, ds.ln_b, ds.eps)
-                hw = (hw[0] // 2, hw[1] // 2)
-                t = cabi.gemm_f16x3_ex(r, cabi.pow2_scale(r, 12), *ds.w, ds.b)
-        outs = {}
-        for i in self.return_indices:
-            t, (h, w) = feats[i]
-            outs[f"features.{2 * i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
-        return outs
+    @staticmethod
+    def _down_tokens(ds: _KDown, t: Tensor, hw: Tuple[int, int]) -> Tensor:
+        r = cabi.layernorm_tokens_s2d(t, hw, ds.ln_w, ds.ln_b, ds.eps)
+        return cabi.gemm_f16x3_ex(r, cabi.pow2_scale(r, 12), *ds.w, ds.b)
+
+    @staticmethod
+    def _down_hw(hw: Tuple[int, int]) -> Tuple[int, int]:
+        return hw[0] // 2, hw[1] // 2

@@ -10,9 +10,10 @@ extractor's keys and shapes, ``relative_position_index`` buffers included.  The 
 reference does it, in the same RNG order, so a seed gives the reference's tensors.  ``forward(x)`` returns
 ``{"features.{2i+1}": map}`` for ``i`` in ``return_indices``, in that order, each the ``permute(0, 3, 1, 2)`` of a BHWC tensor.
 
-``forward`` is the reference's op chain in torch whenever ``tokens_supported(x)`` does not hold: with autograd, on the CPU, with
-active stochastic depth or dropout, for the V2 archs (post-norm, cosine attention, a CPB MLP), and for the 96-wide stages of
-swin_t / swin_s.  Otherwise it is ``forward_tokens(x)``, on token rows ``(b, h*w, C)`` in raster order:
+``forward`` is the reference's op chain in torch, ``forward_torch(x)``, whenever ``tokens_supported(x)`` does not hold: with
+autograd, on the CPU, with active stochastic depth or dropout, for the V2 archs (post-norm, cosine attention, a CPB MLP), and
+for the 96-wide stages of swin_t / swin_s.  Otherwise it is ``forward_tokens(x)``, on token rows ``(b, h*w, C)`` in raster
+order:
 
 - the stem (``sdetr_convnext_stem``): conv 4x4 / 4 and its LayerNorm in fp32 FMAs, read straight from the NCHW batch;
 - per block 11 launches: norm1 (``sdetr_layernorm_tokens``) and its scale, the QKV Linear, the shifted-window attention
@@ -30,10 +31,8 @@ parameter version through ``derived.cached``.  No host synchronisation: the call
 from __future__ import annotations
 
 import inspect
-from collections.abc import Mapping
-from typing import Dict, Tuple
+from typing import Tuple
 
-import torch
 from torch import Tensor, nn
 from torchvision.models.swin_transformer import (  # noqa: F401  (the reference module's classes)
     PatchMerging,
@@ -47,8 +46,8 @@ from torchvision.models.swin_transformer import (  # noqa: F401  (the reference 
 )
 from torchvision.ops import MLP, Permute
 
-from . import cabi, derived
-from .backbone import _cuda_image
+from . import cabi
+from .token_backbone import FeatureBackbone, tokens_ready
 
 
 class _KBlock:
@@ -77,7 +76,7 @@ class _KMerge:
         self.w = cabi.split_f16_pair_dev(pm.reduction.weight.detach())
 
 
-class SwinTransformerBackbone(nn.Module):
+class SwinTransformerBackbone(FeatureBackbone):
     # name -> SwinTransformer arguments (the reference's model_arch table, without the download URLs)
     model_arch = {
         "swin_t": dict(patch_size=(4, 4), embed_dim=96, depths=(2, 2, 6, 2), num_heads=(3, 6, 12, 24), window_size=(7, 7),
@@ -97,68 +96,23 @@ class SwinTransformerBackbone(nn.Module):
         "swin_v2_b": dict(patch_size=[4, 4], embed_dim=128, depths=[2, 2, 18, 2], num_heads=[4, 8, 16, 32], window_size=[8, 8],
                           stochastic_depth_prob=0.5, block=SwinTransformerBlockV2, downsample_layer=PatchMergingV2),
     }
+    network, skip_prefixes, kblock, kdown = SwinTransformer, ("norm.", "head."), _KBlock, _KMerge
 
-    def __init__(self, arch: str, weights=None, return_indices: Tuple[int, ...] = (0, 1, 2, 3), freeze_indices: Tuple = (),
-                 **kwargs):
-        super().__init__()
-        if arch not in self.model_arch:
-            raise ValueError(f"Expected architecture in {list(self.model_arch)} but got {arch}")
+    def _config(self, arch: str, kwargs: dict) -> dict:
         # as the reference merges them: a keyword argument of SwinTransformer overrides the arch's value unless it is None
         names = inspect.signature(SwinTransformer).parameters
         unknown = [k for k in kwargs if k not in names]
         if unknown:
             raise TypeError(f"SwinTransformerBackbone: unexpected keyword arguments {unknown}")
-        cfg = {**self.model_arch[arch], **{k: v for k, v in kwargs.items() if v is not None}}
-        swin = SwinTransformer(**cfg)
-        self._load_weights(swin, weights)
-        feats = swin.features
-        if len(freeze_indices) > 0:
-            frozen = [feats[0]] + [feats[j] for i in freeze_indices for j in (2 * i + 1, 2 * i + 2) if j < len(feats)]
-            for m in frozen:
-                m.eval()
-                for p in m.parameters():
-                    p.requires_grad = False
-        self.return_indices = tuple(int(i) for i in return_indices)
-        # the modules the feature extractor keeps: the stem and everything up to the last returned stage
-        self.features = nn.Sequential(*list(feats)[:2 * max(self.return_indices) + 2])
-        self.num_channels = [cfg["embed_dim"] * 2 ** i for i in self.return_indices]
+        return {**self.model_arch[arch], **{k: v for k, v in kwargs.items() if v is not None}}
 
     @staticmethod
-    def _load_weights(swin: SwinTransformer, weights):
-        """None: keep the initialisation.  A state dict (or one under "model"), or a local path read with torch.load: every key
-        but norm.* and head.* must match the network exactly."""
-        if weights is None:
-            return
-        if isinstance(weights, str):
-            if weights.startswith(("http://", "https://")):
-                raise RuntimeError(f"SwinTransformerBackbone: downloading weights is not supported ({weights}); pass a state "
-                                   "dict or a local file")
-            weights = torch.load(weights, map_location="cpu")
-        if not isinstance(weights, Mapping):
-            raise TypeError(f"SwinTransformerBackbone: weights must be None, a state dict or a path, got {type(weights).__name__}")
-        if "model" in weights:
-            weights = weights["model"]
-        skip = ("norm.", "head.")
-        res = swin.load_state_dict({k: v for k, v in weights.items() if not k.startswith(skip)}, strict=False)
-        missing = [k for k in res.missing_keys if not k.startswith(skip)]
-        if missing or res.unexpected_keys:
-            raise RuntimeError(f"SwinTransformerBackbone: weights do not match the network: missing {missing}, "
-                               f"unexpected {res.unexpected_keys}")
+    def _stage_channels(cfg: dict, i: int) -> int:
+        return cfg["embed_dim"] * 2 ** i
 
-    def _num_stages(self) -> int:
-        return max(self.return_indices) + 1
-
-    def forward(self, x: Tensor) -> Dict[str, Tensor]:
-        if self.tokens_supported(x):
-            return self.forward_tokens(x)
-        feats = {}
-        x = self.features[0](x)
-        for i in range(self._num_stages()):
-            x = self.features[2 * i + 1](x)
-            feats[i] = x
-            if i + 1 < self._num_stages():
-                x = self.features[2 * i + 2](x)
-        return {f"features.{2 * i + 1}": feats[i].permute(0, 3, 1, 2) for i in self.return_indices}
+    @staticmethod
+    def _nchw(x: Tensor) -> Tensor:
+        return x.permute(0, 3, 1, 2)
 
     # ---- token-layout inference --------------------------------------------------------------------------------------
     def tokens_supported(self, x) -> bool:
@@ -166,13 +120,7 @@ class SwinTransformerBackbone(nn.Module):
         1x1, parameters fp32 on its device, nothing that needs a gradient (autograd off, or neither the input nor a parameter
         requires one), no active stochastic depth, dropout or attention dropout (train mode with p > 0), and
         layers_supported()."""
-        if not _cuda_image(x) or x.shape[2] < 4 or x.shape[3] < 4:
-            return False
-        if any(p.device != x.device or p.dtype != torch.float32 for p in self.parameters()):
-            return False
-        if any(t.device != x.device for t in self.buffers()):
-            return False
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
+        if not tokens_ready(self, x) or x.shape[2] < 4 or x.shape[3] < 4:
             return False
         for m in self.features.modules():
             if isinstance(m, SwinTransformerBlock):
@@ -245,48 +193,22 @@ class SwinTransformerBackbone(nn.Module):
             n += 11 * len(self.features[2 * i + 1]) + (3 if i + 1 < self._num_stages() else 0)
         return n
 
-    def _kernel_weights(self):
-        """the stem ((48, C) weight, bias, LayerNorm weight, bias, eps) and per kept stage its blocks and the PatchMerging after
-        it (None after the last), rebuilt when any parameter or buffer changes"""
-        def build():
-            conv, _, ln = self.features[0]
-            c = conv.out_channels
-            stem = (conv.weight.detach().reshape(c, 48).t().contiguous(), conv.bias.detach(), ln.weight.detach(),
-                    ln.bias.detach(), ln.eps)
-            stages = []
-            for i in range(self._num_stages()):
-                blocks = [_KBlock(blk) for blk in self.features[2 * i + 1]]
-                stages.append((blocks, _KMerge(self.features[2 * i + 2]) if i + 1 < self._num_stages() else None))
-            return stem, stages
-        return derived.cached(self, "kernel_weights", list(self.parameters()) + list(self.buffers()), build)
+    @staticmethod
+    def _block_tokens(k: _KBlock, t: Tensor, hw: Tuple[int, int]) -> Tensor:
+        # t = t + proj(attention(norm1(t))), then t = t + fc2(GELU(fc1(norm2(t)))): written over the block input
+        u = cabi.layernorm_tokens(t, *k.ln1)
+        qkv = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.wqkv, k.bqkv)
+        a = cabi.window_attention_tokens(qkv, hw, k.bqkv, k.rel_bias, k.heads, k.window, k.shift)
+        cabi.gemm_f16x3_ex(a, cabi.pow2_scale(a, 12), *k.wproj, k.bproj, z=t, out=t)
+        u = cabi.layernorm_tokens(t, *k.ln2)
+        h = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.w1, k.b1)
+        return cabi.gemm_f16x3_ex(h, cabi.pow2_scale(h, 12), *k.w2, k.b2, act=cabi.ACT_GELU, z=t, out=t)
 
-    def forward_tokens(self, x: Tensor) -> Dict[str, Tensor]:
-        """The backbone on ``x`` (b, 3, H, W) -> {"features.{2i+1}": (b, C, h, w)} for i in return_indices, each a channels-last
-        view (strides (h*w*C, 1, w*C, C)) of its own (b, h*w, C) token buffer; the values of forward() in torch.  No host
-        synchronisation."""
-        if not self.tokens_supported(x):
-            raise RuntimeError("forward_tokens: this call needs forward() (see tokens_supported)")
-        (stem_w, stem_b, ln_w, ln_b, eps), stages = self._kernel_weights()
-        hw = (x.shape[2] // 4, x.shape[3] // 4)
-        t = cabi.convnext_stem(x, stem_w, stem_b, ln_w, ln_b, eps)
-        feats = []
-        for blocks, pm in stages:
-            for k in blocks:
-                # t = t + proj(attention(norm1(t))), then t = t + fc2(GELU(fc1(norm2(t)))): written over the block input
-                u = cabi.layernorm_tokens(t, *k.ln1)
-                qkv = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.wqkv, k.bqkv)
-                a = cabi.window_attention_tokens(qkv, hw, k.bqkv, k.rel_bias, k.heads, k.window, k.shift)
-                cabi.gemm_f16x3_ex(a, cabi.pow2_scale(a, 12), *k.wproj, k.bproj, z=t, out=t)
-                u = cabi.layernorm_tokens(t, *k.ln2)
-                h = cabi.gemm_f16x3_ex(u, cabi.pow2_scale(u, 12), *k.w1, k.b1)
-                cabi.gemm_f16x3_ex(h, cabi.pow2_scale(h, 12), *k.w2, k.b2, act=cabi.ACT_GELU, z=t, out=t)
-            feats.append((t, hw))
-            if pm is not None:
-                r = cabi.patch_merge_layernorm_tokens(t, hw, *pm.ln)
-                hw = ((hw[0] + 1) // 2, (hw[1] + 1) // 2)
-                t = cabi.gemm_f16x3_ex(r, cabi.pow2_scale(r, 12), *pm.w)
-        outs = {}
-        for i in self.return_indices:
-            t, (h, w) = feats[i]
-            outs[f"features.{2 * i + 1}"] = t.unflatten(1, (h, w)).permute(0, 3, 1, 2)
-        return outs
+    @staticmethod
+    def _down_tokens(pm: _KMerge, t: Tensor, hw: Tuple[int, int]) -> Tensor:
+        r = cabi.patch_merge_layernorm_tokens(t, hw, *pm.ln)
+        return cabi.gemm_f16x3_ex(r, cabi.pow2_scale(r, 12), *pm.w)
+
+    @staticmethod
+    def _down_hw(hw: Tuple[int, int]) -> Tuple[int, int]:
+        return (hw[0] + 1) // 2, (hw[1] + 1) // 2

@@ -13,33 +13,13 @@ import torch.nn.functional as F
 
 import salience_detr_b200 as pkg
 from salience_detr_b200 import backbone as bbm
-from salience_detr_b200 import cabi, synthetic
+from salience_detr_b200 import cabi
+from backbone_harness import DEV, FBN
+from backbone_harness import resnet_backbone as _backbone
+from backbone_harness import resnet_images as _padded_images
 from conftest import GOLDEN
 from tools import make_backbone_golden as mbg
 from tools import make_backbone_grad_golden as mgg
-
-DEV = "cuda:0"
-FBN = pkg.FrozenBatchNorm2d
-
-
-def _weights(arch="resnet50"):
-    net = bbm.ResNet(**pkg.ResNetBackbone.model_arch[arch], norm_layer=FBN)
-    return synthetic.resnet_weights({k: list(v.shape) for k, v in net.state_dict().items() if not k.startswith("fc.")},
-                                    mbg.WEIGHT_SEED)
-
-
-def _backbone(arch="resnet50", return_indices=(1, 2, 3), freeze_indices=(0,), **kw):
-    return pkg.ResNetBackbone(arch, weights=_weights(arch), return_indices=return_indices, freeze_indices=freeze_indices,
-                              norm_layer=kw.pop("norm_layer", FBN), **kw)
-
-
-def _padded_images(b, H, W, gen):
-    """b images in an (H, W) batch, image i of (H - 3 i, W - 5 i) pixels and zero padding"""
-    x = torch.zeros(b, 3, H, W)
-    for i in range(b):
-        h, w = max(1, H - 3 * i), max(1, W - 5 * i)
-        x[i, :, :h, :w] = torch.randn(3, h, w, generator=gen)
-    return x
 
 
 def _loss(outs, cot):

@@ -3,11 +3,8 @@ tests/golden/swin_l_backbone.npz, made by tools/make_swin_golden.py from the ref
 window-attention kernel's index arithmetic against the reference's shifted_window_attention, and on the H100 the token path's
 kernels and the module against float64."""
 import copy
-import json
 import math
-import os
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -16,51 +13,18 @@ from torchvision.models.swin_transformer import _patch_merging_pad
 
 import salience_detr_b200 as pkg
 from salience_detr_b200 import swin as swm
-from salience_detr_b200 import synthetic
-from conftest import GOLDEN
-from tools import make_swin_golden as msg
+from backbone_harness import (DEV, chain_graph_matches_eager, check_golden_outputs_on_gpu,
+                              check_no_sync_graph_replay_repeatability_and_launches, check_weight_loading, errors, golden,
+                              mapper_chain, padded_images, rel_err, swin_weights, tf32)
+from backbone_harness import swin_backbone as _backbone
 
-DEV = "cuda:0"
 STB = pkg.SwinTransformerBackbone
 TOKEN_ARCHS = ("swin_b", "swin_l", "swin_b_384", "swin_l_384")
 
 
-def _golden():
-    z = np.load(os.path.join(GOLDEN, "swin_l_backbone.npz"), allow_pickle=False)
-    return {k: (json.loads(str(z[k])) if k.endswith("_json") else torch.from_numpy(z[k])) for k in z.files}
-
-
-def _recipe_weights(arch="swin_l", seed=msg.WEIGHT_SEED):
-    """synthetic.swin_weights for every key of the full network of ``arch`` but norm.* and head.*"""
-    net = swm.SwinTransformer(**STB.model_arch[arch])
-    return synthetic.swin_weights({k: v for k, v in net.state_dict().items() if not k.startswith(("norm.", "head."))}, seed)
-
-
-_WEIGHTS = {}
-
-
-def _backbone(arch="swin_l", return_indices=(1, 2, 3), freeze_indices=(0,), **kw):
-    if arch not in _WEIGHTS:
-        _WEIGHTS[arch] = _recipe_weights(arch)
-    return STB(arch, weights=_WEIGHTS[arch], return_indices=return_indices, freeze_indices=freeze_indices, **kw).eval()
-
-
-def torch_chain(m, x):
-    """the reference's forward written out with the modules (what forward() runs when tokens_supported does not hold)"""
-    feats = {}
-    x = m.features[0](x)
-    n = max(m.return_indices) + 1
-    for i in range(n):
-        x = m.features[2 * i + 1](x)
-        feats[i] = x
-        if i + 1 < n:
-            x = m.features[2 * i + 2](x)
-    return {f"features.{2 * i + 1}": feats[i].permute(0, 3, 1, 2) for i in m.return_indices}
-
-
 # ---- CPU: the module against the reference --------------------------------------------------------------------------------
 def test_state_dict_init_and_freeze_match_reference():
-    g = _golden()
+    g = golden("swin_l_backbone")
     m = _backbone()
     assert {k: list(v.shape) for k, v in m.state_dict().items()} == g["shapes_json"]
     assert len(g["shapes_json"]) == 349 and sum(k.endswith("relative_position_index") for k in g["shapes_json"]) == 24
@@ -77,7 +41,7 @@ def test_state_dict_init_and_freeze_match_reference():
 
 
 def test_torch_forward_matches_reference():
-    g = _golden()
+    g = golden("swin_l_backbone")
     m = _backbone()
     with torch.no_grad():
         outs = m(g["image"])
@@ -133,28 +97,11 @@ def test_kwargs_work_as_in_reference():
 
 
 def test_weights_from_dict_model_and_path(tmp_path):
-    sd = _recipe_weights("swin_b")
-    full = dict(sd, **{"norm.weight": torch.ones(1024), "norm.bias": torch.zeros(1024),
-                       "head.weight": torch.zeros(1000, 1024), "head.bias": torch.zeros(1000)})
-    want = STB("swin_b", weights=sd, return_indices=(1, 2, 3)).state_dict()
-    assert all(torch.equal(want[k], sd[k]) for k in want)
-    for w in (full, {"model": full}):
-        m = STB("swin_b", weights=w, return_indices=(1, 2, 3))
-        assert all(torch.equal(m.state_dict()[k], v) for k, v in want.items())
-    path = tmp_path / "swin_b.pth"
-    torch.save({"model": full}, path)
-    m = STB("swin_b", weights=str(path), return_indices=(1, 2, 3))
-    assert all(torch.equal(m.state_dict()[k], v) for k, v in want.items())
-    with pytest.raises(RuntimeError, match="missing"):
-        STB("swin_b", weights={k: v for k, v in sd.items() if k != "features.1.0.attn.relative_position_index"})
-    with pytest.raises(RuntimeError, match="unexpected"):
-        STB("swin_b", weights=dict(sd, extra=torch.zeros(1)))
-    with pytest.raises(RuntimeError, match="size mismatch"):
-        STB("swin_b", weights=dict(sd, **{"features.0.0.bias": torch.zeros(3)}))
-    with pytest.raises(RuntimeError, match="downloading weights is not supported"):
-        STB("swin_b", weights="https://download.pytorch.org/models/swin_b-68c6b09e.pth")
-    with pytest.raises(ValueError, match="architecture"):
-        STB("swin_xl")
+    check_weight_loading(tmp_path, STB, "swin_b", swin_weights, {},
+                         classifier={"norm.weight": torch.ones(1024), "norm.bias": torch.zeros(1024),
+                                     "head.weight": torch.zeros(1000, 1024), "head.bias": torch.zeros(1000)},
+                         drop="features.1.0.attn.relative_position_index", resize="features.0.0.bias",
+                         url="https://download.pytorch.org/models/swin_b-68c6b09e.pth", bad_arch="swin_xl")
 
 
 def test_tokens_supported_false_cases():
@@ -342,36 +289,6 @@ def test_layernorm_tokens_vs_fp64(rows, C):
 
 
 # ---- GPU: forward_tokens --------------------------------------------------------------------------------------------------
-def _rel_err(got, ref):
-    return float((got.double() - ref).abs().max()) / float(ref.abs().max())
-
-
-def _padded_images(b, H, W, gen):
-    x = torch.zeros(b, 3, H, W)
-    for i in range(b):
-        h, w = max(1, H - 37 * i), max(1, W - 61 * i)
-        x[i, :, :h, :w] = torch.randn(3, h, w, generator=gen)
-    return x
-
-
-def _errors(m, x):
-    """per output: (token path, torch fp32, torch TF32) max |err| / max |ref| against forward() in float64"""
-    m64 = copy.deepcopy(m).double()
-    with torch.no_grad():
-        ref = m64(x.double())
-        del m64
-        tok = m(x)
-        flags = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-        try:
-            torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-            fp32 = torch_chain(m, x)
-            torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = True
-            t32 = torch_chain(m, x)
-        finally:
-            torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = flags
-    return {k: (_rel_err(tok[k], ref[k]), _rel_err(fp32[k], ref[k]), _rel_err(t32[k], ref[k])) for k in ref}, tok
-
-
 FWD_CASES = {
     "l_64x100": ("swin_l", (1, 2, 3), 2, 64, 100),
     "l_ragged_all": ("swin_l", (0, 1, 2, 3), 3, 200, 312),
@@ -388,10 +305,10 @@ def test_forward_tokens_vs_fp64(case):
     TF32's."""
     arch, ri, b, H, W = FWD_CASES[case]
     m = _backbone(arch, return_indices=ri).to(DEV)
-    x = _padded_images(b, H, W, torch.Generator().manual_seed(H + W)).to(DEV)
+    x = padded_images(b, H, W, torch.Generator().manual_seed(H + W)).to(DEV)
     with torch.no_grad():
         assert m.tokens_supported(x)
-    errs, tok = _errors(m, x)
+    errs, tok = errors(m, x)
     assert list(tok) == [f"features.{2 * i + 1}" for i in ri]
     for k, (e_tok, e_fp32, e_tf32) in errs.items():
         print(f"{case} {k}: tokens {e_tok:.3e}  torch fp32 {e_fp32:.3e}  TF32 {e_tf32:.3e}")
@@ -406,49 +323,20 @@ def test_forward_tokens_vs_fp64(case):
 
 @pytest.mark.gpu
 def test_golden_outputs_on_gpu():
-    g = _golden()
-    m = _backbone().to(DEV)
-    with torch.no_grad():
-        assert m.tokens_supported(g["image"].to(DEV))
-        outs = m(g["image"].to(DEV))
-    for k, v in outs.items():
-        want = g[f"out.{k}"]
-        assert float((v.cpu() - want).abs().max()) <= 1e-5 * float(want.abs().max()), k
+    check_golden_outputs_on_gpu(_backbone(), "swin_l_backbone")
 
 
 @pytest.mark.gpu
 def test_no_sync_graph_replay_repeatability_and_launches():
     m = _backbone().to(DEV)
-    x = _padded_images(2, 97, 131, torch.Generator().manual_seed(3)).to(DEV)
-    with torch.no_grad():
-        eager = m(x)  # also builds the kernel weights outside the capture
-        eager = {k: v.clone() for k, v in eager.items()}
-        torch.cuda.synchronize()
-        torch.cuda.set_sync_debug_mode("error")
-        try:
-            n0 = pkg.cabi.launch_count()
-            again = m(x)
-            assert pkg.cabi.launch_count() - n0 == m.launches_per_forward() == 274
-        finally:
-            torch.cuda.set_sync_debug_mode("default")
-        assert all(torch.equal(eager[k], again[k]) for k in eager)
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            m(x)
-        torch.cuda.current_stream().wait_stream(s)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            out = m(x)
-        graph.replay()
-        torch.cuda.synchronize()
-    assert all(torch.equal(out[k], eager[k]) for k in eager)
+    x = padded_images(2, 97, 131, torch.Generator().manual_seed(3)).to(DEV)
+    check_no_sync_graph_replay_repeatability_and_launches(m, x, 274)
 
 
 @pytest.mark.gpu
 def test_kernel_weights_follow_parameter_changes():
     m = _backbone().to(DEV)
-    x = _padded_images(1, 64, 100, torch.Generator().manual_seed(4)).to(DEV)
+    x = padded_images(1, 64, 100, torch.Generator().manual_seed(4)).to(DEV)
     with torch.no_grad():
         outs = [m(x)["features.7"].clone()]
         m.features[5][3].attn.relative_position_bias_table.mul_(-1.0)
@@ -459,7 +347,7 @@ def test_kernel_weights_follow_parameter_changes():
         outs.append(m(x)["features.7"])
         want = copy.deepcopy(m).double()(x.double())["features.7"]
     assert all(not torch.equal(a, b) for a, b in zip(outs, outs[1:]))
-    assert _rel_err(outs[-1], want) < 1e-5
+    assert rel_err(outs[-1], want) < 1e-5
 
 
 @pytest.mark.gpu
@@ -467,7 +355,7 @@ def test_kernel_weights_follow_parameter_changes():
 def test_torch_path_on_cuda_is_the_op_chain(name):
     arch = name if name.startswith("swin_") else "swin_b"
     m = STB(arch, return_indices=(1, 2, 3), freeze_indices=(0, 1, 2, 3) if name != "param_grad" else (0,)).to(DEV).eval()
-    x = _padded_images(1, 64, 96, torch.Generator().manual_seed(5)).to(DEV)
+    x = padded_images(1, 64, 96, torch.Generator().manual_seed(5)).to(DEV)
     if name == "input_grad":
         x.requires_grad_(True)
     if name == "stochastic_depth":
@@ -482,7 +370,7 @@ def test_torch_path_on_cuda_is_the_op_chain(name):
         n0 = pkg.cabi.launch_count()
         got = m(x)
         assert pkg.cabi.launch_count() == n0
-        want = torch_chain(m, x)
+        want = m.forward_torch(x)
     assert list(got) == list(want) and all(torch.equal(got[k], want[k]) for k in got)
     if name in ("input_grad", "param_grad"):
         with pytest.raises(RuntimeError, match="needs forward"):
@@ -496,53 +384,14 @@ def test_backbone_mapper_encoder_chain():
     """images -> Swin-L (channels-last views) -> ChannelMapper(in_channels=num_channels) with zero transposes ->
     forward_encoder: the mapper's tokens within 8x the error of the torch fp32 backbone chain against the float64 backbone, and
     the whole chain in one CUDA graph"""
-    from oracle import make_golden as mg
-    from oracle import oracle as orc
-    from test_backbone import _encoder
-
-    sizes = mg.image_sizes(True)
-    _, masks, pos = orc.synthetic_inputs(sizes, (480, 640), 256, seed=mg.HALF_INPUT_SEED)
-    masks, pos = [m.to(DEV) for m in masks], [p.to(DEV) for p in pos]
-    gen = torch.Generator().manual_seed(21)
-    x = torch.zeros(len(sizes), 3, 480, 640)
-    for i, (h, w) in enumerate(sizes):
-        x[i, :, :h, :w] = torch.randn(3, h, w, generator=gen)
-    x = x.to(DEV)
     bb = _backbone().to(DEV)
-    torch.manual_seed(11)
-    mapper = pkg.ChannelMapper(bb.num_channels, 256, 4).eval().to(DEV)
-    tr = _encoder()
+    c = mapper_chain(bb)
+    with torch.no_grad(), tf32(False):
+        fp32_feats = bb.forward_torch(c.x)
     with torch.no_grad():
-        feats = bb(x)
-        mapper(feats)  # builds the mapper's kernel weights
-        assert [tuple(v.shape[2:]) for v in feats.values()] == [tuple(m.shape[1:]) for m in masks[:3]]
-        n0 = pkg.cabi.launch_count()
-        mapped, _ = mapper.forward_tokens(feats)
-        assert pkg.cabi.launch_count() - n0 == mapper.launches_per_forward(0)  # no transposes
-        plan = tr.make_plan(masks)
-        mem = tr.forward_encoder(mapper(feats), masks, pos, plan=plan)[0]
-        ref_feats = copy.deepcopy(bb).double()(x.double())
-        ref_mapped = mapper.forward_tokens({k: v.float().contiguous(memory_format=torch.channels_last)
-                                            for k, v in ref_feats.items()})[0]
-        flags = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-        try:
-            torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-            fp32_feats = torch_chain(bb, x)
-        finally:
-            torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = flags
-        fp32_mapped = mapper.forward_tokens({k: v.contiguous(memory_format=torch.channels_last) for k, v in fp32_feats.items()})[0]
-        e_tok, e_fp32 = _rel_err(mapped, ref_mapped.double()), _rel_err(fp32_mapped, ref_mapped.double())
-        print(f"mapper tokens: backbone tokens {e_tok:.3e}, torch fp32 {e_fp32:.3e}")
-        assert e_tok <= 8 * e_fp32
-
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            tr.forward_encoder(mapper(bb(x)), masks, pos, plan=plan)
-        torch.cuda.current_stream().wait_stream(s)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            out = tr.forward_encoder(mapper(bb(x)), masks, pos, plan=plan)[0]
-        graph.replay()
-        torch.cuda.synchronize()
-    assert torch.equal(out, mem)
+        fp32_mapped = c.mapper.forward_tokens({k: v.contiguous(memory_format=torch.channels_last)
+                                               for k, v in fp32_feats.items()})[0]
+    e_tok, e_fp32 = rel_err(c.mapped, c.ref_mapped.double()), rel_err(fp32_mapped, c.ref_mapped.double())
+    print(f"mapper tokens: backbone tokens {e_tok:.3e}, torch fp32 {e_fp32:.3e}")
+    assert e_tok <= 8 * e_fp32
+    assert chain_graph_matches_eager(bb, c)

@@ -69,15 +69,6 @@ def peak_mb(fn):
     return round(peak / 2 ** 20, 1)
 
 
-def torch_forward(m, x):
-    x = m.maxpool(m.relu(m.bn1(m.conv1(x))))
-    feats = []
-    for i in range(max(m.return_indices) + 1):
-        x = getattr(m, f"layer{i + 1}")(x)
-        feats.append(x)
-    return {f"layer{i + 1}": feats[i] for i in m.return_indices}
-
-
 def capture(fn):
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -140,12 +131,12 @@ def main():
         m_cl = copy.deepcopy(m).to(memory_format=torch.channels_last)
         with torch.no_grad():
             with FlopCounterMode(display=False) as fc:
-                torch_forward(m, x)
+                m.forward_torch(x)
             gflop = fc.get_total_flops() / 1e9
             arms = {"tokens": (lambda: m.forward_tokens(x), None),
-                    "torch_cudnn_fp32": (lambda: torch_forward(m, x), False),
-                    "torch_cudnn_tf32": (lambda: torch_forward(m, x), True),
-                    "torch_cudnn_tf32_channels_last": (lambda: torch_forward(m_cl, x_cl), True)}
+                    "torch_cudnn_fp32": (lambda: m.forward_torch(x), False),
+                    "torch_cudnn_tf32": (lambda: m.forward_torch(x), True),
+                    "torch_cudnn_tf32_channels_last": (lambda: m_cl.forward_torch(x_cl), True)}
             ref = copy.deepcopy(m).double()(x.double())
             info = {}
             for name, (fn, tf32) in arms.items():
@@ -210,7 +201,7 @@ def main():
         plan = model.make_plan(masks)
         torch.backends.cudnn.allow_tf32 = True
         e2e = {"images_to_memory_tokens_graph": capture(lambda: model.forward_encoder(mapper(m(x)), masks, None, plan=plan)[0]),
-               "images_to_memory_torch_tf32_graph": capture(lambda: model.forward_encoder(mapper(torch_forward(m, x)), masks, None,
+               "images_to_memory_torch_tf32_graph": capture(lambda: model.forward_encoder(mapper(m.forward_torch(x)), masks, None,
                                                                                           plan=plan)[0])}
         res = {k: [] for k in e2e}
         for _ in range(a.rounds):

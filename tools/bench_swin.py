@@ -28,18 +28,6 @@ from salience_detr_b200.swin import SwinTransformer  # noqa: E402
 from tools.bench_backbone import B, H, W, capture, card, gpu_events, peak_mb, timed  # noqa: E402
 
 
-def torch_forward(m, x):
-    feats = {}
-    x = m.features[0](x)
-    n = max(m.return_indices) + 1
-    for i in range(n):
-        x = m.features[2 * i + 1](x)
-        feats[i] = x
-        if i + 1 < n:
-            x = m.features[2 * i + 2](x)
-    return {f"features.{2 * i + 1}": feats[i].permute(0, 3, 1, 2) for i in m.return_indices}
-
-
 def set_tf32(conv, matmul):
     torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = conv, matmul
 
@@ -77,13 +65,13 @@ def main():
     m_cl = copy.deepcopy(m).to(memory_format=torch.channels_last)
     with torch.no_grad():
         with FlopCounterMode(display=False) as fc:
-            torch_forward(m, x)
+            m.forward_torch(x)
         gflop = fc.get_total_flops() / 1e9
         arms = {"tokens": (lambda: m.forward_tokens(x), None),
-                "torch_fp32": (lambda: torch_forward(m, x), (False, False)),
-                "torch_defaults": (lambda: torch_forward(m, x), (True, False)),
-                "torch_tf32": (lambda: torch_forward(m, x), (True, True)),
-                "torch_tf32_channels_last": (lambda: torch_forward(m_cl, x_cl), (True, True))}
+                "torch_fp32": (lambda: m.forward_torch(x), (False, False)),
+                "torch_defaults": (lambda: m.forward_torch(x), (True, False)),
+                "torch_tf32": (lambda: m.forward_torch(x), (True, True)),
+                "torch_tf32_channels_last": (lambda: m_cl.forward_torch(x_cl), (True, True))}
         ref = copy.deepcopy(m).double()(x.double())
         info = {}
         for name, (fn, tf32) in arms.items():
@@ -136,7 +124,7 @@ def main():
         plan = model.make_plan(masks)
         set_tf32(True, True)
         e2e = {"images_to_memory_tokens_graph": capture(lambda: model.forward_encoder(mapper(m(x)), masks, None, plan=plan)[0]),
-               "images_to_memory_torch_tf32_graph": capture(lambda: model.forward_encoder(mapper(torch_forward(m, x)), masks, None,
+               "images_to_memory_torch_tf32_graph": capture(lambda: model.forward_encoder(mapper(m.forward_torch(x)), masks, None,
                                                                                           plan=plan)[0])}
         res = {k: [] for k in e2e}
         for _ in range(a.rounds):

@@ -22,6 +22,9 @@ Differences from the reference:
   sync: the problem is flagged on the device, gets a defined fallback assignment, and every loss of its output is NaN, which
   the caller's finite-loss check catches.  The per-image ``HungarianMatcher.forward`` reads the flag and raises ``ValueError``
   like the reference.
+* Where several assignments reach the same minimum cost (exactly tied costs), the matcher may return a different one from
+  scipy's: both are optimal, but the solver breaks ties toward the lowest query index and scipy's search visits the
+  queries in another order.  The result is still deterministic.
 * ``mixed_match`` (Align-DETR) is not implemented.
 * Inputs must be CUDA tensors; CPU inputs raise ``RuntimeError``.
 """

@@ -390,6 +390,17 @@ int sdetr_split_f16_pair(const float *W, int64_t count, float scale, void *W_hi,
  * C row pitch ldc (TMA stores when ldc % 4 == 0). */
 int sdetr_gemm_f16x3_pre(const float *A, int64_t lda, const void *W_hi, const void *W_lo, float w_scale, const float *bias,
                          float *C, int64_t ldc, int M, int N, int K, int act, sdetr_stream_t stream);
+/* The encoder's class-score head and its per-row max in one launch: out[row] = max_c (A . W^T + bias)[row, c] * row_scale[row],
+ * with the product of sdetr_gemm_f16x3_pre (W split by sdetr_split_f16_pair with scale w_scale; N <= 128; K % 64 == 0) and
+ * the max of sdetr_class_max_times_fg (a NaN value propagates): bit for bit that pair, without the M x N logits. */
+int sdetr_gemm_f16x3_rowmax(const float *A, int64_t lda, const void *W_hi, const void *W_lo, float w_scale, const float *bias,
+                            const float *row_scale, float *out, int M, int N, int K, sdetr_stream_t stream);
+/* An encoder layer's output projection, residual and norm1 in one launch: q = LayerNorm(q + A . W^T + bias) * gamma + beta,
+ * A (M,256) with row pitch lda, W (256,256) split by sdetr_split_f16_pair with scale w_scale, q (M,256) contiguous and
+ * rewritten in place; bias may be NULL.  Bit for bit sdetr_gemm_f16x3_pre followed by sdetr_add_layernorm(q, C, ..., q). */
+int sdetr_gemm_f16x3_add_layernorm(const float *A, int64_t lda, const void *W_hi, const void *W_lo, float w_scale,
+                                   const float *bias, const float *gamma, const float *beta, float eps, float *q, int M,
+                                   sdetr_stream_t stream);
 /* The same product with BOTH scales as device scalars (powers of two; sdetr_pow2_scale): the kernel multiplies A by *a_scale_dev
  * instead of the fixed 16 (activations of unknown magnitude: gradients), the weight pair was split with *w_scale_dev
  * (sdetr_split_f16_pair_dev: weights that change every training step, no host read of max|W|), and the epilogue divides both out.

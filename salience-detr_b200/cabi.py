@@ -71,6 +71,8 @@ SIGNATURES = {
     "sdetr_mask_predictor_level_workspace_floats": (_i64, [_i, _i, _i]),
     "sdetr_mask_predictor_level": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _i64, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _vp, _vp, _vp, _i64, _vp, _i64, _vp]),
+    "sdetr_gemm_f16x3_rowmax": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "sdetr_gemm_f16x3_add_layernorm": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _vp, _f, _vp, _i, _vp]),
     "sdetr_ffn_fused_workspace_floats": (_i64, [_i, _i]),
     "sdetr_ffn_fused_layernorm": (_i, [_vp, _i64, _vp, _vp, _f, _vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _i, _i, _vp, _i64, _vp, _vp]),
     "sdetr_flatten_set_vectorized": (_i, [_i]),
@@ -762,6 +764,46 @@ def gemm_f16x3_pre(x, w_hi, w_lo, w_scale, bias=None, act=0, out=None):
     _check(rc, "sdetr_gemm_f16x3_pre")
     y = y if ldc == N else y[:, :N]
     return y.reshape(*x.shape[:-1], N) if ldc == N else y.unflatten(0, x.shape[:-1])
+
+
+def gemm_f16x3_rowmax(x, w_hi, w_lo, w_scale, bias, row_scale):
+    """max over the N <= 128 columns of (x @ W.T + bias), times row_scale, per row of x (..., K): bit for bit
+    ``class_max_times_fg(gemm_f16x3_pre(x, w_hi, w_lo, w_scale, bias), row_scale)`` in one launch.  -> x.shape[:-1]"""
+    K = x.shape[-1]
+    if not (x.is_cuda and x.dtype == torch.float32 and x.stride(-1) == 1):
+        raise RuntimeError("gemm_f16x3_rowmax needs a CUDA float32 input with unit last stride")
+    x2 = x if x.dim() == 2 else x.reshape(-1, K)
+    M = x2.shape[0]
+    rs = _req(row_scale, "row_scale", torch.float32)
+    if row_scale.numel() != M:
+        raise RuntimeError(f"gemm_f16x3_rowmax: row_scale must hold one value per row ({M})")
+    out = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+    rc = lib().sdetr_gemm_f16x3_rowmax(x2.data_ptr(), x2.stride(0) if M > 1 else K, _req(w_hi, "w_hi", torch.float16),
+                                       _req(w_lo, "w_lo", torch.float16), float(w_scale),
+                                       _req(bias, "bias", torch.float32) if bias is not None else None, rs, out.data_ptr(),
+                                       M, w_hi.shape[0], K, _stream())
+    _check(rc, "sdetr_gemm_f16x3_rowmax")
+    return out
+
+
+def gemm_f16x3_add_layernorm_(q, x, w_hi, w_lo, w_scale, bias, gamma, beta, eps: float = 1e-5):
+    """q = LayerNorm(q + x @ W.T + bias) * gamma + beta in place, W (256, 256) as a ``split_f16_pair`` triple: bit for bit
+    ``add_layernorm(q, gemm_f16x3_pre(x, ...), gamma, beta, eps, out=q)`` in one launch.  q (..., 256) contiguous, x of the
+    same rows with unit last stride."""
+    if not (q.is_cuda and q.dtype == torch.float32 and q.shape[-1] == 256 and q.is_contiguous()):
+        raise RuntimeError("gemm_f16x3_add_layernorm_ needs a contiguous CUDA float32 (..., 256) q")
+    if not (x.is_cuda and x.dtype == torch.float32 and x.shape[-1] == 256 and x.stride(-1) == 1):
+        raise RuntimeError("gemm_f16x3_add_layernorm_ needs a CUDA float32 (..., 256) x with unit last stride")
+    x2 = x if x.dim() == 2 else x.reshape(-1, 256)
+    M = x2.shape[0]
+    if q.numel() != M * 256 or tuple(w_hi.shape) != (256, 256):
+        raise RuntimeError("gemm_f16x3_add_layernorm_: q and x must have the same rows, W must be (256, 256)")
+    rc = lib().sdetr_gemm_f16x3_add_layernorm(
+        x2.data_ptr(), x2.stride(0) if M > 1 else 256, _req(w_hi, "w_hi", torch.float16), _req(w_lo, "w_lo", torch.float16),
+        float(w_scale), _req(bias, "bias", torch.float32) if bias is not None else None, _req(gamma, "gamma", torch.float32),
+        _req(beta, "beta", torch.float32), float(eps), q.data_ptr(), M, _stream())
+    _check(rc, "sdetr_gemm_f16x3_add_layernorm")
+    return q
 
 
 def ffn_fused_layernorm(x, w1, b1, w2, b2, gamma=None, beta=None, eps: float = 1e-5, out=None):

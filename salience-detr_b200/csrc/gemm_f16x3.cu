@@ -103,6 +103,28 @@ extern "C" int sdetr_gemm_f16x3_ex(const float *A, int64_t lda, const float *a_s
     return launch_gemm3x<true, false, true>(A, lda, mh, ml, p, stream, "gemm_f16x3_ex");
 }
 
+// The encoder's class-score head reduced in its epilogue: out[row] = max_c (A . W^T * 2^-(4+s) + bias)[row, c] * row_scale[row],
+// bit for bit what sdetr_gemm_f16x3_pre followed by sdetr_class_max_times_fg gives, without writing the M x N logits.
+extern "C" int sdetr_gemm_f16x3_rowmax(const float *A, int64_t lda, const void *W_hi, const void *W_lo, float w_scale,
+                                       const float *bias, const float *row_scale, float *out, int M, int N, int K,
+                                       sdetr_stream_t stream) {
+    SDETR_REQUIRE(A && W_hi && W_lo && row_scale && out, SDETR_ERR_INVALID_ARG, "gemm_f16x3_rowmax: null pointer");
+    SDETR_REQUIRE(M >= 0 && N > 0 && N <= kGN && K > 0, SDETR_ERR_INVALID_ARG, "gemm_f16x3_rowmax: bad sizes (N <= %d)", kGN);
+    SDETR_REQUIRE(K % Gemm3xShape<true>::kK == 0, SDETR_ERR_UNSUPPORTED, "gemm_f16x3_rowmax: K=%d must be a multiple of %d", K,
+                  Gemm3xShape<true>::kK);
+    SDETR_REQUIRE(w_scale > 0.f, SDETR_ERR_INVALID_ARG, "gemm_f16x3_rowmax: weight scale must be positive");
+    SDETR_REQUIRE(lda % 4 == 0 && aligned16(A) && aligned16(W_hi) && aligned16(W_lo) && lda >= K, SDETR_ERR_INVALID_ARG,
+                  "gemm_f16x3_rowmax: operands must be 16-byte aligned with 16-byte row pitch");
+    if (M == 0) return SDETR_OK;
+    CUtensorMap mh, ml;
+    SDETR_REQUIRE(make_map_2d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_hi, N, K, K, 64, kGN) &&
+                      make_map_2d(&ml, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W_lo, N, K, K, 64, kGN),
+                  SDETR_ERR_CUDA, "gemm_f16x3_rowmax: cuTensorMapEncodeTiled failed");
+    Gemm3xParams p{bias, out, 1, M, N, K, 0, kActScale, 1.f / (kActScale * w_scale), nullptr, nullptr};
+    p.row_scale = row_scale;
+    return launch_gemm3x<true, false, false, true>(A, lda, mh, ml, p, stream, "gemm_f16x3_rowmax");
+}
+
 namespace sdetr {
 __global__ void split_f16_pair_dev_kernel(const float *__restrict__ w, int64_t n, const float *__restrict__ scale_dev,
                                           __half *__restrict__ hi, __half *__restrict__ lo) {

@@ -201,6 +201,7 @@ struct Gemm3xParams {
     const float *col_scale;    // EX only: per-column scale s (N) or NULL
     const float *Z;            // EX only: residual z (M rows, pitch ldz) or NULL; may alias C
     int64_t ldz;
+    const float *row_scale;    // ROWMAX only: s (M); C[row] = max over the N columns of (acc * out_scale + bias), times s[row]
 };
 
 // Consumer side of one k-block, first half: wait until stage `st` has landed (SPLIT_W: split its raw W in place, both
@@ -267,13 +268,64 @@ __device__ __forceinline__ void gemm3x_issue(float (&d)[64], const uint32_t (&ah
     wgmma_commit();
 }
 
+// ROWMAX epilogue of a tile that holds all N <= 128 columns: C[row] = max_c (acc * out_scale + bias[c]) * row_scale[row], the
+// column values computed as the plain epilogue computes them and their max taken in class_max_kernel's order (tokens.cu):
+// lane l of a row's warp there folds columns l, l + 32, l + 64, l + 96 from -inf, then the xor-16/8/4/2/1 butterfly, each
+// step fmax_nan(own, partner) and lane 0's result kept.  Column l = 8a + 2q + e (a < 4, e < 2) sits in this thread's
+// acc[4 (a + 4k) + 2h + e], so the lane partials of a = 0..3 are this thread's; the steps 16 and 8 combine them in registers,
+// 4 and 2 are quad shuffles and 1 is the last register step.
+__device__ __forceinline__ void gemm3x_rowmax_epilogue(const Gemm3xParams &p, const float (&acc)[64], int m0, int r0, int q,
+                                                       float out_scale) {
+    float b[16][2];
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * q + e;
+            b[j][e] = p.bias && col < p.N ? __ldg(p.bias + col) : 0.f;
+        }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float v[4][2];  // lane partials of lanes 8a + 2q + e
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float m = -INFINITY;
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    if (8 * (a + 4 * k) + 2 * q + e < p.N)
+                        m = fmax_nan(m, __fmaf_rn(acc[4 * (a + 4 * k) + 2 * h + e], out_scale, b[a + 4 * k][e]));
+                v[a][e] = m;
+            }
+        float w[4][2];
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) w[a][e] = fmax_nan(v[a][e], v[a ^ 2][e]);  // xor 16
+        float x[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            x[e] = fmax_nan(w[0][e], w[1][e]);                                        // xor 8 (lanes 2q + e remain)
+            x[e] = fmax_nan(x[e], __shfl_xor_sync(0xffffffffu, x[e], 2));            // xor 4
+            x[e] = fmax_nan(x[e], __shfl_xor_sync(0xffffffffu, x[e], 1));            // xor 2
+        }
+        const int row = m0 + r0 + 8 * h;
+        if (q == 0 && row < p.M) p.C[row] = fmax_nan(x[0], x[1]) * __ldg(p.row_scale + row);  // xor 1, lane 0
+    }
+}
+
 // Epilogue of tile t: C = acc * out_scale + bias (EX: C = z + s * (acc * out_scale + bias), s and z optional; each thread
-// reads its z elements before it writes the same C elements, so z may alias C).  acc[4j + {0,1}] = (row r0, cols
-// 8j + 2q + {0,1}), acc[4j + {2,3}] = (row r0 + 8, same cols).
-template <bool EX>
+// reads its z elements before it writes the same C elements, so z may alias C; ROWMAX: gemm3x_rowmax_epilogue).
+// acc[4j + {0,1}] = (row r0, cols 8j + 2q + {0,1}), acc[4j + {2,3}] = (row r0 + 8, same cols).
+template <bool EX, bool ROWMAX>
 __device__ __forceinline__ void gemm3x_epilogue(const Gemm3xParams &p, const float (&acc)[64], int t, int n_tiles, int r0, int q,
                                                 float out_scale) {
     const int m0 = (t / n_tiles) * kGM, n0 = (t % n_tiles) * kGN;
+    if (ROWMAX) {
+        gemm3x_rowmax_epilogue(p, acc, m0, r0, q, out_scale);
+        return;
+    }
     const bool pair = (p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -317,7 +369,7 @@ __device__ __forceinline__ void wgmma_hold(const uint32_t (&a)[4][4], bool never
 }
 
 // The consumer loop of gemm3x_kernel, with the input activation fixed at compile time.
-template <bool F16, bool SPLIT_W, bool EX, int ACT>
+template <bool F16, bool SPLIT_W, bool EX, bool ROWMAX, int ACT>
 __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *smem, uint64_t *full, uint64_t *empty, int tiles,
                                                int n_tiles, int kblocks, int r0, int q, int lane, float a_scale, float out_scale) {
     using S = Gemm3xShape<F16>;
@@ -342,7 +394,7 @@ __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *s
         const int nt = last ? t + (int)gridDim.x : t;
         const bool more = nt < tiles;
         if (kb == 0 && t != (int)blockIdx.x) {
-            gemm3x_epilogue<EX>(p, acc, t - (int)gridDim.x, n_tiles, r0, q, out_scale);
+            gemm3x_epilogue<EX, ROWMAX>(p, acc, t - (int)gridDim.x, n_tiles, r0, q, out_scale);
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;  // not acc = d below: 0.f + d turns a -0 product into +0
         }
@@ -360,13 +412,14 @@ __device__ __forceinline__ void gemm3x_consume(const Gemm3xParams &p, uint8_t *s
 #pragma unroll
             for (int j = 0; j < 4; ++j) ahi[kk][j] = nhi[kk][j], alo[kk][j] = nlo[kk][j];
     }
-    gemm3x_epilogue<EX>(p, acc, t, n_tiles, r0, q, out_scale);
+    gemm3x_epilogue<EX, ROWMAX>(p, acc, t, n_tiles, r0, q, out_scale);
 }
 
 // F16: fp16 pieces (W given as a pre-scaled fp16 pair).  !F16: TF32 pieces; SPLIT_W: W arrives raw (fp32) in the W_hi slot
 // and the consumer warpgroups split it in place into W_hi / W_lo with the arithmetic of sdetr_split_tf32_pair.  EX: the
 // epilogue also applies the per-column scale and the residual of Gemm3xParams (instances without it compile as before).
-template <bool F16, bool SPLIT_W, bool EX = false>
+// ROWMAX: one n-tile (N <= 128), and the epilogue writes one value per row (gemm3x_rowmax_epilogue) instead of the tile.
+template <bool F16, bool SPLIT_W, bool EX = false, bool ROWMAX = false>
 __global__ void __launch_bounds__(kGThreads, 1)
     gemm3x_kernel(const __grid_constant__ CUtensorMap ma, const __grid_constant__ CUtensorMap mh,
                   const __grid_constant__ CUtensorMap ml, const Gemm3xParams p) {
@@ -415,9 +468,9 @@ __global__ void __launch_bounds__(kGThreads, 1)
         out_scale = p.a_scale_dev ? 1.f / (a_scale * __ldg(p.w_scale_dev)) : p.out_scale;
     }
     switch (p.act) {  // one copy of the loop per activation keeps its test out of the per-element split
-        case 1: gemm3x_consume<F16, SPLIT_W, EX, 1>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
-        case 2: gemm3x_consume<F16, SPLIT_W, EX, 2>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
-        default: gemm3x_consume<F16, SPLIT_W, EX, 0>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale);
+        case 1: gemm3x_consume<F16, SPLIT_W, EX, ROWMAX, 1>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        case 2: gemm3x_consume<F16, SPLIT_W, EX, ROWMAX, 2>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale); break;
+        default: gemm3x_consume<F16, SPLIT_W, EX, ROWMAX, 0>(p, smem, full, empty, tiles, n_tiles, kblocks, r0, q, lane, a_scale, out_scale);
     }
 }
 
@@ -453,7 +506,7 @@ inline bool make_map_2d(CUtensorMap *m, CUtensorMapDataType dt, int elem_bytes, 
 }
 
 // A (M,K) fp32 with row pitch lda; W maps made by the caller (F16: fp16 boxes of 64 x 128, else fp32 boxes of 32 x 128)
-template <bool F16, bool SPLIT_W, bool EX = false>
+template <bool F16, bool SPLIT_W, bool EX = false, bool ROWMAX = false>
 inline int launch_gemm3x(const float *A, int64_t lda, const CUtensorMap &mh, const CUtensorMap &ml, const Gemm3xParams &p,
                          sdetr_stream_t stream, const char *what) {
     using S = Gemm3xShape<F16>;
@@ -461,9 +514,9 @@ inline int launch_gemm3x(const float *A, int64_t lda, const CUtensorMap &mh, con
     SDETR_REQUIRE(make_map_2d(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, A, p.M, p.K, lda, 32, kGM), SDETR_ERR_CUDA,
                   "%s: cuTensorMapEncodeTiled failed", what);
     static PerDeviceOnce once;
-    SDETR_OPT_IN_SMEM(once, (gemm3x_kernel<F16, SPLIT_W, EX>), S::kSmem, what);
+    SDETR_OPT_IN_SMEM(once, (gemm3x_kernel<F16, SPLIT_W, EX, ROWMAX>), S::kSmem, what);
     const int tiles = ((p.N + kGN - 1) / kGN) * ((p.M + kGM - 1) / kGM), ctas = persistent_ctas();
-    gemm3x_kernel<F16, SPLIT_W, EX><<<tiles < ctas ? tiles : ctas, kGThreads, S::kSmem, (cudaStream_t)stream>>>(ma, mh, ml, p);
+    gemm3x_kernel<F16, SPLIT_W, EX, ROWMAX><<<tiles < ctas ? tiles : ctas, kGThreads, S::kSmem, (cudaStream_t)stream>>>(ma, mh, ml, p);
     return check_launch(what);
 }
 

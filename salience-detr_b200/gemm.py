@@ -89,6 +89,15 @@ def _rows(x: Tensor) -> Tensor:
     return x2.clone(memory_format=torch.contiguous_format)
 
 
+def f16x3_route(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None) -> bool:
+    """True when ``linear(x, weight, bias)`` (no input activation) runs ``sdetr_gemm_f16x3_pre``.  The kernels that fuse a
+    consumer into that GEMM's epilogue (``cabi.gemm_f16x3_rowmax``, ``cabi.gemm_f16x3_add_layernorm_``) reproduce its product
+    bit for bit, so callers take them exactly where ``linear`` would have taken this route."""
+    k = weight.shape[-1]
+    return (MODE == "auto" and OWN_KERNEL == "f16x3" and k % 64 == 0 and not (k >= 1024 and LONG_K_PRESPLIT) and
+            x.numel() // max(k, 1) > SMALL_M and _native(x, weight, bias))
+
+
 def linear(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, relu_input: bool = False,
            input_act: Optional[str] = None) -> Tensor:
     """y = act(x) @ weight.T + bias (act: None | "relu" | "gelu", fused into the operand load / split), inference only.

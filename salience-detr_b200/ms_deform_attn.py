@@ -140,13 +140,20 @@ class MultiScaleDeformableAttention(nn.Module):
                           value_token_stride: int, value_offset: int, num_value: int, spatial_shapes: Tensor,
                           level_start_index: Tensor, query_order: Optional[Tensor] = None, schedule: int = 0) -> Tensor:
         """Inference path with an already projected (and masked) value buffer; 2-d reference points."""
+        out = self.sample_projected(query, reference_points, value_buf, value_batch_stride, value_token_stride, value_offset,
+                                    num_value, spatial_shapes, level_start_index, query_order, schedule)
+        return gemm.linear(out, self.output_proj.weight, self.output_proj.bias)
+
+    def sample_projected(self, query: Tensor, reference_points: Tensor, value_buf: Tensor, value_batch_stride: int,
+                         value_token_stride: int, value_offset: int, num_value: int, spatial_shapes: Tensor,
+                         level_start_index: Tensor, query_order: Optional[Tensor] = None, schedule: int = 0) -> Tensor:
+        """``forward_projected`` without the output projection: the sampled (b,Nq,C) rows it is applied to."""
         w, b = self.fused_projection()
         proj = gemm.linear(query, w, b)
-        out = cabi.msda_fused_forward(value_buf, value_batch_stride, value_token_stride, value_offset, spatial_shapes,
-                                      level_start_index, reference_points, proj, self.num_heads,
-                                      self.embed_dim // self.num_heads, self.num_levels, self.num_points, num_value,
-                                      query_order, schedule)
-        return gemm.linear(out, self.output_proj.weight, self.output_proj.bias)
+        return cabi.msda_fused_forward(value_buf, value_batch_stride, value_token_stride, value_offset, spatial_shapes,
+                                       level_start_index, reference_points, proj, self.num_heads,
+                                       self.embed_dim // self.num_heads, self.num_levels, self.num_points, num_value,
+                                       query_order, schedule)
 
     def forward(self, query: Tensor, reference_points: Tensor, value: Tensor, spatial_shapes: Tensor,
                 level_start_index: Tensor, key_padding_mask: Tensor) -> Tensor:

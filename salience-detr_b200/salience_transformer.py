@@ -235,9 +235,16 @@ class SalienceTransformerEncoderLayer(nn.Module):
                      level_start_index, order=None, qs=None):
         """``qs``: optional q + qp buffer (from the gather); the fused pre-attention keeps its rewritten rows current."""
         q, qs, top = self._pre_attention_fast(q, qp, mc, qs)
-        a = self.self_attn.forward_projected(qs if qs is not None else q + qp, ref_q, vbuf, v_bstride, v_tstride, v_off, num_value, spatial_shapes,
-                                             level_start_index, order, MSDA_SCHEDULE)
-        q = cabi.add_layernorm(q, a, self.norm1.weight, self.norm1.bias, self.norm1.eps, out=q)
+        s = self.self_attn.sample_projected(qs if qs is not None else q + qp, ref_q, vbuf, v_bstride, v_tstride, v_off, num_value,
+                                            spatial_shapes, level_start_index, order, MSDA_SCHEDULE)
+        op = self.self_attn.output_proj
+        if self.embed_dim == 256 and q.is_contiguous() and gemm.f16x3_route(s, op.weight, op.bias):
+            # output projection, residual and norm1 in one launch, bit for bit the two below
+            w_hi, w_lo, w_scale = gemm.split_weight_f16(op.weight)
+            cabi.gemm_f16x3_add_layernorm_(q, gemm._rows(s), w_hi, w_lo, w_scale, op.bias, self.norm1.weight, self.norm1.bias,
+                                           self.norm1.eps)
+        else:
+            q = cabi.add_layernorm(q, gemm.linear(s, op.weight, op.bias), self.norm1.weight, self.norm1.bias, self.norm1.eps, out=q)
         rows = q.shape[0] * q.shape[1]
         relu = isinstance(self.activation, nn.ReLU)
         if (relu and self.embed_dim == 256 and self.linear1.out_features % 128 == 0 and gemm.MODE == "auto" and
@@ -325,7 +332,12 @@ class SalienceTransformerEncoder(nn.Module):
             inds = foreground_inds[j]
             nq = inds.shape[1]
             q, qp, fq, rq, qs = cabi.token_gather(out, pos, fg, vr, inds, spatial_shapes, level_start_index, nq, want_sum=True)
-            mc = cabi.class_max_times_fg(gemm.linear(q, self.enhance_mcsp.weight, self.enhance_mcsp.bias), fq)
+            w, bw = self.enhance_mcsp.weight, self.enhance_mcsp.bias
+            if w.shape[0] <= 128 and gemm.f16x3_route(q, w, bw):  # class scores and their row max in one launch, bit for bit
+                w_hi, w_lo, w_scale = gemm.split_weight_f16(w)
+                mc = cabi.gemm_f16x3_rowmax(gemm._rows(q), w_hi, w_lo, w_scale, bw, fq).view(fq.shape)
+            else:
+                mc = cabi.class_max_times_fg(gemm.linear(q, w, bw), fq)
             q = layer.forward_fast(q, qp, mc, rq, vbuf, nv * wide, wide, j * c, nv, spatial_shapes,
                                    level_start_index, None if query_orders is None else query_orders[j], qs=qs)
             cabi.token_scatter_(out, q, inds, focus)

@@ -729,6 +729,43 @@ int sdetr_patch_merge_layernorm_tokens(const float *x, int batch, int H, int W, 
  * in fp32; a NaN in a row gives a NaN row.  Operands 16-byte aligned, y must not alias x.  One launch. */
 int sdetr_layernorm_tokens(const float *x, int64_t rows, int C, const float *ln_weight, const float *ln_bias, float eps, float *y,
                            sdetr_stream_t stream);
+/* ---- FocalNet backbone in token layout (models/backbones/focalnet.py; FocalNetBackbone.forward_tokens) ---------------------
+ * Token rows (batch, H * W, C) in raster order, C % 64 == 0 and C <= 1536.  The Linears of a block (f, h, proj, fc1, fc2) run on
+ * sdetr_gemm_f16x3_ex, a downsample's 3x3 / stride-2 convolution on sdetr_conv2d_f16x3, its LayerNorm and the output norms on
+ * sdetr_layernorm_tokens.  GELU is the exact one.
+ * The stem: y = LayerNorm(conv(x, W) + bias), conv 7x7, stride 4, padding 2, 3 -> C, on the image zero-padded on the right and
+ * bottom to a multiple of 4 (PatchEmbed): y (batch, ceil(H / 4) * ceil(W / 4), C), every tap outside the image a zero.  x: (batch,
+ * 3, H, W) NCHW contiguous fp32; weight (147, C) = W[co, c, ky, kx] at row (c * 7 + ky) * 7 + kx, column co.  fp32 FMAs, taps in
+ * (c, ky, kx) order, then the bias (sdetr_convnext_stem's body).  Two-pass LayerNorm per row.  One launch. */
+int sdetr_focalnet_stem(const float *x, int batch, int H, int W, int C, const float *weight, const float *bias,
+                        const float *ln_weight, const float *ln_bias, float eps, float *y, sdetr_stream_t stream);
+/* The floats of the partial channel sums that the last focal level writes and sdetr_focal_global_context reads: batch times
+ * the row tiles of an H x W map (at most 128) times C. */
+int64_t sdetr_focal_context_workspace_floats(int batch, int H, int W, int C);
+/* One focal level of FocalModulation: p = GELU(dwconv_k(ctx)), depthwise k x k, padding k / 2 (zeros), no bias, weight (k * k, C)
+ * = W[c, 0, ky, kx] at row ky * k + kx, k in {3, 5, 7, 9}; then ctx_all = ctx_all + p * gate per pixel (first: 0 + p * gate),
+ * the product and the sum rounded on their own, as the reference's chain.  ctx and gate: pixel r of image n at (n H W + r) *
+ * ld_ctx (ld_gate), e.g. column slices of f's output; ctx 8-byte aligned, ld_ctx even.  out (batch, H * W, C) receives p, or NULL;
+ * ctx_all (batch, H * W, C) is read (unless first) and written.  partials (sdetr_focal_context_workspace_floats) or NULL: on the
+ * last level the per-tile channel sums of p for sdetr_focal_global_context, each in a fixed order.  out, ctx_all and ctx must not
+ * alias.  fp32 FMAs.  One launch. */
+int sdetr_focal_level_tokens(const float *ctx, int64_t ld_ctx, const float *gate, int64_t ld_gate, const float *weight, int ksize,
+                             int batch, int H, int W, int C, int first, float *out, float *ctx_all, float *partials,
+                             int64_t partials_floats, sdetr_stream_t stream);
+/* The global context of FocalModulation: m = GELU(mean over the image's H * W pixels of ctx_L), the partial sums of the last
+ * focal level reduced in a fixed order (repeated calls give the same bits; a NaN pixel poisons its image), then in place
+ * ctx_all = ctx_all + m * gate, divided by (focal_level + 1) when normalize is set, each operation rounded on its own.  gate:
+ * pixel r of image n at (n H W + r) * ld_gate.  One launch. */
+int sdetr_focal_global_context(const float *partials, int64_t partials_floats, const float *gate, int64_t ld_gate, int batch, int H,
+                               int W, int C, int focal_level, int normalize, float *ctx_all, sdetr_stream_t stream);
+/* y = q * h over rows x C (C % 4 == 0): q row r at r * ld_q (ld_q % 4 == 0), h and y contiguous; y may be h, not q.  Operands
+ * 16-byte aligned.  One launch. */
+int sdetr_focal_modulate(const float *q, int64_t ld_q, const float *h, int64_t rows, int C, float *y, sdetr_stream_t stream);
+/* The post-LN residual of a FocalModulationBlock: t = t + gamma * LayerNorm(y) in place, y and t contiguous rows of C, gamma (C),
+ * the LayerNorm of sdetr_layernorm_tokens, the product and the sum rounded on their own.  t must not alias y; operands 16-byte
+ * aligned.  One launch. */
+int sdetr_layernorm_scale_add_tokens(const float *y, int64_t rows, int C, const float *ln_weight, const float *ln_bias, float eps,
+                                     const float *gamma, float *t, sdetr_stream_t stream);
 #ifdef __cplusplus
 }
 #endif

@@ -41,6 +41,7 @@ from .channel_mapper import ChannelMapper, level_views, tokens_of  # noqa: F401
 from .backbone import FrozenBatchNorm2d, ResNetBackbone  # noqa: F401
 from .convnext import ConvNeXtBackbone  # noqa: F401
 from .swin import SwinTransformerBackbone  # noqa: F401
+from .focalnet import FocalNetBackbone  # noqa: F401
 from .salience_transformer import (  # noqa: F401
     EncoderPlan,
     MaskPredictor,

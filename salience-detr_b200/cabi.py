@@ -118,6 +118,12 @@ SIGNATURES = {
     "sdetr_window_attention_tokens": (_i, [_vp, _vp, _vp] + [_i] * 9 + [_vp, _vp]),
     "sdetr_patch_merge_layernorm_tokens": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _vp, _vp]),
     "sdetr_layernorm_tokens": (_i, [_vp, _i64, _i, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_focalnet_stem": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    "sdetr_focal_context_workspace_floats": (_i64, [_i, _i, _i, _i]),
+    "sdetr_focal_level_tokens": (_i, [_vp, _i64, _vp, _i64, _vp] + [_i] * 6 + [_vp, _vp, _vp, _i64, _vp]),
+    "sdetr_focal_global_context": (_i, [_vp, _i64, _vp, _i64] + [_i] * 6 + [_vp, _vp]),
+    "sdetr_focal_modulate": (_i, [_vp, _i64, _vp, _i64, _i, _vp, _vp]),
+    "sdetr_layernorm_scale_add_tokens": (_i, [_vp, _i64, _i, _vp, _vp, _f, _vp, _vp, _vp]),
 }
 
 
@@ -1508,3 +1514,108 @@ def layernorm_tokens(x, ln_weight, ln_bias, eps: float = 1e-5):
                                       float(eps), y.data_ptr(), _stream())
     _check(rc, "sdetr_layernorm_tokens")
     return y
+
+
+# ---- FocalNet backbone in token layout (focalnet.FocalNetBackbone.forward_tokens) -------------------------------------------
+def focalnet_stem(x, weight, bias, ln_weight, ln_bias, eps: float = 1e-5):
+    """LayerNorm(conv 7x7 / 4, padding 2 (x) + bias) over C on the image zero-padded to a multiple of 4 -> (b, ceil(H / 4) *
+    ceil(W / 4), C) token rows.  x: (b, 3, H, W) NCHW contiguous fp32 CUDA; weight: (147, C) = W.reshape(C, 147).T, contiguous;
+    bias, ln_weight, ln_bias (C)."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.is_contiguous()):
+        raise RuntimeError("focalnet_stem: x must be a contiguous CUDA float32 (b, 3, H, W) tensor")
+    b, _, H, W = x.shape
+    C = weight.shape[1]
+    if weight.dim() != 2 or weight.shape[0] != 147 or any(tuple(t.shape) != (C,) for t in (bias, ln_weight, ln_bias)):
+        raise RuntimeError("focalnet_stem: weight must be (147, C) and bias, ln_weight, ln_bias (C)")
+    y = torch.empty(b, ((H + 3) // 4) * ((W + 3) // 4), C, device=x.device, dtype=torch.float32)
+    rc = lib().sdetr_focalnet_stem(_req(x, "x", torch.float32), b, H, W, C, _req(weight, "weight", torch.float32),
+                                   _req(bias, "bias", torch.float32), _req(ln_weight, "ln_weight", torch.float32),
+                                   _req(ln_bias, "ln_bias", torch.float32), float(eps), y.data_ptr(), _stream())
+    _check(rc, "sdetr_focalnet_stem")
+    return y
+
+
+def focal_context_partials(b: int, hw, C: int, device):
+    """the workspace of the last focal level's partial channel sums (focal_level_tokens / focal_global_context)"""
+    n = int(lib().sdetr_focal_context_workspace_floats(b, int(hw[0]), int(hw[1]), C))
+    return torch.empty(max(n, 4), device=device, dtype=torch.float32)
+
+
+def _rows_view(t, name, b, n, c):
+    """(pointer, row stride) of a (b, n, c) fp32 CUDA view whose rows are one stride apart (a column slice of a contiguous
+    tensor) with unit channel stride"""
+    if not (t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (b, n, c) and t.stride(2) == 1
+            and (b * n <= 1 or t.stride(0) == n * t.stride(1))):
+        raise RuntimeError(f"{name} must be a CUDA float32 ({b}, {n}, {c}) view with rows one stride apart and unit channel stride")
+    if t.device.index != _current_device():
+        raise RuntimeError(f"{name} lives on {t.device} but cuda:{_current_device()} is current")
+    return t.data_ptr(), (t.stride(1) if n > 1 else t.stride(0) if b > 1 else c)
+
+
+def focal_level_tokens(ctx, gate, hw, weight, ctx_all, first: bool, out=True, partials=None):
+    """One focal level: p = GELU(depthwise conv k x k, padding k // 2 (ctx)), ctx_all = (0 if first else ctx_all) + p * gate.
+    ctx: (b, H*W, C) view with rows one stride apart (e.g. a column slice of f's output); gate: (b, H*W, 1) view likewise;
+    weight: (k * k, C) = W.reshape(C, k * k).T, contiguous; ctx_all: contiguous (b, H*W, C), updated in place.  out: True (a new
+    tensor receives p, returned), or False (p not written, None returned); partials: None, or on the last level the workspace
+    of focal_context_partials, which receives its per-tile channel sums."""
+    b, n, C = ctx.shape
+    H, W = hw
+    if n != H * W:
+        raise RuntimeError(f"focal_level_tokens: ctx has {n} rows per image, the map is {H}x{W}")
+    kk = weight.shape[0]
+    k = int(round(kk ** 0.5))
+    if weight.dim() != 2 or k * k != kk or weight.shape[1] != C:
+        raise RuntimeError(f"focal_level_tokens: weight must be (k * k, {C})")
+    cp, ldc = _rows_view(ctx, "ctx", b, n, C)
+    gp, ldg = _rows_view(gate, "gate", b, n, 1)
+    if not (ctx_all.is_cuda and tuple(ctx_all.shape) == (b, n, C) and ctx_all.is_contiguous()):
+        raise RuntimeError(f"focal_level_tokens: ctx_all must be a contiguous ({b}, {n}, {C}) tensor")
+    y = torch.empty(b, n, C, device=ctx.device, dtype=torch.float32) if out else None
+    rc = lib().sdetr_focal_level_tokens(cp, ldc, gp, ldg, _req(weight, "weight", torch.float32), k, b, int(H), int(W), C,
+                                        int(bool(first)), y.data_ptr() if y is not None else None,
+                                        _req(ctx_all, "ctx_all", torch.float32),
+                                        _req(partials, "partials", torch.float32) if partials is not None else None,
+                                        partials.numel() if partials is not None else 0, _stream())
+    _check(rc, "sdetr_focal_level_tokens")
+    return y
+
+
+def focal_global_context(partials, gate, hw, ctx_all, focal_level: int, normalize: bool):
+    """ctx_all = (ctx_all + GELU(mean over each image's pixels of ctx_L) * gate) [/ (focal_level + 1)] in place, the mean from the
+    last focal level's partials.  gate: (b, H*W, 1) view with rows one stride apart."""
+    b, n, C = ctx_all.shape
+    H, W = hw
+    if n != H * W or not ctx_all.is_contiguous():
+        raise RuntimeError(f"focal_global_context: ctx_all must be a contiguous (b, {H * W}, C) tensor")
+    gp, ldg = _rows_view(gate, "gate", b, n, 1)
+    rc = lib().sdetr_focal_global_context(_req(partials, "partials", torch.float32), partials.numel(), gp, ldg, b, int(H), int(W), C,
+                                          int(focal_level), int(bool(normalize)), _req(ctx_all, "ctx_all", torch.float32), _stream())
+    _check(rc, "sdetr_focal_global_context")
+    return ctx_all
+
+
+def focal_modulate(q, h, out=None):
+    """out = q * h: q (b, n, C) view with rows one stride apart (f's output's first C columns), h contiguous (b, n, C); out
+    None (a new tensor) or a contiguous (b, n, C) tensor, which may be h."""
+    b, n, C = h.shape
+    qp, ldq = _rows_view(q, "q", b, n, C)
+    y = out if out is not None else torch.empty_like(h)
+    if tuple(y.shape) != (b, n, C) or not y.is_contiguous():
+        raise RuntimeError(f"focal_modulate: out must be a contiguous ({b}, {n}, {C}) tensor")
+    rc = lib().sdetr_focal_modulate(qp, ldq, _req(h, "h", torch.float32), b * n, C, y.data_ptr(), _stream())
+    _check(rc, "sdetr_focal_modulate")
+    return y
+
+
+def layernorm_scale_add_tokens_(t, y, ln_weight, ln_bias, gamma, eps: float = 1e-5):
+    """t = t + gamma * LayerNorm(y) over the last dimension C (a multiple of 64 up to 1536), in place; t and y contiguous of the
+    same shape; returns t"""
+    C = y.shape[-1]
+    if tuple(t.shape) != tuple(y.shape) or any(tuple(v.shape) != (C,) for v in (ln_weight, ln_bias, gamma)):
+        raise RuntimeError(f"layernorm_scale_add_tokens_: t must have y's shape and ln_weight, ln_bias, gamma ({C},)")
+    rc = lib().sdetr_layernorm_scale_add_tokens(_req(y, "y", torch.float32), y.numel() // C if C else 0, C,
+                                                _req(ln_weight, "ln_weight", torch.float32), _req(ln_bias, "ln_bias", torch.float32),
+                                                float(eps), _req(gamma, "gamma", torch.float32), _req(t, "t", torch.float32),
+                                                _stream())
+    _check(rc, "sdetr_layernorm_scale_add_tokens")
+    return t

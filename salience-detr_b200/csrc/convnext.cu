@@ -2,7 +2,8 @@
 // Linears of every CNBlock and every 2x2 / stride-2 downsampling convolution run on sdetr_gemm_f16x3_ex (gemm_f16x3.cu).
 //
 //   sdetr_convnext_stem                conv 4x4, stride 4, 3 -> C channels with bias, then LayerNorm over C (affine), from the
-//                                      NCHW fp32 image batch to (b, Ho*Wo, C) token rows.  fp32 FMAs, taps in (c, ky, kx) order.
+//                                      NCHW fp32 image batch to (b, Ho*Wo, C) token rows.  fp32 FMAs, taps in (c, ky, kx) order
+//                                      (patch_stem_kernel<4, 0> of patch_stem.cuh).
 //   sdetr_dwconv7x7_layernorm_tokens   depthwise conv 7x7, padding 3, with bias, then LayerNorm over C (affine), token rows in,
 //                                      token rows out (a separate buffer: the block input stays the residual).
 //   sdetr_layernorm_tokens_s2d         LayerNorm over C of token rows, written space-to-depth: output row (y, x) of the
@@ -14,46 +15,12 @@
 
 #include "common.cuh"
 #include "layernorm_rows.cuh"
+#include "patch_stem.cuh"
 
 namespace sdetr {
 
-constexpr int kCnMaxJ = 24;     // C <= 64 * 24 = 1536
-constexpr int kCnWarps = 8;     // token rows per CTA of 256 threads
-
-__global__ void __launch_bounds__(32 * kCnWarps) convnext_stem_kernel(const float *__restrict__ x, int batch, int H, int W, int Ho,
-                                                                       int Wo, int C, const float *__restrict__ w /* (48, C) */,
-                                                                       const float *__restrict__ bias, const float *__restrict__ g,
-                                                                       const float *__restrict__ beta, float eps,
-                                                                       float *__restrict__ y) {
-    const int lane = threadIdx.x & 31, nj = C >> 6;
-    const int64_t tok = (int64_t)blockIdx.x * kCnWarps + (threadIdx.x >> 5), hw = (int64_t)Ho * Wo;
-    if (tok >= batch * hw) return;
-    const int n = (int)(tok / hw), pix = (int)(tok - n * hw), oy = pix / Wo, ox = pix - oy * Wo;
-    float2 v[kCnMaxJ];
-#pragma unroll
-    for (int j = 0; j < kCnMaxJ; ++j) v[j] = make_float2(0.f, 0.f);
-    const float *xn = x + (int64_t)n * 3 * H * W + (int64_t)(4 * oy) * W + 4 * ox;
-    for (int c = 0; c < 3; ++c)
-        for (int ky = 0; ky < 4; ++ky)
-#pragma unroll
-            for (int kx = 0; kx < 4; ++kx) {
-                const float xv = __ldg(xn + ((int64_t)c * H + ky) * W + kx);  // one address per warp: a broadcast
-                const float *wr = w + (int64_t)((c * 4 + ky) * 4 + kx) * C + 2 * lane;
-#pragma unroll
-                for (int j = 0; j < kCnMaxJ; ++j)
-                    if (j < nj) {
-                        const float2 wv = __ldg(reinterpret_cast<const float2 *>(wr + 64 * j));
-                        v[j].x = fmaf(xv, wv.x, v[j].x), v[j].y = fmaf(xv, wv.y, v[j].y);
-                    }
-            }
-#pragma unroll
-    for (int j = 0; j < kCnMaxJ; ++j)
-        if (j < nj) {
-            const float2 bv = __ldg(reinterpret_cast<const float2 *>(bias + 64 * j + 2 * lane));
-            v[j].x += bv.x, v[j].y += bv.y;
-        }
-    cn_layernorm_store(v, nj, C, lane, g, beta, eps, y + tok * C);
-}
+constexpr int kCnMaxJ = kStemMaxJ;     // C <= 64 * 24 = 1536
+constexpr int kCnWarps = kStemWarps;   // token rows per CTA of 256 threads
 
 __global__ void __launch_bounds__(32 * kCnWarps) dwconv7x7_layernorm_kernel(const float *__restrict__ x, int batch, int H, int W, int C,
                                                                              const float *__restrict__ w /* (49, C) */,
@@ -133,8 +100,8 @@ extern "C" int sdetr_convnext_stem(const float *x, int batch, int H, int W, int 
     const int64_t toks = (int64_t)batch * Ho * Wo;
     SDETR_REQUIRE((int64_t)batch * 3 * H * W < (1LL << 40) && toks < (1LL << 31), SDETR_ERR_INVALID_ARG, "convnext_stem: image too large");
     if (toks == 0) return SDETR_OK;
-    convnext_stem_kernel<<<cn_blocks(toks), 32 * kCnWarps, 0, (cudaStream_t)stream>>>(x, batch, H, W, Ho, Wo, C, weight, bias,
-                                                                                        ln_weight, ln_bias, eps, y);
+    patch_stem_kernel<4, 0><<<cn_blocks(toks), 32 * kCnWarps, 0, (cudaStream_t)stream>>>(x, batch, H, W, Ho, Wo, C, weight, bias,
+                                                                                           ln_weight, ln_bias, eps, y);
     return check_launch("convnext_stem");
 }
 

@@ -93,6 +93,28 @@ def swin_weights(state: Mapping[str, torch.Tensor], seed: int = 0) -> "OrderedDi
     return out
 
 
+def focalnet_weights(state: Mapping[str, torch.Tensor], seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded weights for a FocalNet state dict (in its order), swin_weights' rules -- Linear and convolution weights
+    N(0, 1 / fan_in), biases N(0, 0.1^2), LayerNorm weights 1 + U(-0.25, 0.25) -- with the layer scales gamma_1 / gamma_2
+    U(0.05, 1): at their 1e-4 initialisation every block is nearly the identity, which would hide an error in it."""
+    g = torch.Generator().manual_seed(seed)
+    out = OrderedDict()
+    for k, v in state.items():
+        shape = tuple(v.shape)
+        if k.endswith(("gamma_1", "gamma_2")):
+            t = 0.05 + torch.rand(shape, generator=g) * 0.95
+        elif len(shape) >= 2:
+            t = torch.randn(shape, generator=g) / math.sqrt(math.prod(shape[1:]))
+        elif k.endswith("bias"):
+            t = torch.randn(shape, generator=g) * 0.1
+        elif k.endswith("weight"):
+            t = 1.0 + (torch.rand(shape, generator=g) - 0.5) * 0.5
+        else:
+            raise ValueError(f"focalnet_weights: no rule for {k} {shape}")
+        out[k] = t
+    return out
+
+
 def level_shapes(h: int, w: int, strides: Sequence[int]) -> List[Tuple[int, int]]:
     out: List[Tuple[int, int]] = []
     for i, s in enumerate(strides):

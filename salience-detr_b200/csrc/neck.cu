@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(kGateThreads) gate_combine_kernel(const float 
         for (int c = lane; c < C; c += 32) s = fmaf(__ldg(w1 + (int64_t)j * C + c), ctx[c], s);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) hid[j] = fmaxf(s, 0.f);
+        if (lane == 0) hid[j] = relu_nan(s);  // torch's ReLU: a NaN context (a NaN anywhere in the image) stays NaN
     }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += kGateThreads) {

@@ -531,6 +531,21 @@ int64_t sdetr_group_norm_tokens_workspace_floats(int batch, int channels, int nu
 int sdetr_group_norm_tokens(const float *x, float *y, int64_t pitch, int batch, int channels, int num_levels,
                             const int32_t *level_size_host, const float *gamma, const float *beta, int num_groups, float eps,
                             float *workspace, int64_t workspace_floats, sdetr_stream_t stream);
+/* Training: the backward of sdetr_group_norm_tokens with the same level table and operand rules.  x is the forward's input:
+ * the (mean, rstd) of every (image, level, group) are recomputed by the forward's own kernels, so they are the forward's bits.
+ * With xhat = (x - mean) * rstd and g = gamma[l] * dy:  dx = rstd * (g - mean_grp(g) - xhat * mean_grp(g * xhat)),
+ * dgamma[l, c] = sum over images and the level's tokens of dy * xhat, dbeta[l, c] = sum of dy ((num_levels, C) row-major; either
+ * may be NULL, which skips its work; both NULL skip a launch).  Per-tile partials in a fixed order, then fixed trees: no
+ * atomics, the result depends only on the data.  dx may alias x or dy (each element is read, then written, by the same
+ * thread).  A NaN in dy or x makes its (image, level, group) of dx NaN, as torch's backward does.  Five launches, six with
+ * dgamma or dbeta; batch 0 writes nothing.  workspace: sdetr_group_norm_tokens_backward_workspace_floats(...) floats, 8-byte
+ * aligned. */
+int64_t sdetr_group_norm_tokens_backward_workspace_floats(int batch, int channels, int num_groups, int num_levels,
+                                                          const int32_t *level_size_host);
+int sdetr_group_norm_tokens_backward(const float *dy, const float *x, float *dx, int64_t pitch, int batch, int channels,
+                                     int num_levels, const int32_t *level_size_host, const float *gamma, int num_groups,
+                                     float eps, float *dgamma, float *dbeta, float *workspace, int64_t workspace_floats,
+                                     sdetr_stream_t stream);
 /* The transformer's front end for features that are already tokens (salience_transformer.py:107-113 without the flatten):
  * lpos = pos + level_embeds[l];  x = (feat + lpos) * keep[b,t]  -- the operations of sdetr_flatten_tokens[_pos] in the same
  * order, so lpos and x are bit-identical to theirs for the same values.  feat, pos, lpos, x (b,Nv,C) contiguous, 16-byte

@@ -94,6 +94,8 @@ SIGNATURES = {
     "sdetr_upsample_nearest_concat_backward": (_i, [_vp, _i64, _i64, _i, _i, _i, _i, _i, _i, _vp, _i64, _i64, _vp]),
     "sdetr_group_norm_tokens_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
     "sdetr_group_norm_tokens": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _i, _f, _vp, _i64, _vp]),
+    "sdetr_group_norm_tokens_backward_workspace_floats": (_i64, [_i, _i, _i, _i, _vp]),
+    "sdetr_group_norm_tokens_backward": (_i, [_vp, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp, _vp, _i64, _vp]),
     "sdetr_token_lpos_keep": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "sdetr_set_match_workspace_floats": (_i64, [_vp, _i]),
     "sdetr_set_match": (_i, [_vp, _i, _i, _f, _f, _f, _f, _f, _vp, _vp, _i64, _vp]),
@@ -1116,24 +1118,60 @@ def upsample_nearest_concat_backward(g_hi, lo_hw, hi_hw):
 
 
 # ---- ChannelMapper in token layout (channel_mapper.ChannelMapper.forward_tokens) ----------------------------------------------
-def group_norm_tokens_(tokens, level_sizes: Sequence[int], gamma, beta, num_groups: int, eps: float):
-    """nn.GroupNorm of every level of ``tokens`` (b, Nv, C) in place (three launches for all levels).  ``tokens`` may be a
-    token-range view of a larger buffer (unit channel stride, rows C apart); gamma / beta: (L, C) contiguous."""
+def _gn_rows(t, name, b, nv, c):
+    if not (t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (b, nv, c) and t.stride(2) == 1 and t.stride(1) == c):
+        raise RuntimeError(f"{name} must be CUDA float32 ({b}, {nv}, {c}) with contiguous rows")
+    if t.device.index != _current_device():
+        raise RuntimeError(f"{name} lives on {t.device} but cuda:{_current_device()} is current")
+    return t.stride(0) if b > 1 else nv * c
+
+
+def group_norm_tokens_(tokens, level_sizes: Sequence[int], gamma, beta, num_groups: int, eps: float, out=None):
+    """nn.GroupNorm of every level of ``tokens`` (b, Nv, C) in place, or into ``out`` (three launches for all levels).  ``tokens``
+    may be a token-range view of a larger buffer (unit channel stride, rows C apart); ``out``, when given, has its image pitch;
+    gamma / beta: (L, C) contiguous."""
     b, nv, c = tokens.shape
     L = len(level_sizes)
-    if not (tokens.is_cuda and tokens.dtype == torch.float32 and tokens.stride(2) == 1 and tokens.stride(1) == c):
-        raise RuntimeError("group_norm_tokens_: tokens must be CUDA float32 (b, Nv, C) with contiguous rows")
+    pitch = _gn_rows(tokens, "group_norm_tokens_: tokens", b, nv, c)
+    y = tokens if out is None else out
+    if out is not None and _gn_rows(out, "group_norm_tokens_: out", b, nv, c) != pitch:
+        raise RuntimeError("group_norm_tokens_: out must have the image pitch of tokens")
     if sum(level_sizes) != nv or tuple(gamma.shape) != (L, c) or tuple(beta.shape) != (L, c):
         raise RuntimeError(f"group_norm_tokens_: {nv} tokens, levels {list(level_sizes)}, gamma / beta must be ({L}, {c})")
     sizes = _host_i32(level_sizes)
     ws = torch.empty(max(int(lib().sdetr_group_norm_tokens_workspace_floats(b, c, int(num_groups), L, sizes)), 4),
                      device=tokens.device, dtype=torch.float32)
-    pitch = tokens.stride(0) if b > 1 else nv * c
-    rc = lib().sdetr_group_norm_tokens(tokens.data_ptr(), tokens.data_ptr(), pitch, b, c, L, sizes, _req(gamma, "gamma", torch.float32),
+    rc = lib().sdetr_group_norm_tokens(tokens.data_ptr(), y.data_ptr(), pitch, b, c, L, sizes, _req(gamma, "gamma", torch.float32),
                                        _req(beta, "beta", torch.float32), int(num_groups), float(eps), ws.data_ptr(), ws.numel(),
                                        _stream())
     _check(rc, "sdetr_group_norm_tokens")
-    return tokens
+    return y
+
+
+def group_norm_tokens_backward(dy, x, level_sizes: Sequence[int], gamma, num_groups: int, eps: float, dx=None,
+                               dgamma: bool = True, dbeta: bool = True):
+    """Gradient of group_norm_tokens_ -> (dx, dgamma, dbeta).  dy, x: (b, Nv, C) views with contiguous rows and one image pitch
+    (x the forward's input); gamma: (L, C) contiguous.  ``dx``: optional destination with that pitch, may be ``x`` or ``dy``
+    itself.  dgamma / dbeta: (L, C) tables when asked for, else None (and, with neither, one launch less)."""
+    b, nv, c = x.shape
+    L = len(level_sizes)
+    pitch = _gn_rows(x, "group_norm_tokens_backward: x", b, nv, c)
+    dx = dx if dx is not None else torch.empty(b, nv, c, device=x.device, dtype=torch.float32)
+    if _gn_rows(dy, "group_norm_tokens_backward: dy", b, nv, c) != pitch or _gn_rows(dx, "group_norm_tokens_backward: dx", b, nv, c) != pitch:
+        raise RuntimeError("group_norm_tokens_backward: dy, x and dx must have the same image pitch")
+    if sum(level_sizes) != nv or tuple(gamma.shape) != (L, c):
+        raise RuntimeError(f"group_norm_tokens_backward: {nv} tokens, levels {list(level_sizes)}, gamma must be ({L}, {c})")
+    dg = torch.empty(L, c, device=x.device, dtype=torch.float32) if dgamma else None
+    db = torch.empty(L, c, device=x.device, dtype=torch.float32) if dbeta else None
+    sizes = _host_i32(level_sizes)
+    ws = torch.empty(max(int(lib().sdetr_group_norm_tokens_backward_workspace_floats(b, c, int(num_groups), L, sizes)), 4),
+                     device=x.device, dtype=torch.float32)
+    rc = lib().sdetr_group_norm_tokens_backward(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), pitch, b, c, L, sizes,
+                                                _req(gamma, "gamma", torch.float32), int(num_groups), float(eps),
+                                                dg.data_ptr() if dg is not None else None, db.data_ptr() if db is not None else None,
+                                                ws.data_ptr(), ws.numel(), _stream())
+    _check(rc, "sdetr_group_norm_tokens_backward")
+    return dx, dg, db
 
 
 def token_lpos_keep(feat, pos, level_embeds, keep, level_sizes: Sequence[int], lpos=None):

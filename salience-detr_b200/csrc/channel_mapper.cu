@@ -6,6 +6,9 @@
 //                                of its rows (in the frame shifted by the tile's first row); (2) one CTA per (group, level, image) merges the tiles' and channels' partials
 //                                with Chan's formula in a fixed order and writes (mean, rstd); (3) the affine apply, same tiles
 //                                as (1).  No atomics: the result depends only on the data, never on the grid or launch order.
+//   sdetr_group_norm_tokens_backward  its gradient: the forward's (1) and (2) recompute the statistics, then (1') per-tile sums
+//                            of dy and dy * xhat, (2') one CTA per (group, level, image) forms the two group means, (3') per
+//                            (level, channel) dgamma / dbeta, (4') the element-wise dx.  Equally free of atomics.
 //   sdetr_token_lpos_keep    lpos = pos + level_embeds[l], x = (feat + lpos) * keep, on token rows: the same fp32 operations in
 //                            the same order as sdetr_flatten_tokens[_pos], so both outputs are bit-identical to theirs.
 #include <math.h>
@@ -147,6 +150,141 @@ __global__ void gn_apply_kernel(const float *x, float *y, int64_t pitch, int C, 
     }
 }
 
+// ---- backward: (dy, x) -> dx = rstd * (gamma dy - mean_grp(gamma dy) - xhat mean_grp(gamma dy xhat)), dgamma, dbeta ------------
+__device__ __forceinline__ float4 sm4(const float *p, int c) { return *reinterpret_cast<const float4 *>(p + c); }
+
+// (1) same tiles and threads as gn_partial_kernel: per channel, sum of dy and of dy * xhat over the tile's rows, each lane in row
+// order, the lanes in order.  pdy / pdyx: [b][tile][C]
+__global__ void gnb_partial_kernel(const float *__restrict__ dy, const float *__restrict__ x, int64_t pitch, int C, int G,
+                                   GnLevels lv, int total_tiles, const float2 *__restrict__ stats, float *__restrict__ pdy,
+                                   float *__restrict__ pdyx) {
+    extern __shared__ float gn_smem[];
+    const int C4 = C / 4, R = blockDim.x / C4;
+    const int j = threadIdx.x % C4, r = threadIdx.x / C4, c = 4 * j, cg = C / G;
+    const int tile = blockIdx.x, b = blockIdx.y;
+    const int l = gn_level_of_tile(lv, tile);
+    const int t0 = (tile - lv.tile0[l]) * kGnTile;
+    const int rows = min(kGnTile, lv.size[l] - t0);
+    const float2 *st = stats + ((int64_t)b * lv.L + l) * G;
+    const float2 s0 = st[(c + 0) / cg], s1 = st[(c + 1) / cg], s2 = st[(c + 2) / cg], s3 = st[(c + 3) / cg];
+    const int64_t base = (int64_t)b * pitch + (int64_t)(lv.start[l] + t0) * C + c;
+    float4 sd = make_float4(0.f, 0.f, 0.f, 0.f), sx = sd;
+    for (int t = r; t < rows; t += R) {
+        const int64_t o = base + (int64_t)t * C;
+        const float4 g = ld_stream_f4(dy + o), v = ld_stream_f4(x + o);
+        sd.x += g.x, sx.x = fmaf(g.x, (v.x - s0.x) * s0.y, sx.x);
+        sd.y += g.y, sx.y = fmaf(g.y, (v.y - s1.x) * s1.y, sx.y);
+        sd.z += g.z, sx.z = fmaf(g.z, (v.z - s2.x) * s2.y, sx.z);
+        sd.w += g.w, sx.w = fmaf(g.w, (v.w - s3.x) * s3.y, sx.w);
+    }
+    float *sm = gn_smem, *sq = gn_smem + R * C;  // [R][C] each
+    *reinterpret_cast<float4 *>(sm + r * C + c) = sd;
+    *reinterpret_cast<float4 *>(sq + r * C + c) = sx;
+    __syncthreads();
+    if (r != 0) return;
+    float4 a = sm4(sm, c), q = sm4(sq, c);
+    for (int u = 1; u < R; ++u) {
+        const float4 p = sm4(sm + u * C, c), w = sm4(sq + u * C, c);
+        a.x += p.x, a.y += p.y, a.z += p.z, a.w += p.w;
+        q.x += w.x, q.y += w.y, q.z += w.z, q.w += w.w;
+    }
+    const int64_t o = ((int64_t)b * total_tiles + tile) * C + c;
+    *reinterpret_cast<float4 *>(pdy + o) = a;
+    *reinterpret_cast<float4 *>(pdyx + o) = q;
+}
+
+// (2) one CTA per (group, level, image): the level's tiles x the group's channels, gamma applied per channel, each thread a
+// strided share in order, then a fixed tree.  coef[(b * L + l) * G + g] = (mean_grp(gamma dy), mean_grp(gamma dy xhat))
+__global__ void __launch_bounds__(kGnCombineThreads) gnb_combine_kernel(const float *__restrict__ pdy, const float *__restrict__ pdyx,
+                                                                        const float *__restrict__ gamma, int C, int G, GnLevels lv,
+                                                                        int total_tiles, float2 *__restrict__ coef) {
+    __shared__ float s1[kGnCombineThreads], s2[kGnCombineThreads];
+    const int g = blockIdx.x, l = blockIdx.y, b = blockIdx.z, cg = C / G;
+    int size = 0, tile0 = 0, ntiles = 0;  // lv.*[l] by selection, as in gn_combine_kernel
+#pragma unroll
+    for (int u = 0; u < kMaxLevels; ++u)
+        if (u == l) size = lv.size[u], tile0 = lv.tile0[u], ntiles = lv.tile0[u + 1] - lv.tile0[u];
+    const int64_t items = (int64_t)ntiles * cg;
+    const float *pd = pdy + ((int64_t)b * total_tiles + tile0) * C, *px = pdyx + ((int64_t)b * total_tiles + tile0) * C;
+    const float *ga = gamma + (int64_t)l * C;
+    float a1 = 0.f, a2 = 0.f;
+    for (int64_t k = threadIdx.x; k < items; k += kGnCombineThreads) {
+        const int tl = (int)(k / cg), c = g * cg + (int)(k % cg);
+        const float gc = __ldg(ga + c);
+        a1 = fmaf(gc, __ldg(pd + (int64_t)tl * C + c), a1);
+        a2 = fmaf(gc, __ldg(px + (int64_t)tl * C + c), a2);
+    }
+    s1[threadIdx.x] = a1, s2[threadIdx.x] = a2;
+    __syncthreads();
+    for (int s = kGnCombineThreads / 2; s > 0; s >>= 1) {
+        if ((int)threadIdx.x < s) s1[threadIdx.x] += s1[threadIdx.x + s], s2[threadIdx.x] += s2[threadIdx.x + s];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const float inv_n = 1.f / ((float)size * (float)cg);
+        coef[((int64_t)b * lv.L + l) * G + g] = make_float2(s1[0] * inv_n, s2[0] * inv_n);
+    }
+}
+
+constexpr int kGnParamLanes = 8;  // gnb_param_kernel: CTA (32 channels, kGnParamLanes lanes)
+
+// (3) one CTA per (32 channels, level): dgamma[l, c] = sum of pdyx, dbeta[l, c] = sum of pdy over the level's (image, tile)
+// partials; lane u of a channel sums the partials u, u + kGnParamLanes, ... in (image, tile) order, the lanes in order.  Either
+// output may be NULL.
+__global__ void __launch_bounds__(32 * kGnParamLanes) gnb_param_kernel(const float *__restrict__ pdy, const float *__restrict__ pdyx,
+                                                                       int batch, int C, GnLevels lv, int total_tiles,
+                                                                       float *__restrict__ dgamma, float *__restrict__ dbeta) {
+    __shared__ float sg[kGnParamLanes][32], sb[kGnParamLanes][32];
+    const int l = blockIdx.y, c = blockIdx.x * 32 + threadIdx.x, u = threadIdx.y;
+    int tile0 = 0, ntiles = 0;
+#pragma unroll
+    for (int v = 0; v < kMaxLevels; ++v)
+        if (v == l) tile0 = lv.tile0[v], ntiles = lv.tile0[v + 1] - lv.tile0[v];
+    float ag = 0.f, ab = 0.f;
+    if (c < C) {
+        const int items = batch * ntiles;
+        for (int k = u; k < items; k += kGnParamLanes) {
+            const int64_t o = ((int64_t)(k / ntiles) * total_tiles + tile0 + k % ntiles) * C + c;
+            ag += __ldg(pdyx + o), ab += __ldg(pdy + o);
+        }
+    }
+    sg[u][threadIdx.x] = ag, sb[u][threadIdx.x] = ab;
+    __syncthreads();
+    if (u != 0 || c >= C) return;
+    for (int v = 1; v < kGnParamLanes; ++v) ag += sg[v][threadIdx.x], ab += sb[v][threadIdx.x];
+    if (dgamma) dgamma[(int64_t)l * C + c] = ag;
+    if (dbeta) dbeta[(int64_t)l * C + c] = ab;
+}
+
+// (4) dx = rstd * (gamma dy - m1 - xhat m2), same tiles and threads as gn_apply_kernel; dx may alias x or dy (each element is
+// read, then written, by the same thread)
+__global__ void gnb_apply_kernel(const float *dy, const float *x, float *dx, int64_t pitch, int C, int G, GnLevels lv,
+                                 const float *__restrict__ gamma, const float2 *__restrict__ stats, const float2 *__restrict__ coef) {
+    const int C4 = C / 4, R = blockDim.x / C4;
+    const int j = threadIdx.x % C4, r = threadIdx.x / C4, c = 4 * j, cg = C / G;
+    const int tile = blockIdx.x, b = blockIdx.y;
+    const int l = gn_level_of_tile(lv, tile);
+    const int t0 = (tile - lv.tile0[l]) * kGnTile;
+    const int rows = min(kGnTile, lv.size[l] - t0);
+    const float4 ga = ldg_f4(gamma + (int64_t)l * C + c);
+    const int64_t sidx = ((int64_t)b * lv.L + l) * G;
+    const float2 s0 = stats[sidx + (c + 0) / cg], s1 = stats[sidx + (c + 1) / cg], s2 = stats[sidx + (c + 2) / cg],
+                 s3 = stats[sidx + (c + 3) / cg];
+    const float2 k0 = coef[sidx + (c + 0) / cg], k1 = coef[sidx + (c + 1) / cg], k2 = coef[sidx + (c + 2) / cg],
+                 k3 = coef[sidx + (c + 3) / cg];
+    const int64_t base = (int64_t)b * pitch + (int64_t)(lv.start[l] + t0) * C + c;
+    for (int t = r; t < rows; t += R) {
+        const int64_t o = base + (int64_t)t * C;
+        const float4 g = *reinterpret_cast<const float4 *>(dy + o), v = *reinterpret_cast<const float4 *>(x + o);
+        float4 d;
+        d.x = s0.y * (fmaf(ga.x, g.x, -k0.x) - (v.x - s0.x) * s0.y * k0.y);
+        d.y = s1.y * (fmaf(ga.y, g.y, -k1.x) - (v.y - s1.x) * s1.y * k1.y);
+        d.z = s2.y * (fmaf(ga.z, g.z, -k2.x) - (v.z - s2.x) * s2.y * k2.y);
+        d.w = s3.y * (fmaf(ga.w, g.w, -k3.x) - (v.w - s3.x) * s3.y * k3.y);
+        *reinterpret_cast<float4 *>(dx + o) = d;
+    }
+}
+
 struct LevelStarts {
     int start[kMaxLevels];
     int L;
@@ -245,6 +383,64 @@ extern "C" int sdetr_group_norm_tokens(const float *x, float *y, int64_t pitch, 
     gn_apply_kernel<<<dim3(tiles, batch), threads, 0, (cudaStream_t)stream>>>(x, y, pitch, channels, num_groups, lv, gamma, beta,
                                                                              stats);
     return check_launch("group_norm_tokens (apply)");
+}
+
+extern "C" int64_t sdetr_group_norm_tokens_backward_workspace_floats(int batch, int channels, int num_groups, int num_levels,
+                                                                     const int32_t *level_size_host) {
+    const int64_t fwd = sdetr_group_norm_tokens_workspace_floats(batch, channels, num_groups, num_levels, level_size_host);
+    return fwd ? fwd + 2LL * batch * num_levels * num_groups : 0;  // + the (m1, m2) table
+}
+
+extern "C" int sdetr_group_norm_tokens_backward(const float *dy, const float *x, float *dx, int64_t pitch, int batch, int channels,
+                                                int num_levels, const int32_t *level_size_host, const float *gamma, int num_groups,
+                                                float eps, float *dgamma, float *dbeta, float *workspace, int64_t workspace_floats,
+                                                sdetr_stream_t stream) {
+    SDETR_REQUIRE(dy && x && dx && level_size_host && gamma && workspace, SDETR_ERR_INVALID_ARG,
+                  "group_norm_tokens_backward: null pointer");
+    SDETR_REQUIRE(batch >= 0 && batch <= 65535 && channels > 0 && num_groups > 0 && num_levels > 0, SDETR_ERR_INVALID_ARG,
+                  "group_norm_tokens_backward: bad sizes");
+    SDETR_REQUIRE(num_levels <= kMaxLevels, SDETR_ERR_UNSUPPORTED, "group_norm_tokens_backward: at most %d levels", kMaxLevels);
+    SDETR_REQUIRE(channels % 4 == 0 && channels <= 4096 && channels % num_groups == 0, SDETR_ERR_UNSUPPORTED,
+                  "group_norm_tokens_backward: channels=%d must be a multiple of 4, at most 4096, and divisible by num_groups=%d",
+                  channels, num_groups);
+    SDETR_REQUIRE(eps >= 0.f, SDETR_ERR_INVALID_ARG, "group_norm_tokens_backward: eps must not be negative");
+    SDETR_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned16(gamma) && pitch % 4 == 0, SDETR_ERR_INVALID_ARG,
+                  "group_norm_tokens_backward: dy, x, dx, gamma and the image pitch must be 16-byte aligned");
+    GnLevels lv;
+    int nv;
+    SDETR_REQUIRE(gn_levels(level_size_host, num_levels, lv, nv), SDETR_ERR_INVALID_ARG, "group_norm_tokens_backward: empty level");
+    SDETR_REQUIRE(pitch >= (int64_t)nv * channels, SDETR_ERR_INVALID_ARG, "group_norm_tokens_backward: image pitch below Nv * C");
+    if (batch == 0) return SDETR_OK;
+    SDETR_REQUIRE(workspace_floats >=
+                      sdetr_group_norm_tokens_backward_workspace_floats(batch, channels, num_groups, num_levels, level_size_host),
+                  SDETR_ERR_WORKSPACE, "group_norm_tokens_backward: workspace too small");
+    const int tiles = lv.tile0[num_levels], threads = gn_threads(channels);
+    // the forward's statistics, recomputed by its own kernels (the same bits); then the partials' space holds the backward's
+    float *p0 = workspace, *p1 = workspace + (int64_t)batch * tiles * channels;
+    float2 *stats = reinterpret_cast<float2 *>(p1 + (int64_t)batch * tiles * channels);
+    float2 *coef = stats + (int64_t)batch * num_levels * num_groups;
+    SDETR_REQUIRE((reinterpret_cast<uintptr_t>(stats) & 7) == 0, SDETR_ERR_INVALID_ARG,
+                  "group_norm_tokens_backward: workspace misaligned");
+    const size_t smem = 2 * sizeof(float) * (size_t)threads * 4;
+    cudaStream_t s = (cudaStream_t)stream;
+    gn_partial_kernel<<<dim3(tiles, batch), threads, smem, s>>>(x, pitch, channels, lv, tiles, p0, p1);
+    int rc = check_launch("group_norm_tokens_backward (statistics partials)");
+    if (rc) return rc;
+    gn_combine_kernel<<<dim3(num_groups, num_levels, batch), kGnCombineThreads, 0, s>>>(p0, p1, channels, num_groups, lv, tiles, eps,
+                                                                                       stats);
+    if ((rc = check_launch("group_norm_tokens_backward (statistics combine)"))) return rc;
+    gnb_partial_kernel<<<dim3(tiles, batch), threads, smem, s>>>(dy, x, pitch, channels, num_groups, lv, tiles, stats, p0, p1);
+    if ((rc = check_launch("group_norm_tokens_backward (partials)"))) return rc;
+    gnb_combine_kernel<<<dim3(num_groups, num_levels, batch), kGnCombineThreads, 0, s>>>(p0, p1, gamma, channels, num_groups, lv,
+                                                                                        tiles, coef);
+    if ((rc = check_launch("group_norm_tokens_backward (combine)"))) return rc;
+    if (dgamma || dbeta) {
+        gnb_param_kernel<<<dim3((channels + 31) / 32, num_levels), dim3(32, kGnParamLanes), 0, s>>>(p0, p1, batch, channels, lv, tiles,
+                                                                                                   dgamma, dbeta);
+        if ((rc = check_launch("group_norm_tokens_backward (dgamma, dbeta)"))) return rc;
+    }
+    gnb_apply_kernel<<<dim3(tiles, batch), threads, 0, s>>>(dy, x, dx, pitch, channels, num_groups, lv, gamma, stats, coef);
+    return check_launch("group_norm_tokens_backward (dx)");
 }
 
 extern "C" int sdetr_token_lpos_keep(const float *feat, const float *pos, const float *level_embeds, const float *keep,
